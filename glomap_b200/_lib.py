@@ -129,11 +129,28 @@ PROTOTYPES = {
     "b200sfm_ra_solve_gravity": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int64] + [c_void_p] * 5 + [c_int32, c_void_p, P(RAStats)]),
 }
 
+
+class BAStepProbeOut(ct.Structure):
+    """b200sfm_test_ba_step_out (include/b200sfm_testing.h)."""
+    _fields_ = [(f, c_void_p) for f in ("U", "g_c", "jscale_c", "V", "g_p", "jscale_p", "Dc", "Minv", "b", "px",
+                                        "cand_points", "cand_quat", "cand_trans", "cand_intr", "cand_sensor_quat",
+                                        "cand_sensor_trans")] + \
+              [(f, c_double) for f in ("cost", "gmax", "model_cost_change", "cand_cost", "step_norm", "x_norm")] + \
+              [(f, c_int32) for f in ("pcg_iterations", "use_v2", "use_ell", "kfast", "nk", "ext", "ext_k", "ext_s",
+                                      "schur_jacobi", "nbk")]
+
+
+# name -> (restype, argtypes); the test-only probe of include/b200sfm_testing.h (not part of the drop-in ABI)
+TEST_PROTOTYPES = {
+    "b200sfm_test_ba_step": (c_int32, [c_void_p, P(BAOpts), c_double, c_double, P(BAStepProbeOut)]),
+    "b200sfm_test_ba_apply": (c_int32, [c_void_p, c_void_p, c_void_p]),
+}
+
 _lib = None
 
 
 def load() -> ct.CDLL:
-    """Load libb200sfm.so and bind every prototype.  Raises if missing."""
+    """Load libb200sfm.so and bind every prototype (the test probe's included).  Raises if missing."""
     global _lib
     if _lib is not None:
         return _lib
@@ -146,6 +163,12 @@ def load() -> ct.CDLL:
         fn = getattr(lib, name)      # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args
+    # the probe is bound where it is exported (libb200sfm.so always exports it; the host-side mock library does not)
+    for name, (res, args) in TEST_PROTOTYPES.items():
+        if hasattr(lib, name):
+            fn = getattr(lib, name)
+            fn.restype = res
+            fn.argtypes = args
     _lib = lib
     return lib
 

@@ -484,6 +484,33 @@ int b200sfm_ba_problem_filter_triangulation_angle(b200sfm_ba_problem* p, double 
   });
 }
 
+// ---- test probe (include/b200sfm_testing.h) ----------------------------------------------------------------------
+int b200sfm_test_ba_step(b200sfm_ba_problem* p, const b200sfm_ba_opts* opts, double first_radius, double radius,
+                         b200sfm_test_ba_step_out* out) {
+  if (!p || !opts || !out || !(radius > 0.0) || first_radius < 0.0) return B200SFM_ERR_INVALID_ARG;
+  if (p->ctx->world > 1) { p->ctx->err = "the test probe is single-rank only"; return B200SFM_ERR_INVALID_ARG; }
+  return guarded(p->ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(p->ctx->device));
+    if (opts->min_num_view_per_track != p->min_views) {
+      p->ctx->err = "min_num_view_per_track differs from the value the problem was created with";
+      return (int)B200SFM_ERR_INVALID_ARG;
+    }
+    p->test_step(*opts, first_radius, radius, out);
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_ba_apply(b200sfm_ba_problem* p, const double* x, double* y) {
+  if (!p || !x || !y) return B200SFM_ERR_INVALID_ARG;
+  if (p->ctx->world > 1) { p->ctx->err = "the test probe is single-rank only"; return B200SFM_ERR_INVALID_ARG; }
+  if (!p->probe_ready) { p->ctx->err = "b200sfm_test_ba_apply needs a preceding b200sfm_test_ba_step"; return B200SFM_ERR_INVALID_ARG; }
+  return guarded(p->ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(p->ctx->device));
+    p->test_apply(x, y);
+    return (int)B200SFM_OK;
+  });
+}
+
 void b200sfm_ba_problem_free(b200sfm_ba_problem* p) {
   if (!p) return;
   cudaSetDevice(p->ctx->device);

@@ -946,12 +946,14 @@ __global__ void __launch_bounds__(256) ba_cost(BAView v, const double* __restric
 // ---------------------------------------------------------------------------
 // camera update: q_new = exp(d_rot) (x) q (EigenQuaternionManifold), t_new = t + d_t
 //   cscal[0] += gc.dc, cscal[1] += dc.rho (PCG residual), cscal[2] += sum Dc dc^2,
-//   cscal[3] += |x_new - x|^2 (ambient), cscal[4] += |x|^2 (ambient, variable blocks)
+//   cscal[3] += |x_new - x|^2 (ambient), cscal[4] += |x|^2 (ambient, over the parameter blocks of the problem: observed
+//   by a kept observation and not held constant, whatever their curvature -- Ceres' x_norm over the reduced program)
 // ---------------------------------------------------------------------------
 __global__ void ba_update_cams(int C, const double* __restrict__ quat, const double* __restrict__ trans,
                                const double* __restrict__ dc, const double* __restrict__ gc,
                                const double* __restrict__ resid, const double* __restrict__ Dc,
-                               const double* __restrict__ jscale_c, double* __restrict__ quat_new,
+                               const double* __restrict__ jscale_c, const double* __restrict__ blk_used,
+                               const unsigned char* __restrict__ cam_mask, double* __restrict__ quat_new,
                                double* __restrict__ trans_new, double* __restrict__ cscal) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   double a0 = 0, a1 = 0, a2 = 0, a3 = 0, a4 = 0;
@@ -967,8 +969,8 @@ __global__ void ba_update_cams(int C, const double* __restrict__ quat, const dou
       a2 += Dc[i] * d[k] * d[k];
     }
     const double q[4] = {quat[4 * c], quat[4 * c + 1], quat[4 * c + 2], quat[4 * c + 3]};
-    const bool rvar = jscale_c[(size_t)c * 6] >= 0.0 || jscale_c[(size_t)c * 6 + 1] >= 0.0 || jscale_c[(size_t)c * 6 + 2] >= 0.0;
-    const bool tvar = jscale_c[(size_t)c * 6 + 3] >= 0.0 || jscale_c[(size_t)c * 6 + 4] >= 0.0 || jscale_c[(size_t)c * 6 + 5] >= 0.0;
+    const bool used = blk_used[c] > 0.0;
+    const bool rvar = used && !(cam_mask[c] & 1), tvar = used && !(cam_mask[c] & 2);
     const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
     double qn[4] = {q[0], q[1], q[2], q[3]};
     if (nrm > 0.0) {

@@ -416,13 +416,14 @@ __global__ void __launch_bounds__(128) bax_pass_b(BAView v, ExtView ex, BAViewV2
 
 // ---- trial step of the extra blocks -----------------------------------------------------------------------------------
 //   intrinsics: params[pidx[j]] += d[j];  sensors: q <- exp(d_rot) (x) q (EigenQuaternionManifold), t += d_t
-//   cscal as ba_update_cams: [0] g.d  [1] d.resid  [2] sum D d^2  [3] |x_new - x|^2  [4] |x|^2 over variable blocks
+//   cscal as ba_update_cams: [0] g.d  [1] d.resid  [2] sum D d^2  [3] |x_new - x|^2  [4] |x|^2 over the blocks of the problem
 __global__ void bax_update_extras(ExtView ex, const IntrVarRec* __restrict__ ivar, const int* __restrict__ intr_model,
                                   const double* __restrict__ intr, double* __restrict__ intr_new,
                                   const double* __restrict__ sq, const double* __restrict__ st, double* __restrict__ sq_new,
                                   double* __restrict__ st_new, const double* __restrict__ dc, const double* __restrict__ gc,
                                   const double* __restrict__ resid, const double* __restrict__ Dc,
-                                  const double* __restrict__ jscale_c, int count_norms, double* __restrict__ cscal) {
+                                  const double* __restrict__ jscale_c, const double* __restrict__ blk_used, int count_norms,
+                                  double* __restrict__ cscal) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   double a0 = 0, a1 = 0, a2 = 0, a3 = 0, a4 = 0;
   if (i < ex.K) {
@@ -431,11 +432,9 @@ __global__ void bax_update_extras(ExtView ex, const IntrVarRec* __restrict__ iva
     double p[12];
 #pragma unroll
     for (int j = 0; j < 12; ++j) p[j] = intr[(size_t)i * 12 + j];
-    bool any = false;
     for (int j = 0; j < iv.mb; ++j) {
       const size_t k = blk * 6 + j;
       if (!(jscale_c[k] >= 0.0)) continue;
-      any = true;
       const double d = dc[k];
       a0 += gc[k] * d;
       a1 += resid[k] * d;
@@ -443,7 +442,7 @@ __global__ void bax_update_extras(ExtView ex, const IntrVarRec* __restrict__ iva
       a3 += d * d;
       p[iv.pidx[j]] += d;
     }
-    if (any) {
+    if (iv.mb > 0 && blk_used[blk] > 0.0) {   // x norm: every block of the problem, whatever its curvature
       const int npar = intr_model[i] == 0 ? 3 : (intr_model[i] == 3 ? 5 : 4);
       for (int j = 0; j < npar; ++j) a4 += intr[(size_t)i * 12 + j] * intr[(size_t)i * 12 + j];
     }
@@ -466,6 +465,8 @@ __global__ void bax_update_extras(ExtView ex, const IntrVarRec* __restrict__ iva
         if (k < 3) rvar = true; else tvar = true;
       }
     }
+    // x norm: the sensor is a parameter block of the problem when it is an unknown and observed
+    const bool in_problem = ex.sensor_var && ex.sensor_var[s] && blk_used[blk] > 0.0;
     const double q[4] = {sq[4 * s], sq[4 * s + 1], sq[4 * s + 2], sq[4 * s + 3]};
     double qn[4] = {q[0], q[1], q[2], q[3]};
     const double nrm = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
@@ -483,13 +484,15 @@ __global__ void bax_update_extras(ExtView ex, const IntrVarRec* __restrict__ iva
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       sq_new[4 * s + k] = qn[k];
-      if (rvar) { a3 += (qn[k] - q[k]) * (qn[k] - q[k]); a4 += q[k] * q[k]; }
+      if (rvar) a3 += (qn[k] - q[k]) * (qn[k] - q[k]);
+      if (in_problem) a4 += q[k] * q[k];
     }
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       const double t = st[3 * s + k];
       st_new[3 * s + k] = t + d[3 + k];
-      if (tvar) { a3 += d[3 + k] * d[3 + k]; a4 += t * t; }
+      if (tvar) a3 += d[3 + k] * d[3 + k];
+      if (in_problem) a4 += t * t;
     }
   }
   if (!count_norms) { a3 = 0; a4 = 0; }

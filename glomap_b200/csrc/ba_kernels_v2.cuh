@@ -743,7 +743,9 @@ __global__ void __launch_bounds__(256) ba2k_cross(int C, int K, const double* __
         yf += uik * xk[k];
         tk[k] += uik * xf[i];
       }
-      if (yf != 0.0) y[(size_t)c * 6 + i] += yf;   // this thread owns y_f of its image (pass B has finished: stream order)
+      // plain read-modify-write: this thread owns y_f of its image, and pass B, which adds to y_f with atomics, is
+      // launched after this kernel on the same stream
+      if (yf != 0.0) y[(size_t)c * 6 + i] += yf;
     }
 #pragma unroll
     for (int k = 0; k < NK; ++k) {

@@ -11,6 +11,7 @@
 #include <cstdlib>
 #include <vector>
 
+#include "../../include/b200sfm_testing.h"
 #include "ba_kernels.cuh"
 #include "ba_kernels_v2.cuh"
 #include "ba_kernels_v3.cuh"
@@ -89,6 +90,18 @@ __global__ void k_gather_int(int n, const int* __restrict__ idx, const int* __re
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = src[idx[i]];
 }
+// blk_used[b] = 1: block b (frame f | C + intrinsics k | C + K + sensor s) has an observation of a kept track, i.e. it
+// is a parameter block of the problem whatever its curvature (plain stores of the same value: the races are benign)
+__global__ void k_block_used(int VC, int smul, int C, int K, const int* __restrict__ cam_count,
+                             const int* __restrict__ cam_intr, const int* __restrict__ sensor_intr,
+                             double* __restrict__ blk_used) {
+  const int vc = blockIdx.x * blockDim.x + threadIdx.x;
+  if (vc >= VC || cam_count[vc] == 0) return;
+  const int f = vc / smul, s = vc - f * smul;
+  blk_used[f] = 1.0;
+  blk_used[C + (sensor_intr ? sensor_intr[s] : cam_intr[f])] = 1.0;
+  if (sensor_intr) blk_used[C + K + s] = 1.0;
+}
 __global__ void k_eff_mask(int C, const unsigned char* __restrict__ base, int fix_rot, int fix_trn,
                            unsigned char* __restrict__ out) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -136,6 +149,7 @@ struct b200sfm_ba_problem {
   DevBuf<int4> tile_desc;
   DevBuf<unsigned> pt_begin;
   DevBuf<unsigned char> cam_mask_base, cam_mask;
+  DevBuf<double> blk_used;   // [CB] > 0: the block is a parameter block of the problem (k_block_used; summed over the ranks)
   // state + candidate + snapshot
   DevBuf<double> quat[2], trans[2], points[2], intr, intr_cand, quat_saved, trans_saved, points_saved, intr_saved;
   // extended path (ba_kernels_ext.cuh): intrinsics blocks and unknown cam_from_rig poses as pseudo-camera blocks
@@ -326,6 +340,11 @@ struct b200sfm_ba_problem {
     tb = tmp.bytes();
     cub::DeviceScan::ExclusiveSum(tmp.p, tb, cam_count.p, cam_begin.p, VC + 1, s);
     B200_LAUNCH(ctx, k_seg_counts, cdiv(VC, 256), 256, 0, VC, cam_count.p, seg_count.p);
+    blk_used.alloc(CB);
+    blk_used.zero(s);
+    B200_LAUNCH(ctx, k_block_used, cdiv(VC, 256), 256, 0, VC, smul, C, K, cam_count.p, cam_intr.p,
+                S > 0 ? sensor_intr.p : nullptr, blk_used.p);
+    ctx->allreduce_sum(blk_used.p, CB);   // a block observed on any rank is a block of the problem on every rank
     tb = tmp.bytes();
     cub::DeviceScan::ExclusiveSum(tmp.p, tb, seg_count.p, seg_off.p, VC + 1, s);
     ctx->launches += 4;
@@ -776,6 +795,64 @@ struct b200sfm_ba_problem {
     else B200_LAUNCH(ctx, ba2k_cross<1>, cdiv(C, 256), 256, 0, C, K, cam_rec.p, Ufk.p, x, y, ctl);
   }
 
+  // Schur-Jacobi blocks need the stored A_o rows of the fast path; the extended path preconditions with block-Jacobi
+  bool matrix_free() const { return ext && !kfast; }   // matrix-free extended mat-vec (ba_kernels_ext.cuh); kfast: stored rows
+  bool schur_jacobi_on(const b200sfm_ba_opts& o, bool points_var) const {
+    return points_var && o.preconditioner == 1 && !matrix_free();   // kfast: frames Schur-Jacobi, intrinsics block-Jacobi
+  }
+
+  // Observation passes of one mat-vec of the reduced camera system S + D, then the all-reduce of y over the ranks.
+  // They leave in y what pcg_apply_diag does not add: everything but the blocks U + D (the matrix-free extended
+  // path: everything but D).  y must be zero on entry.  The v2 point pass reads x through its packed copy xq (filled by ba2_pcg_direction_pack, or by
+  // ba2_pack_x + ba2k_pack_xk), the other kernels read x itself.
+  void matvec(const double* x, double* y, const b200sfm_ba_opts& o, double radius, bool points_var, bool split_ar,
+              bool profile, const b200::PcgCtl* ctl) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    BAView v = view();
+    const int nB6 = nbk * 6;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (profile) {
+      e0 = timer_mv.next();
+      e1 = timer_mv.next();
+      B200_CUDA_OK(cudaEventRecord(e0, s));
+    }
+    if (matrix_free()) {
+      ext_matvec(x, y, o.thres_loss_function, radius, points_var, ctl);
+    } else if (kfast && !points_var) {
+      // constant points: no Schur term; U x = block diagonal (apply_diag) + the frame x intrinsics coupling
+      launch_cross(x, y, ctl);
+    } else if (use_v2) {
+      if (use_ell)
+        launch_pass_a0(v, radius, ctl);
+      else
+        B200_LAUNCH(ctx, ba2_pass_a<0>, n_tiles, kTile, smem_k3v2, v, view2(), xq.p, points[cur].p, nullptr, radius, nullptr, ctl);
+      if (kfast) launch_cross(x, y, ctl);   // before pass B: its y_f updates are plain stores of the owning thread
+      if (split_ar) {
+        // cameras below C/2 are complete after the first half of the (camera-sorted) segments: their all-reduce
+        // runs on the second stream while pass B works through the upper half
+        launch_pass_b(v, y, ctl, 0, seg_mid);
+        B200_CUDA_OK(cudaEventRecord(ctx->ev_half, s));
+        B200_CUDA_OK(cudaStreamWaitEvent(ctx->comm_stream, ctx->ev_half, 0));
+        ctx->allreduce_sum_on(ctx->comm_stream, y, (size_t)(C / 2) * 6);
+        B200_CUDA_OK(cudaEventRecord(ctx->ev_comm, ctx->comm_stream));
+        launch_pass_b(v, y, ctl, seg_mid, n_segs);
+      } else if (n_segs > 0) {
+        launch_pass_b(v, y, ctl);
+      }
+    } else {
+      B200_LAUNCH(ctx, ba_schur_pass<0>, n_tiles, kTile, smem_k3, v, x, y, nullptr, nullptr, radius, nullptr, nullptr,
+                  nullptr, 0, ctl);
+    }
+    if (profile) B200_CUDA_OK(cudaEventRecord(e1, s));
+    if (split_ar) {
+      ctx->allreduce_sum(y + (size_t)(C / 2) * 6, nB6 - (size_t)(C / 2) * 6);   // upper half + pseudo-camera blocks
+      B200_CUDA_OK(cudaStreamWaitEvent(s, ctx->ev_comm, 0));
+    } else {
+      ctx->allreduce_sum(y, nB6);
+    }
+  }
+
   // One trust-region step at the current linearisation: damping, preconditioner,
   // PCG on the reduced camera system, back-substitution, candidate + its cost.
   StepResult compute_step(const b200sfm_ba_opts& o, double radius, bool points_var, bool set_jscale_p, bool profile) {
@@ -785,9 +862,8 @@ struct b200sfm_ba_problem {
     const int nB6 = nbk * 6;
     if (points_var) B200_LAUNCH(ctx, ba_damp_points, cdiv(P, 256), 256, 0, P, V.p, jscale_p.p, set_jscale_p ? 1 : 0, radius, Vinv.p);
     B200_LAUNCH(ctx, ba_damp_cams, cdiv(nB6, 256), 256, 0, nbk, U(), jscale_c.p, radius, Dc.p);
-    // Schur-Jacobi blocks need the stored A_o rows of the fast path; the extended path preconditions with block-Jacobi
-    const bool recomp = ext && !kfast;   // matrix-free extended mat-vec (ba_kernels_ext.cuh); kfast: stored rows
-    const bool schur_jacobi = points_var && o.preconditioner == 1 && !recomp;   // kfast: frames Schur-Jacobi, intrinsics block-Jacobi
+    const bool recomp = matrix_free();
+    const bool schur_jacobi = schur_jacobi_on(o, points_var);
     double* yrhs = Sd.p + (size_t)CB * 21;   // W Vinv g_p accumulates next to Sd so that both share one all-reduce
     Sd.zero(s);
     if (schur_jacobi && n_segs > 0) {
@@ -842,48 +918,7 @@ struct b200sfm_ba_problem {
           else
             B200_LAUNCH(ctx, pcg_direction<6>, nblk, kPcgThreads, 0, nbk, nblk, it, o.pcg_min_iterations, o.pcg_rel_tolerance, pz.p,
                         pp.p, yw.p, d_pp, part_rz, part_rr, nullptr, d_pub, ctl);
-          if (has_mv) {
-            cudaEvent_t e0 = nullptr, e1 = nullptr;
-            if (profile) {
-              e0 = timer_mv.next();
-              e1 = timer_mv.next();
-              B200_CUDA_OK(cudaEventRecord(e0, s));
-            }
-            if (recomp) {
-              ext_matvec(pp.p, yw.p, o.thres_loss_function, radius, points_var, ctl);
-            } else if (kfast && !points_var) {
-              // constant points: no Schur term; U x = block diagonal (apply_diag) + the frame x intrinsics coupling
-              launch_cross(pp.p, yw.p, ctl);
-            } else if (use_v2) {
-              if (use_ell)
-                launch_pass_a0(v, radius, ctl);
-              else
-                B200_LAUNCH(ctx, ba2_pass_a<0>, n_tiles, kTile, smem_k3v2, v, view2(), xq.p, points[cur].p, nullptr, radius, nullptr, ctl);
-              if (kfast) launch_cross(pp.p, yw.p, ctl);   // before pass B: its y_f updates are plain stores of the owning thread
-              if (split_ar) {
-                // cameras below C/2 are complete after the first half of the (camera-sorted) segments: their all-reduce
-                // runs on the second stream while pass B works through the upper half
-                launch_pass_b(v, yw.p, ctl, 0, seg_mid);
-                B200_CUDA_OK(cudaEventRecord(ctx->ev_half, s));
-                B200_CUDA_OK(cudaStreamWaitEvent(ctx->comm_stream, ctx->ev_half, 0));
-                ctx->allreduce_sum_on(ctx->comm_stream, yw.p, (size_t)(C / 2) * 6);
-                B200_CUDA_OK(cudaEventRecord(ctx->ev_comm, ctx->comm_stream));
-                launch_pass_b(v, yw.p, ctl, seg_mid, n_segs);
-              } else if (n_segs > 0) {
-                launch_pass_b(v, yw.p, ctl);
-              }
-            } else {
-              B200_LAUNCH(ctx, ba_schur_pass<0>, n_tiles, kTile, smem_k3, v, pp.p, yw.p, nullptr, nullptr, radius, nullptr, nullptr,
-                          nullptr, 0, ctl);
-            }
-            if (profile) B200_CUDA_OK(cudaEventRecord(e1, s));
-            if (split_ar) {
-              ctx->allreduce_sum(yw.p + (size_t)(C / 2) * 6, nB6 - (size_t)(C / 2) * 6);   // upper half + pseudo-camera blocks
-              B200_CUDA_OK(cudaStreamWaitEvent(s, ctx->ev_comm, 0));
-            } else {
-              ctx->allreduce_sum(yw.p, nB6);
-            }
-          }
+          if (has_mv) matvec(pp.p, yw.p, o, radius, points_var, split_ar, profile, ctl);
           // extended path: J^T J is inside yw already, only the damping is added here
           B200_LAUNCH(ctx, pcg_apply_diag<6>, nblk, kPcgThreads, 0, nbk, recomp ? nullptr : U(), Dc.p, pp.p, has_mv ? yw.p : nullptr, pq.p,
                       part_pq, ctl);
@@ -901,7 +936,7 @@ struct b200sfm_ba_problem {
     if (ext) {
       B200_LAUNCH(ctx, bax_update_extras, cdiv(std::max(K + S, 1), 128), 128, 0, ext_view(), ivar.p, intr_model.p, intr.p, intr_cand.p,
                   S > 0 ? sens_q[cur].p : nullptr, S > 0 ? sens_t[cur].p : nullptr, S > 0 ? sens_q[nxt].p : nullptr,
-                  S > 0 ? sens_t[nxt].p : nullptr, px.p, gc(), pr.p, Dc.p, jscale_c.p, 1, scal.p + 8);
+                  S > 0 ? sens_t[nxt].p : nullptr, px.p, gc(), pr.p, Dc.p, jscale_c.p, blk_used.p, 1, scal.p + 8);
     } else {
       B200_CUDA_OK(cudaMemcpyAsync(intr_cand.p, intr.p, intr.bytes(), cudaMemcpyDeviceToDevice, s));
       if (S > 0) {   // the cam_from_rig poses follow `cur` like the frame poses: the candidate buffer mirrors them
@@ -946,7 +981,7 @@ struct b200sfm_ba_problem {
       B200_CUDA_OK(cudaMemcpyAsync(points[nxt].p, points[cur].p, points[cur].bytes(), cudaMemcpyDeviceToDevice, s));
     }
     B200_LAUNCH(ctx, ba_update_cams, cdiv(C, 128), 128, 0, C, quat[cur].p, trans[cur].p, px.p, gc(), pr.p, Dc.p, jscale_c.p,
-                quat[nxt].p, trans[nxt].p, scal.p + 8);
+                blk_used.p, cam_mask.p, quat[nxt].p, trans[nxt].p, scal.p + 8);
     build_records(nxt);
     launch_cost(nxt, o.thres_loss_function);
     // bscal[0..3] + cand cost are per-shard partial sums; cscal[8..12] is replicated but summed
@@ -967,11 +1002,11 @@ struct b200sfm_ba_problem {
     return res;
   }
 
-  // The LM loop, Ceres order of checks (see oracle/ceres_lm.py).
-  int solve(const b200sfm_ba_opts& o, b200sfm_lm_stats* st) {
+  // Which parameter blocks beyond the frame poses are unknowns of a solve with options `o`, and which kernel
+  // paths it takes (v1 / v2 tile / ELL, stored-row intrinsics, matrix-free extended); sizes their buffers.
+  void select_paths(const b200sfm_ba_opts& o) {
     using namespace b200;
     cudaStream_t s = ctx->stream;
-    // ---- which parameter blocks beyond the frame poses are unknowns of this solve ------------------------------
     // intrinsics (bundle_adjustment.cc:273-293): optimize_principal_point -> no manifold is set at all, EVERY parameter
     // of every camera is variable; else optimize_intrinsics -> SubsetManifold holding the principal point; else constant
     {
@@ -1018,6 +1053,22 @@ struct b200sfm_ba_problem {
       if (Bc.n < crow) Bc.alloc(crow);
       if (Ufk.n < (size_t)C * 6 * nk) Ufk.alloc((size_t)C * 6 * nk);
     }
+  }
+  // effective per-camera mask: the caller's mask | optimize_rotations / optimize_translation off
+  void launch_eff_mask(const b200sfm_ba_opts& o) {
+    B200_LAUNCH(ctx, b200::k_eff_mask, b200::cdiv(C, 256), 256, 0, C, cam_mask_base.p, o.optimize_rotations ? 0 : 1,
+                o.optimize_translation ? 0 : 1, cam_mask.p);
+  }
+
+  // A step that is not accepted: compute_step ended by building the records of the candidate (for its cost); the next
+  // step works on the same linearisation, whose stored rows and Jacobians belong to the current state's records.
+  void reject_step() { build_records(cur); }
+
+  // The LM loop, Ceres order of checks (see oracle/ceres_lm.py).
+  int solve(const b200sfm_ba_opts& o, b200sfm_lm_stats* st) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    select_paths(o);
     // v2: keep z4 (written by pass A, gathered by pass B) in the persisting part of L2 when it fits there
     const bool l2_persist = use_v2 && !(getenv("B200SFM_L2_PERSIST") && atoi(getenv("B200SFM_L2_PERSIST")) == 0) &&
                             l2_persist_window(s, ctx->device, z4.p, z4.bytes());
@@ -1030,8 +1081,7 @@ struct b200sfm_ba_problem {
     B200_CUDA_OK(cudaEventRecord(ev0, s));
     const bool points_var = o.optimize_points != 0;
     const bool profile = o.profile_kernels != 0;
-    B200_LAUNCH(ctx, k_eff_mask, cdiv(C, 256), 256, 0, C, cam_mask_base.p, o.optimize_rotations ? 0 : 1,
-                o.optimize_translation ? 0 : 1, cam_mask.p);
+    launch_eff_mask(o);
     double cost = 0, gmax = 0;
     linearize(o.thres_loss_function, points_var, true, profile, cost, gmax);
     b200sfm_lm_stats local{};
@@ -1053,6 +1103,7 @@ struct b200sfm_ba_problem {
       local.pcg_iterations += r.pcg_iters;
       if (!r.finite || !(r.model_cost_change > 0.0)) {
         if (++invalid >= 5) { term = B200SFM_TERM_INVALID_STEPS; local.usable = 0; break; }
+        reject_step();
         radius /= decrease;
         decrease *= 2;
         continue;
@@ -1072,6 +1123,7 @@ struct b200sfm_ba_problem {
         decrease = 2.0;
         if (!fixed && gmax <= o.gradient_tolerance) { term = B200SFM_TERM_GRADIENT_TOLERANCE; break; }
       } else {
+        reject_step();
         radius /= decrease;
         decrease *= 2;
       }
@@ -1106,5 +1158,83 @@ struct b200sfm_ba_problem {
       *st = local;
     }
     return B200SFM_OK;
+  }
+
+  // ---- test probe (include/b200sfm_testing.h) ----------------------------------------------------------------------
+  b200sfm_ba_opts probe_opts{};
+  double probe_radius = 0;
+  bool probe_ready = false;
+
+  // the first LM iteration of solve() up to the candidate and its cost, without accepting it; with first_radius > 0 the
+  // step at `radius` is the second one, after a step at first_radius that was not accepted (same linearisation)
+  void test_step(const b200sfm_ba_opts& o, double first_radius, double radius, b200sfm_test_ba_step_out* out) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    select_paths(o);
+    launch_eff_mask(o);
+    const bool points_var = o.optimize_points != 0;
+    double cost = 0, gmax = 0;
+    linearize(o.thres_loss_function, points_var, true, false, cost, gmax);
+    if (first_radius > 0.0) {
+      compute_step(o, first_radius, points_var, true, false);
+      reject_step();
+    }
+    const StepResult r = compute_step(o, radius, points_var, !(first_radius > 0.0), false);
+    reject_step();
+    probe_opts = o;
+    probe_radius = radius;
+    probe_ready = true;
+    const int nxt = cur ^ 1;
+    const size_t nb6 = (size_t)nbk * 6;
+    if (out->U) B200_CUDA_OK(cudaMemcpyAsync(out->U, U(), (size_t)nbk * 21 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (out->g_c) B200_CUDA_OK(cudaMemcpyAsync(out->g_c, gc(), nb6 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (out->jscale_c) jscale_c.download(out->jscale_c, nb6, s);
+    if (out->V) V.download(out->V, (size_t)P * 6, s);
+    if (out->g_p) gp.download(out->g_p, (size_t)P * 3, s);
+    if (out->jscale_p) jscale_p.download(out->jscale_p, (size_t)P * 3, s);
+    if (out->Dc) Dc.download(out->Dc, nb6, s);
+    if (out->Minv) Minv.download(out->Minv, (size_t)nbk * 21, s);
+    if (out->b) bvec.download(out->b, nb6, s);
+    if (out->px) px.download(out->px, nb6, s);
+    if (out->cand_points) points[nxt].download(out->cand_points, (size_t)P * 3, s);
+    if (out->cand_quat) quat[nxt].download(out->cand_quat, (size_t)C * 4, s);
+    if (out->cand_trans) trans[nxt].download(out->cand_trans, (size_t)C * 3, s);
+    if (out->cand_intr) intr_cand.download(out->cand_intr, (size_t)K * B200SFM_INTR_STRIDE, s);
+    if (S > 0 && out->cand_sensor_quat) sens_q[nxt].download(out->cand_sensor_quat, (size_t)S * 4, s);
+    if (S > 0 && out->cand_sensor_trans) sens_t[nxt].download(out->cand_sensor_trans, (size_t)S * 3, s);
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    out->cost = cost;
+    out->gmax = gmax;
+    out->model_cost_change = r.model_cost_change;
+    out->cand_cost = r.cand_cost;
+    out->step_norm = r.step_norm;
+    out->x_norm = r.x_norm;
+    out->pcg_iterations = r.pcg_iters;
+    out->use_v2 = use_v2; out->use_ell = use_ell; out->kfast = kfast; out->nk = nk;
+    out->ext = ext; out->ext_k = ext_k; out->ext_s = ext_s;
+    out->schur_jacobi = schur_jacobi_on(o, points_var);
+    out->nbk = nbk;
+  }
+
+  // y = (S + D) x at the linearisation and damping of the last test_step, through the mat-vec chain of a PCG iteration
+  void test_apply(const double* h_x, double* h_y) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    const bool points_var = probe_opts.optimize_points != 0;
+    const int nblk = cdiv(nbk, kPcgThreads);
+    PcgCtl* ctl = ctx->pcgh.d_ctl;
+    B200_CUDA_OK(cudaMemsetAsync(ctl, 0, sizeof(PcgCtl), s));   // every kernel of the chain returns early once ctl->done is set
+    pp.upload(h_x, (size_t)nbk * 6, s);
+    yw.zero(s);
+    if (points_var && use_v2 && !matrix_free()) {   // what ba2_pcg_direction_pack does inside PCG
+      B200_LAUNCH(ctx, ba2_pack_x, cdiv(C, 256), 256, 0, C, pp.p, cam_rec.p, xq.p);
+      if (kfast) B200_LAUNCH(ctx, ba2k_pack_xk, cdiv(C, 256), 256, 0, C, cam_rec.p, pp.p, xq.p, ctl);
+    }
+    const bool has_mv = points_var || ext;
+    if (has_mv) matvec(pp.p, yw.p, probe_opts, probe_radius, points_var, false, false, ctl);
+    B200_LAUNCH(ctx, pcg_apply_diag<6>, nblk, kPcgThreads, 0, nbk, matrix_free() ? nullptr : U(), Dc.p, pp.p,
+                has_mv ? yw.p : nullptr, pq.p, ctx->pcgh.d_part, ctl);
+    pq.download(h_y, (size_t)nbk * 6, s);
+    B200_CUDA_OK(cudaStreamSynchronize(s));
   }
 };

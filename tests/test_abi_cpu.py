@@ -109,3 +109,46 @@ def test_null_arguments_are_rejected_without_touching_the_device():
     assert lib.b200sfm_last_error(None) == b"null context" or lib.b200sfm_last_error(None) is not None
     lib.b200sfm_ba_problem_free(None); lib.b200sfm_gp_problem_free(None); lib.b200sfm_destroy(None)   # no-ops
     assert lib.b200sfm_rank(None) == -1 and lib.b200sfm_world_size(None) == -1 and lib.b200sfm_kernel_launches(None) == 0
+
+
+# ---- the test-only probe (include/b200sfm_testing.h): exported, mirrored, plain C, validated before any CUDA call ----
+def testing_symbols():
+    src = open(os.path.join(ROOT, "include", "b200sfm_testing.h")).read()
+    src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
+    return sorted(set(re.findall(r"\b(b200sfm_test_[a-z0-9_]+)\s*\(", src)))
+
+
+def test_testing_header_symbols_are_exported_and_mirrored():
+    lib = _lib.load()
+    syms = testing_symbols()
+    assert syms == sorted(_lib.TEST_PROTOTYPES), syms
+    for s in syms:
+        assert hasattr(lib, s), f"{s} declared in include/b200sfm_testing.h but not exported"
+    assert not set(syms) & set(declared_symbols())      # not part of the drop-in ABI
+
+
+def test_testing_header_is_plain_c99_and_its_struct_matches_ctypes(tmp_path):
+    import subprocess
+    fields = [f for f, _ in _lib.BAStepProbeOut._fields_]
+    lines = ["#include <stdio.h>", "#include <stddef.h>", '#include "b200sfm_testing.h"', "int main(void) {",
+             '  printf("size %zu\\n", sizeof(b200sfm_test_ba_step_out));']
+    lines += [f'  printf("{f} %zu\\n", offsetof(b200sfm_test_ba_step_out, {f}));' for f in fields]
+    lines += ["  return 0;", "}"]
+    src = tmp_path / "probe.c"
+    src.write_text("\n".join(lines))
+    exe = tmp_path / "probe"
+    subprocess.check_call(["/usr/bin/gcc", "-std=c99", "-Wall", "-Wextra", "-pedantic", "-Werror",
+                           "-I" + os.path.join(ROOT, "include"), "-o", str(exe), str(src)])
+    out = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).splitlines())
+    assert int(out["size"]) == ct.sizeof(_lib.BAStepProbeOut)
+    for f in fields:
+        assert int(out[f]) == getattr(_lib.BAStepProbeOut, f).offset, f
+
+
+def test_probe_rejects_a_null_problem_without_touching_the_device():
+    lib = _lib.load()
+    INVALID = 1   # B200SFM_ERR_INVALID_ARG
+    o, out = _lib.BAOpts(), _lib.BAStepProbeOut()
+    x = (ct.c_double * 6)()
+    assert lib.b200sfm_test_ba_step(None, ct.byref(o), 0.0, 1e4, ct.byref(out)) == INVALID
+    assert lib.b200sfm_test_ba_apply(None, x, x) == INVALID
