@@ -7,6 +7,7 @@
 #include <cub/cub.cuh>
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <vector>
@@ -24,42 +25,50 @@
 namespace b200 {
 
 // ---- structure-building kernels ----------------------------------------------
+// largest share of L2 that one point slice's 32-B records (z4 / pts4) may fill in the camera-order passes: 8 slices at
+// config 4 on an H100 (64 MB of records, 50 MB of L2), where the slice-count sweep of DESIGN §6 flattens; one at config 2
+constexpr double kSliceL2Share = 1.0 / 6.0;
+
 __global__ void k_expand_obs_pt(int P, const unsigned* __restrict__ pt_begin, int* __restrict__ obs_pt) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P) return;
   for (unsigned o = pt_begin[p]; o < pt_begin[p + 1]; ++o) obs_pt[o] = p;
 }
-// sort key = "virtual camera" (frame, sensor): vc = frame * smul + sensor  (smul = 1, sensor = 0 without rigs)
-__global__ void k_cam_keys(long long N, int VC, int smul, int min_views, const int* __restrict__ obs_cam,
-                           const unsigned short* __restrict__ obs_sensor,
+// sort key = bucket (camera half, point slice, "virtual camera"): ((half * n_slices + pt / slice_pts) * VC + vc, where
+// vc = frame * smul + sensor (smul = 1, sensor = 0 without rigs) and half = frame >= half_frame.  Excluded observations
+// get the key n_buckets, past every bucket.  One slice and half_frame past the last frame: the key is vc.
+__global__ void k_cam_keys(long long N, int VC, int smul, int min_views, int slice_pts, int n_slices, int half_frame,
+                           int n_buckets, const int* __restrict__ obs_cam, const unsigned short* __restrict__ obs_sensor,
                            const int* __restrict__ obs_pt, const unsigned* __restrict__ pt_begin,
-                           int* __restrict__ keys, int* __restrict__ vals, int* __restrict__ cam_count,
+                           int* __restrict__ keys, int* __restrict__ vals, int* __restrict__ bucket_count,
                            int* __restrict__ bad) {
   const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (o >= N) return;
   const int pt = obs_pt[o];
   const bool valid = (int)(pt_begin[pt + 1] - pt_begin[pt]) >= min_views;
   const int cam = obs_cam[o] * smul + (obs_sensor ? (int)obs_sensor[o] : 0);
-  const int C = VC;
   // caller-supplied camera index out of range: flag it (-> B200SFM_ERR_INVALID_ARG) instead of writing out of bounds
-  const bool in_range = obs_cam[o] >= 0 && cam < C;
+  const bool in_range = obs_cam[o] >= 0 && cam < VC;
   if (!in_range) *bad = 1;
-  keys[o] = (valid && in_range) ? cam : C;
+  const int bucket = ((obs_cam[o] >= half_frame ? n_slices : 0) + pt / slice_pts) * VC + cam;
+  keys[o] = (valid && in_range) ? bucket : n_buckets;
   vals[o] = (int)o;
-  if (valid && in_range) atomicAdd(&cam_count[cam], 1);
+  if (valid && in_range) atomicAdd(&bucket_count[bucket], 1);
 }
-__global__ void k_seg_counts(int C, const int* __restrict__ cam_count, int* __restrict__ seg_count) {
+__global__ void k_seg_counts(int n_buckets, const int* __restrict__ bucket_count, int* __restrict__ seg_count) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < C) seg_count[c] = (cam_count[c] + kSeg - 1) / kSeg;
+  if (c < n_buckets) seg_count[c] = (bucket_count[c] + kSeg - 1) / kSeg;
 }
-__global__ void k_fill_segs(int VC, int smul, const int* __restrict__ cam_begin, const int* __restrict__ seg_off,
+// segments of <= kSeg observations of one bucket (k_cam_keys): bucket c belongs to virtual camera c % VC
+__global__ void k_fill_segs(int n_buckets, int VC, int smul, const int* __restrict__ cam_begin, const int* __restrict__ seg_off,
                             const int* __restrict__ cam_intr, const int* __restrict__ sensor_intr,
                             int* __restrict__ seg_cam, int* __restrict__ seg_sensor, int* __restrict__ seg_intr,
                             int* __restrict__ seg_begin, int* __restrict__ seg_end) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= VC) return;
+  if (c >= n_buckets) return;
   const int b = cam_begin[c], e = cam_begin[c + 1];
-  const int frame = c / smul, sensor = c - frame * smul;
+  const int vc = c % VC;
+  const int frame = vc / smul, sensor = vc - frame * smul;
   const int blk = sensor_intr ? sensor_intr[sensor] : (cam_intr ? cam_intr[frame] : 0);
   int s = seg_off[c];
   for (int i = b; i < e; i += kSeg, ++s) {
@@ -92,11 +101,14 @@ __global__ void k_gather_int(int n, const int* __restrict__ idx, const int* __re
 }
 // blk_used[b] = 1: block b (frame f | C + intrinsics k | C + K + sensor s) has an observation of a kept track, i.e. it
 // is a parameter block of the problem whatever its curvature (plain stores of the same value: the races are benign)
-__global__ void k_block_used(int VC, int smul, int C, int K, const int* __restrict__ cam_count,
+__global__ void k_block_used(int VC, int n_groups, int smul, int C, int K, const int* __restrict__ bucket_count,
                              const int* __restrict__ cam_intr, const int* __restrict__ sensor_intr,
                              double* __restrict__ blk_used) {
   const int vc = blockIdx.x * blockDim.x + threadIdx.x;
-  if (vc >= VC || cam_count[vc] == 0) return;
+  if (vc >= VC) return;
+  int n = 0;   // observations of vc over its n_groups buckets (camera half x point slice)
+  for (int g = 0; g < n_groups; ++g) n += bucket_count[(size_t)g * VC + vc];
+  if (n == 0) return;
   const int f = vc / smul, s = vc - f * smul;
   blk_used[f] = 1.0;
   blk_used[C + (sensor_intr ? sensor_intr[s] : cam_intr[f])] = 1.0;
@@ -135,6 +147,7 @@ struct b200sfm_ba_problem {
   long long N = 0;
   int Nv = 0, n_tiles = 0, n_segs = 0, min_views = 3;
   int seg_mid = 0;   // first camera-order segment of a camera >= C / 2 (split all-reduce of the multi-GPU mat-vec)
+  int n_slices = 1, slice_pts = 0;   // camera-order rows are grouped by point slices of slice_pts points (create())
   long long n_obs_used = 0;
 
   // structure
@@ -318,58 +331,75 @@ struct b200sfm_ba_problem {
     if (st) st->h2d_bytes += N * 20 + ((long long)P + 1) * 4 + (long long)tiles.size() * 4 + (long long)C * 5 + K * 4;
 
     B200_LAUNCH(ctx, k_expand_obs_pt, cdiv(P, 256), 256, 0, P, pt_begin.p, obs_pt.p);
-    // camera order
+    // camera order, grouped by point slice.  Every camera-order kernel gathers one per-point record per observation
+    // (z4 / pts4: 32 B, Vinv: 48 B) at a random address.  CTAs start roughly in blockIdx order, so with the rows of
+    // one point slice together the resident warps gather from that slice's records only, and those stay in L2.
+    // Slices start on ELL windows; there are as many as it takes for a slice's 32-B records to fill at most
+    // kSliceL2Share of L2 (one slice, the plain camera order, when they all fit).  B200SFM_PT_SLICES=n asks for n.
+    {
+      int want = 1;
+      if (getenv("B200SFM_PT_SLICES")) {
+        want = std::max(1, atoi(getenv("B200SFM_PT_SLICES")));
+      } else {
+        int l2 = 0;
+        B200_CUDA_OK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, ctx->device));
+        want = std::max(1, cdiv((long long)P * 32, std::max(1ll, (long long)(l2 * kSliceL2Share))));
+      }
+      want = std::min(want, std::max(1, (INT_MAX - 1) / (2 * VC)));   // bucket keys stay ints
+      slice_pts = std::max(1, cdiv(cdiv(P, want), kEllWindow)) * kEllWindow;
+      n_slices = std::max(1, cdiv(P, slice_pts));
+    }
+    // buckets (camera half, point slice, virtual camera): the halves split at frame C/2, so that every camera below
+    // C/2 is complete after segment seg_mid (split all-reduce of the multi-GPU mat-vec); within a bucket the stable
+    // sort keeps point order
+    const int n_groups = 2 * n_slices, n_buckets = n_groups * VC;
     DevBuf<int> keys, vals, keys_out, cam_count, seg_count, cam_begin, seg_off, bad;
     keys.alloc(N); vals.alloc(N); keys_out.alloc(N); camord_obs.alloc(N);
-    cam_count.alloc((size_t)VC + 1); seg_count.alloc((size_t)VC + 1); cam_begin.alloc((size_t)VC + 1); seg_off.alloc((size_t)VC + 1);
+    cam_count.alloc((size_t)n_buckets + 1); seg_count.alloc((size_t)n_buckets + 1); cam_begin.alloc((size_t)n_buckets + 1);
+    seg_off.alloc((size_t)n_buckets + 1);
     bad.alloc(1);
     cam_count.zero(s); seg_count.zero(s); bad.zero(s);
-    B200_LAUNCH(ctx, k_cam_keys, cdiv(N, 256), 256, 0, N, VC, smul, min_views, obs_cam.p, S > 0 ? obs_sensor.p : nullptr,
-                obs_pt.p, pt_begin.p, keys.p, vals.p, cam_count.p, bad.p);
+    B200_LAUNCH(ctx, k_cam_keys, cdiv(N, 256), 256, 0, N, VC, smul, min_views, slice_pts, n_slices, C / 2, n_buckets,
+                obs_cam.p, S > 0 ? obs_sensor.p : nullptr, obs_pt.p, pt_begin.p, keys.p, vals.p, cam_count.p, bad.p);
     int end_bit = 1;
-    while ((1ll << end_bit) <= VC) ++end_bit;
+    while ((1ll << end_bit) <= n_buckets) ++end_bit;
     size_t tmp_bytes = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys.p, keys_out.p, vals.p, camord_obs.p, (int)N, 0, end_bit, s);
     size_t scan_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cam_count.p, cam_begin.p, VC + 1, s);
+    cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, cam_count.p, cam_begin.p, n_buckets + 1, s);
     DevBuf<unsigned char> tmp;
     tmp.alloc(std::max(tmp_bytes, scan_bytes) + 16);
     size_t tb = tmp.bytes();
     cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys.p, keys_out.p, vals.p, camord_obs.p, (int)N, 0, end_bit, s);
     ctx->launches += 8;
     tb = tmp.bytes();
-    cub::DeviceScan::ExclusiveSum(tmp.p, tb, cam_count.p, cam_begin.p, VC + 1, s);
-    B200_LAUNCH(ctx, k_seg_counts, cdiv(VC, 256), 256, 0, VC, cam_count.p, seg_count.p);
+    cub::DeviceScan::ExclusiveSum(tmp.p, tb, cam_count.p, cam_begin.p, n_buckets + 1, s);
+    B200_LAUNCH(ctx, k_seg_counts, cdiv(n_buckets, 256), 256, 0, n_buckets, cam_count.p, seg_count.p);
     blk_used.alloc(CB);
     blk_used.zero(s);
-    B200_LAUNCH(ctx, k_block_used, cdiv(VC, 256), 256, 0, VC, smul, C, K, cam_count.p, cam_intr.p,
+    B200_LAUNCH(ctx, k_block_used, cdiv(VC, 256), 256, 0, VC, n_groups, smul, C, K, cam_count.p, cam_intr.p,
                 S > 0 ? sensor_intr.p : nullptr, blk_used.p);
     ctx->allreduce_sum(blk_used.p, CB);   // a block observed on any rank is a block of the problem on every rank
     tb = tmp.bytes();
-    cub::DeviceScan::ExclusiveSum(tmp.p, tb, seg_count.p, seg_off.p, VC + 1, s);
+    cub::DeviceScan::ExclusiveSum(tmp.p, tb, seg_count.p, seg_off.p, n_buckets + 1, s);
     ctx->launches += 4;
-    int h_tot[3];
-    B200_CUDA_OK(cudaMemcpyAsync(&h_tot[0], cam_begin.p + VC, sizeof(int), cudaMemcpyDeviceToHost, s));
-    B200_CUDA_OK(cudaMemcpyAsync(&h_tot[1], seg_off.p + VC, sizeof(int), cudaMemcpyDeviceToHost, s));
+    int h_tot[4];
+    B200_CUDA_OK(cudaMemcpyAsync(&h_tot[0], cam_begin.p + n_buckets, sizeof(int), cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaMemcpyAsync(&h_tot[1], seg_off.p + n_buckets, sizeof(int), cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaMemcpyAsync(&h_tot[2], bad.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaMemcpyAsync(&h_tot[3], seg_off.p + (size_t)n_slices * VC, sizeof(int), cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     if (h_tot[2]) throw InvalidInput{"obs_cam out of range [0, C)"};
     Nv = h_tot[0];
     n_segs = h_tot[1];
+    seg_mid = h_tot[3];   // the first segment of the upper camera half
     seg_cam.alloc(std::max(n_segs, 1)); seg_begin.alloc(std::max(n_segs, 1)); seg_end.alloc(std::max(n_segs, 1));
     seg_sensor.alloc(std::max(n_segs, 1)); seg_intr.alloc(std::max(n_segs, 1));
     pt_c.alloc(std::max(Nv, 1)); xy_c.alloc(std::max(Nv, 1));
-    B200_LAUNCH(ctx, k_fill_segs, cdiv(VC, 256), 256, 0, VC, smul, cam_begin.p, seg_off.p, cam_intr.p,
+    B200_LAUNCH(ctx, k_fill_segs, cdiv(n_buckets, 256), 256, 0, n_buckets, VC, smul, cam_begin.p, seg_off.p, cam_intr.p,
                 S > 0 ? sensor_intr.p : nullptr, seg_cam.p, seg_sensor.p, seg_intr.p, seg_begin.p, seg_end.p);
     if (Nv > 0)
       B200_LAUNCH(ctx, k_gather_camorder, cdiv(Nv, 256), 256, 0, Nv, camord_obs.p, obs_pt.p, obs_xy.p, pt_c.p, xy_c.p);
-    seg_mid = n_segs;
-    if (ctx->world > 1 && n_segs > 0) {   // segments are sorted by camera (frame): split point of the overlapped all-reduce
-      std::vector<int> h_seg_cam(n_segs);
-      B200_CUDA_OK(cudaMemcpyAsync(h_seg_cam.data(), seg_cam.p, (size_t)n_segs * sizeof(int), cudaMemcpyDeviceToHost, s));
-      B200_CUDA_OK(cudaStreamSynchronize(s));
-      seg_mid = (int)(std::lower_bound(h_seg_cam.begin(), h_seg_cam.end(), C / 2) - h_seg_cam.begin());
-    }
     // v2 camera-order rows: every segment starts on a 32-row group boundary
     {
       DevBuf<int> padded;

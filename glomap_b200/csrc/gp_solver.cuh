@@ -146,8 +146,9 @@ struct b200sfm_gp_problem {
     cam_count.alloc((size_t)C + 1); seg_count.alloc((size_t)C + 1); cam_begin.alloc((size_t)C + 1); seg_off.alloc((size_t)C + 1);
     bad.alloc(1);
     cam_count.zero(s); seg_count.zero(s); bad.zero(s);
-    B200_LAUNCH(ctx, k_cam_keys, cdiv(N, 256), 256, 0, N, C, 1, min_views, obs_cam.p, nullptr, obs_pt.p, pt_begin.p, keys.p, vals.p,
-                cam_count.p, bad.p);
+    // plain camera order: one point slice, no camera halves (keys = camera)
+    B200_LAUNCH(ctx, k_cam_keys, cdiv(N, 256), 256, 0, N, C, 1, min_views, std::max(P, 1), 1, C, C, obs_cam.p, nullptr, obs_pt.p,
+                pt_begin.p, keys.p, vals.p, cam_count.p, bad.p);
     int end_bit = 1;
     while ((1ll << end_bit) <= C) ++end_bit;
     size_t tmp_bytes = 0, scan_bytes = 0;
@@ -173,7 +174,7 @@ struct b200sfm_gp_problem {
     n_segs = h_tot[1];
     seg_cam.alloc(std::max(n_segs, 1)); seg_begin.alloc(std::max(n_segs, 1)); seg_end.alloc(std::max(n_segs, 1));
     pt_c.alloc(std::max(Nv, 1));
-    B200_LAUNCH(ctx, k_fill_segs, cdiv(C, 256), 256, 0, C, 1, cam_begin.p, seg_off.p, nullptr, nullptr, seg_cam.p, nullptr, nullptr,
+    B200_LAUNCH(ctx, k_fill_segs, cdiv(C, 256), 256, 0, C, C, 1, cam_begin.p, seg_off.p, nullptr, nullptr, seg_cam.p, nullptr, nullptr,
                 seg_begin.p, seg_end.p);
     if (Nv > 0) B200_LAUNCH(ctx, k_gather_int, cdiv(Nv, 256), 256, 0, Nv, camord_obs.p, obs_pt.p, pt_c.p);
     for (int i = 0; i < 2; ++i) {
