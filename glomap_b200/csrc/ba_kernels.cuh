@@ -30,7 +30,6 @@ constexpr double kZEps = 1e-12;
 constexpr int kSeg = 256;     // observations per camera-order segment (one warp)
 constexpr int kIntrSmem = 16; // intrinsics blocks cached in shared memory by the point-order kernels
 constexpr int kJpDoubles = 6;  // v2 point-order row: A_o = J_pt^T J_pt (packed symmetric 3x3) -> 48 B
-constexpr int kJcDoubles = 9;  // v2 camera-order row: A_o (6), X_p (3) -> 72 B, stored SoA in groups of 32 rows
 constexpr int kSensorRec = 16; // known rigs: R_cam_from_rig (9, row-major), t_cam_from_rig (3), intrinsics idx, pad
 
 struct BAView {
@@ -52,7 +51,6 @@ struct BAView {
   const int* seg_cam;           // [n_segs]
   const int* seg_begin;         // [n_segs+1] (only within one camera: seg_end = seg_begin2[s])
   const int* seg_end;
-  const int* seg_row0;          // [n_segs] first (32-aligned) padded row of the segment in the v2 camera-order rows
   // known (constant) rigs -- bundle_adjustment.cc:147-161.  S == 0: every frame is trivial, obs_cam is the
   // image and the intrinsics index rides in the camera record.  S > 0: obs_cam is the FRAME (rig_from_world),
   // obs_sensor picks the constant cam_from_rig + intrinsics of the observing image; camera-order segments

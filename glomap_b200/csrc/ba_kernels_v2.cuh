@@ -7,19 +7,18 @@
 // (left-perturbed rotation, translation), so that with the symmetric 3x3
 //     A_o = J_pt^T J_pt        (what the observation adds to V_p)
 // W_o = G^T A_o,  W_o^T x = A_o v  with  v = R^T x_t - 2 X x (R^T x_r),
-// W_o z = [ 2 R (X x w) ; R w ],  w = A_o z.   Only A_o (48 B) is stored per
-// observation, in BOTH traversal orders:
-//     Ap[N][6]   point order  (tiles moved by TMA)
-//     Ac         camera order {A_o, X_p} (72 B, written by the camera-order linearisation), SoA in
-//                groups of 32 rows: element k of padded row r at ((r >> 5) * 9 + k) * 32 + (r & 31); every
-//                segment starts on a group boundary (seg_row0), so lane l of the segment's warp owns
-//                rows l, l + 32, ... and every load/store of the warp is one contiguous 256-B line pair
-// and the implicit-Schur mat-vec is two streaming passes
-//     pass A (point order):  s_p = sum_o A_o v_o,  z_p = Vinv s_p -> z4[P]      gathers R^T x (48 B)
-//     pass B (camera order): y_c -= R-rotated sum_o [2 X x (A_o z_p) ; A_o z_p]  gathers z_p (32 B)
+// W_o z = [ 2 R (X x w) ; R w ],  w = A_o z.   A_o (48 B) is stored per observation in POINT order only
+// (Ap[N][6], or the ELL rows of ba_kernels_v3.cuh), and the implicit-Schur mat-vec is two passes
+//     pass A (point order):  s_p = sum_o A_o v_o,  z_p = Vinv s_p -> z4[P]      streams A_o, gathers R^T x (64 B)
+//     pass B (camera order): y_c -= R-rotated sum_o [2 X x (A_o z_p) ; A_o z_p]  gathers X_p (pts4) and z_p (32 B each)
 //                            one warp per <= 256-observation segment of ONE camera: register
 //                            accumulation, shuffle reduction, 6 atomics per segment.
-// All arithmetic stays FP64.  Algorithmic bytes per mat-vec: 52 N + 80 P (A) + 76 N + 32 P (B).
+// In camera order the segment's camera, intrinsics and sensor records are warp-uniform, so pass B (and the Schur-Jacobi
+// diagonal) rebuild A_o from them, the pixel and the point with the linearisation's own arithmetic (obs_core +
+// obs_point_blocks) instead of streaming a stored camera-order row: about 160 FP64 instructions per observation in
+// place of 72 B of HBM traffic, the cheaper side on an H100.  All arithmetic stays FP64.
+// Algorithmic bytes per mat-vec: 52 N + 80 P (A) + 20 N + 64 P (B, point records gathered from L2: see the slices of
+// BAProblem::create).
 #pragma once
 #include "ba_kernels.cuh"
 #include "pcg.cuh"
@@ -27,12 +26,11 @@
 namespace b200 {
 
 struct BAViewV2 {
-  const double* Ap;   // [N][6]   (aliases BAView::W)
-  double* Ac;         // camera-order rows, SoA-32 (see above)
-  double* z4;         // [P][4]
-  // stored-row intrinsics path (NK > 0, see below): B_o = rho' J_pt^T J_k in camera order, the frame x intrinsics
-  // cross blocks of every image, the variable-parameter table and the number of frames (block C + k = intrinsics k)
-  double* Bc = nullptr;              // [rows32][3 * NK][32]
+  const double* Ap;     // [N][6]   (aliases BAView::W)
+  double* z4;           // [P][4]
+  const double* pts4;   // [P][4]   {X_p, 0} of the current state (ba2_pad_points at every linearisation)
+  // stored-row intrinsics path (NK > 0, see below): the frame x intrinsics cross blocks of every image, the
+  // variable-parameter table and the number of frames (block C + k = intrinsics k)
   double* Ufk = nullptr;             // [C][6][NK]
   const IntrVarRec* ivar = nullptr;  // [K]
   int C = 0;
@@ -43,12 +41,12 @@ struct BAViewV2 {
 // parameters per camera: SIMPLE_PINHOLE f; SIMPLE_RADIAL f, k; PINHOLE fx, fy -- the reference default
 // optimize_intrinsics = true, optimize_principal_point = false, bundle_adjustment.cc:273-293).
 // Intrinsics block k is pseudo-camera block C + k of the reduced system (ba_kernels_ext.cuh).  With J_k = d e / d(params)
-// (2 x NK) and B_o = rho' J_pt^T J_k (3 x NK, stored next to A_o in BOTH orders, 24 NK bytes each):
+// (2 x NK) and B_o = rho' J_pt^T J_k (3 x NK, stored next to A_o in point order, 24 NK bytes; recomputed in camera order):
 //     W^T x   per point:   s_p = sum_o ( A_o w_o + B_o x_k(o) )                    (pass A, x_k rides in the xq record)
 //     W z     per image:   y_f -= G^T sum_o A_o z_p,   y_k -= sum_o B_o^T z_p       (pass B)
 //     U x:    block diagonal U_ff, U_kk by pcg_apply_diag; the frame x intrinsics coupling is ONE 6 x NK block per image
 //             (an image has one camera):  y_f += U_fk x_k,  y_k += U_fk^T x_f       (ba2k_cross, C threads)
-// so the per-iteration cost over the constant-intrinsics path is 48 NK bytes per observation of streamed rows.
+// so the per-iteration cost over the constant-intrinsics path is 24 NK bytes per observation of streamed rows.
 // ---------------------------------------------------------------------------
 template <int NK>
 __device__ __forceinline__ void obs_intr_rows(const ObsCore& o, const double* __restrict__ ir, const IntrVarRec& iv,
@@ -123,7 +121,8 @@ __global__ void __launch_bounds__(kPcgThreads) ba2_pcg_direction_pack(int nb, in
   }
 }
 
-// pts4[p] = {X_p, 0}: 32-B rows for the camera-order gathers (one sector per observation)
+// pts4[p] = {X_p, 0}: 32-B rows for the camera-order gathers (one sector per observation).  Written at every
+// linearisation from points[cur]; a rejected step keeps points[cur], so it stays valid until the next one.
 __global__ void ba2_pad_points(int P, const double* __restrict__ points, double* __restrict__ pts4) {
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= P) return;
@@ -132,12 +131,11 @@ __global__ void ba2_pad_points(int P, const double* __restrict__ points, double*
 }
 
 // ---------------------------------------------------------------------------
-// camera-order linearisation: U_c, g_c AND the camera-order rows Ac = {A_o, X_p}
+// camera-order linearisation: U_c, g_c (and, NK > 0, U_kk, g_k, U_fk)
 // ---------------------------------------------------------------------------
 template <int NK>
 __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linearize_cams(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec,
-                                                         const double* __restrict__ intr_rec,
-                                                         const double* __restrict__ /*points: read through v2.z4 (padded copy)*/, double huber_a) {
+                                                         const double* __restrict__ intr_rec, double huber_a) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= v.n_segs) return;
@@ -154,13 +152,11 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
   for (int k = 0; k < 6; ++k) g[k] = 0.0;
   const int cmask = (int)(__double_as_longlong(t4c.w) & 0xff);
   const bool tvar = !(cmask & 2), rvar = !(cmask & 1);
-  double* row = v2.Ac + (size_t)(v.seg_row0[warp] >> 5) * (kJcDoubles * 32) + lane;
-  // stored-row intrinsics path: B_o rows, U_kk / g_k of the segment's intrinsics block and the image's 6 x NK cross block
+  // stored-row intrinsics path: U_kk / g_k of the segment's intrinsics block and the image's 6 x NK cross block
   constexpr int NKK = NK > 0 ? NK : 1;
   const int blk = v.seg_intr[warp];
   IntrVarRec iv{};
   if (NK > 0) iv = v2.ivar[blk];
-  double* rowB = NK > 0 ? v2.Bc + (size_t)(v.seg_row0[warp] >> 5) * (3 * NK * 32) + lane : nullptr;
   double Ukk[NKK * (NKK + 1) / 2], gk[NKK], Ufk[6][NKK];
 #pragma unroll
   for (int k = 0; k < NKK * (NKK + 1) / 2; ++k) Ukk[k] = 0.0;
@@ -173,9 +169,8 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
   // index -> point gather -> ~400 instructions: the first use of the gathered point and the address computed from the
   // streamed index each wait a full memory latency.  Register pipeline: the index of iteration + 2 and the
   // point / pixel of iteration + 1 are in flight while iteration + 0 is computed.  The points come from the 32-B padded
-  // copy (pts4 = the z4 buffer, idle during linearisation): ONE 32-B record (two 128-bit loads of one sector) instead of
-  // three 64-bit gathers.
-  const double* __restrict__ pts4 = v2.z4;
+  // copy pts4: ONE 32-B record (two 128-bit loads of one sector) instead of three 64-bit gathers.
+  const double* __restrict__ pts4 = v2.pts4;
   int i = b + lane;
   int pt_nxt = 0;
   double2 xy = make_double2(0, 0);
@@ -186,7 +181,7 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
     xy = ld_stream(v.xy_c + i);
     Xc = ld_rec32(pts4 + 4 * (size_t)pt0);
   }
-  for (; i < e; i += 32, row += kJcDoubles * 32) {
+  for (; i < e; i += 32) {
     double4 Xn = Xc;
     double2 xyn = xy;
     int pt_nn = 0;
@@ -200,11 +195,6 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
     obs_core(q4c, t4c, irc, src, X0, X1, X2, xy, huber_a, o);
     double Jp[6], A[6], bo[3];
     obs_point_blocks(o, Jp, A, bo);
-#pragma unroll
-    for (int k = 0; k < 6; ++k) st_stream(row + 32 * k, A[k]);
-    st_stream(row + 192, X0);
-    st_stream(row + 224, X1);
-    st_stream(row + 256, X2);
     // camera blocks: J_t = J, J_r = J (-2 [R X]x)  (EigenQuaternionManifold: left perturbation of angle 2|d|), masked;
     // U += rho' Jc^T Jc, g += rho' Jc^T e
     double Jc[2][6];
@@ -230,9 +220,6 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
     if (NK > 0) {
       double Jk[2][NKK], Bo[3 * NKK];
       obs_intr_rows<NK>(o, irc, iv, Jp, Jk, Bo);
-#pragma unroll
-      for (int k = 0; k < 3 * NK; ++k) st_stream(rowB + 32 * k, Bo[k]);
-      rowB += 3 * NK * 32;
       int ik = 0;
 #pragma unroll
       for (int a = 0; a < NK; ++a) {
@@ -278,27 +265,55 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
 }
 
 // ---------------------------------------------------------------------------
-// Schur-Jacobi diagonal from the camera-order rows, accumulated in the world
+// Schur-Jacobi diagonal in camera order, accumulated in the world
 // frame:  Sd_c = Rb ( sum_o Gh^T N Gh ) Rb^T,  N = A_o Vinv_p A_o,
 //         Gh = [ -2 [X]x | I ],  Rb = blockdiag(R, R)
+// A_o is recomputed as in pass B; per observation the kernel gathers the point (pts4, 32 B) and Vinv_p (48 B).
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) ba2_schur_diag(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec) {
+__global__ void __launch_bounds__(128) ba2_schur_diag(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec,
+                                                      const double* __restrict__ intr_rec, double huber_a) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= v.n_segs) return;
   const int cam = v.seg_cam[warp];
   const int b = v.seg_begin[warp], e = v.seg_end[warp];
+  const double4 q4c = ld_rec32(cam_rec + (size_t)cam * kCamRec);
+  const double4 t4c = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
+  const double* irc = intr_rec + (size_t)v.seg_intr[warp] * kIntrRec;
+  const double* src = sensor_of_seg(v, warp);
   // world-frame accumulators: RR (sym 6), RT (full 9), TT (sym 6)
   double RR[6] = {0, 0, 0, 0, 0, 0}, RT[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, TT[6] = {0, 0, 0, 0, 0, 0};
-  const double* row = v2.Ac + (size_t)(v.seg_row0[warp] >> 5) * (kJcDoubles * 32) + lane;
-  for (int i = b + lane; i < e; i += 32, row += kJcDoubles * 32) {
-    const double A[6] = {ld_stream(row), ld_stream(row + 32), ld_stream(row + 64), ld_stream(row + 96), ld_stream(row + 128),
-                         ld_stream(row + 160)};
-    const double X[3] = {ld_stream(row + 192), ld_stream(row + 224), ld_stream(row + 256)};
-    const int pt = ld_stream(v.pt_c + i);
-    const double2* vp = reinterpret_cast<const double2*>(v.Vinv + (size_t)pt * 6);
-    const double2 v0 = vp[0], v1 = vp[1], v2_ = vp[2];
-    const double vi[6] = {v0.x, v0.y, v1.x, v1.y, v2_.x, v2_.y};
+  // register pipeline of ba2_linearize_cams: the index of iteration + 2 and the point / pixel / Vinv of iteration + 1
+  // are in flight while iteration + 0 is computed
+  int i = b + lane;
+  int pt_nxt = 0;
+  double2 xy = make_double2(0, 0), va = xy, vb = xy, vc = xy;
+  double4 Xc = make_double4(0, 0, 0, 0);
+  if (i < e) {
+    const int pt0 = ld_stream(v.pt_c + i);
+    if (i + 32 < e) pt_nxt = ld_stream(v.pt_c + i + 32);
+    xy = ld_stream(v.xy_c + i);
+    Xc = ld_rec32(v2.pts4 + 4 * (size_t)pt0);
+    const double2* vp = reinterpret_cast<const double2*>(v.Vinv + (size_t)pt0 * 6);
+    va = vp[0]; vb = vp[1]; vc = vp[2];
+  }
+  for (; i < e; i += 32) {
+    double4 Xn = Xc;
+    double2 xyn = xy, van = va, vbn = vb, vcn = vc;
+    int pt_nn = 0;
+    if (i + 32 < e) {
+      Xn = ld_rec32(v2.pts4 + 4 * (size_t)pt_nxt);
+      xyn = ld_stream(v.xy_c + i + 32);
+      const double2* vp = reinterpret_cast<const double2*>(v.Vinv + (size_t)pt_nxt * 6);
+      van = vp[0]; vbn = vp[1]; vcn = vp[2];
+    }
+    if (i + 64 < e) pt_nn = ld_stream(v.pt_c + i + 64);
+    const double X[3] = {Xc.x, Xc.y, Xc.z};
+    ObsCore o;
+    obs_core(q4c, t4c, irc, src, X[0], X[1], X[2], xy, huber_a, o);
+    double Jp[6], A[6], bo[3];
+    obs_point_blocks(o, Jp, A, bo);
+    const double vi[6] = {va.x, va.y, vb.x, vb.y, vc.x, vc.y};
     // T = Vinv A (columns), N = A T (symmetric 3x3)
     const double Ac0[3] = {A[0], A[1], A[2]}, Ac1[3] = {A[1], A[3], A[4]}, Ac2[3] = {A[2], A[4], A[5]};
     double T0[3], T1[3], T2[3];
@@ -338,6 +353,7 @@ __global__ void __launch_bounds__(128) ba2_schur_diag(BAView v, BAViewV2 v2, con
 #pragma unroll
       for (int c = 0; c < 3; ++c) RT[3 * r + c] += P[r][c];
     TT[0] += N[0][0]; TT[1] += N[0][1]; TT[2] += N[0][2]; TT[3] += N[1][1]; TT[4] += N[1][2]; TT[5] += N[2][2];
+    Xc = Xn; xy = xyn; va = van; vb = vbn; vc = vcn; pt_nxt = pt_nn;
   }
 #pragma unroll
   for (int k = 0; k < 6; ++k) RR[k] = warp_sum(RR[k]);
@@ -346,8 +362,6 @@ __global__ void __launch_bounds__(128) ba2_schur_diag(BAView v, BAViewV2 v2, con
 #pragma unroll
   for (int k = 0; k < 6; ++k) TT[k] = warp_sum(TT[k]);
   if (lane == 0) {
-    const double4 q4c = ld_rec32(cam_rec + (size_t)cam * kCamRec);
-    const double4 t4c = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
     const int mask = (int)(__double_as_longlong(t4c.w) & 0xff);
     const double q[4] = {q4c.x, q4c.y, q4c.z, q4c.w};
     double R[9];
@@ -581,10 +595,14 @@ __global__ void ba2_point_rhs_z(BAView v, BAViewV2 v2) {
 }
 
 // ---------------------------------------------------------------------------
-// pass B (camera order): y_c -= [ 2 R sum (X x w) ; R sum w ],  w = A_o z_p
+// pass B (camera order): y_c -= [ 2 R sum (X x w) ; R sum w ],  w = A_o z_p   (NK > 0: y_k -= sum B_o^T z_p)
+// A_o (and B_o) are rebuilt per observation from the segment's camera / intrinsics / sensor records, the pixel and the
+// point, by the arithmetic of the linearisations (obs_core, obs_point_blocks, obs_intr_rows); per observation the
+// kernel streams the index and the pixel (20 B) and gathers two 32-B point records, X_p (pts4) and z_p (z4).
 // ---------------------------------------------------------------------------
 template <int NK>
 __global__ void __launch_bounds__(128, B200_PB_MIN_CTAS) ba2_pass_b(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec,
+                                                 const double* __restrict__ intr_rec, double huber_a,
                                                  double* __restrict__ y, const PcgCtl* __restrict__ ctl, int seg_lo,
                                                  int seg_hi) {
   if (ctl && ctl->done) return;
@@ -593,102 +611,77 @@ __global__ void __launch_bounds__(128, B200_PB_MIN_CTAS) ba2_pass_b(BAView v, BA
   if (warp >= seg_hi) return;
   const int cam = v.seg_cam[warp];
   const int b = v.seg_begin[warp], e = v.seg_end[warp];
-  double acc[6] = {0, 0, 0, 0, 0, 0};
+  const double4 q4c = ld_rec32(cam_rec + (size_t)cam * kCamRec);
+  const double4 t4c = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
+  const int blk = v.seg_intr[warp];
+  const double* irc = intr_rec + (size_t)blk * kIntrRec;
+  const double* src = sensor_of_seg(v, warp);
   constexpr int NKK = NK > 0 ? NK : 1;
+  IntrVarRec iv{};
+  if (NK > 0) iv = v2.ivar[blk];
+  double acc[6] = {0, 0, 0, 0, 0, 0};
   double accK[NKK];
 #pragma unroll
   for (int k = 0; k < NKK; ++k) accK[k] = 0.0;
-  const double* rowB0 = NK > 0 ? v2.Bc + (size_t)(v.seg_row0[warp] >> 5) * (3 * NK * 32) + lane : nullptr;
-  // two observations per lane and iteration: both index loads, then both gathers, are in flight together
-  const double* row0 = v2.Ac + (size_t)(v.seg_row0[warp] >> 5) * (kJcDoubles * 32) + lane;
   const uint64_t keep = l2_policy_evict_last();
-  // all point indices of the segment first (<= kSeg / 32 per lane): the z gathers then depend on nothing but
-  // these registers, so every iteration costs one memory latency instead of two (index, then gather)
-  int ptr[kSeg / 32];
-#if B200_PB_PREFETCH
-#pragma unroll
-  for (int j = 0; j < kSeg / 32; ++j) {
-    const int i = b + lane + 32 * j;
-    ptr[j] = i < e ? ld_stream(v.pt_c + i) : -1;
+  // register pipeline of ba2_linearize_cams: the index of iteration + 2 and the point, z and pixel of iteration + 1 are
+  // in flight while iteration + 0 is computed
+  int i = b + lane;
+  int pt_nxt = 0;
+  double4 X = make_double4(0, 0, 0, 0), z = X;
+  double2 xy = make_double2(0, 0);
+  if (i < e) {
+    const int pt0 = ld_stream(v.pt_c + i);
+    if (i + 32 < e) pt_nxt = ld_stream(v.pt_c + i + 32);
+    X = ld_rec32(v2.pts4 + 4 * (size_t)pt0);
+    z = ld_keep4(v2.z4 + 4 * (size_t)pt0, keep);
+    xy = ld_stream(v.xy_c + i);
   }
-#endif
+  for (; i < e; i += 32) {
+    double4 Xn = X, zn = z;
+    double2 xyn = xy;
+    int pt_nn = 0;
+    if (i + 32 < e) {
+      Xn = ld_rec32(v2.pts4 + 4 * (size_t)pt_nxt);
+      zn = ld_keep4(v2.z4 + 4 * (size_t)pt_nxt, keep);
+      xyn = ld_stream(v.xy_c + i + 32);
+    }
+    if (i + 64 < e) pt_nn = ld_stream(v.pt_c + i + 64);
+    ObsCore o;
+    obs_core(q4c, t4c, irc, src, X.x, X.y, X.z, xy, huber_a, o);
+    double Jp[6], a[6], bo[3];
+    obs_point_blocks(o, Jp, a, bo);
+    const double w0 = a[0] * z.x + a[1] * z.y + a[2] * z.z;
+    const double w1 = a[1] * z.x + a[3] * z.y + a[4] * z.z;
+    const double w2 = a[2] * z.x + a[4] * z.y + a[5] * z.z;
+    acc[0] += 2.0 * (X.y * w2 - X.z * w1);
+    acc[1] += 2.0 * (X.z * w0 - X.x * w2);
+    acc[2] += 2.0 * (X.x * w1 - X.y * w0);
+    acc[3] += w0;
+    acc[4] += w1;
+    acc[5] += w2;
+    if (NK > 0) {
+      double Jk[2][NKK], Bo[3 * NKK];
+      obs_intr_rows<NK>(o, irc, iv, Jp, Jk, Bo);
 #pragma unroll
-  for (int j = 0; j < kSeg / 32; j += 2) {
-    if (b + 32 * j >= e) break;
-#if !B200_PB_PREFETCH
-    {
-      const int i = b + lane + 32 * j;
-      ptr[j] = i < e ? ld_stream(v.pt_c + i) : -1;
-      ptr[j + 1] = i + 32 < e ? ld_stream(v.pt_c + i + 32) : -1;
+      for (int k = 0; k < NK; ++k) accK[k] += Bo[3 * k] * z.x + Bo[3 * k + 1] * z.y + Bo[3 * k + 2] * z.z;
     }
-#endif
-    const int pt0 = ptr[j], pt1 = ptr[j + 1];
-    const bool ok0 = pt0 >= 0, ok1 = pt1 >= 0;
-    const double* r0p = row0 + (size_t)j * (kJcDoubles * 32);
-    const double* r1p = ok1 ? r0p + kJcDoubles * 32 : r0p;
-    double a[kJcDoubles], c[kJcDoubles];
-    double4 z0 = make_double4(0, 0, 0, 0), z1 = z0;
-    if (ok0) {
-#pragma unroll
-      for (int k = 0; k < kJcDoubles; ++k) a[k] = ld_stream(r0p + 32 * k);
-#pragma unroll
-      for (int k = 0; k < kJcDoubles; ++k) c[k] = ld_stream(r1p + 32 * k);
-      z0 = ld_keep4(v2.z4 + 4 * (size_t)pt0, keep);
-      z1 = ld_keep4(v2.z4 + 4 * (size_t)(ok1 ? pt1 : pt0), keep);
-    }
-    if (NK > 0 && ok0) {   // y_k -= sum_o B_o^T z_p
-      const double* b0p = rowB0 + (size_t)j * (3 * NK * 32);
-      const double* b1p = ok1 ? b0p + 3 * NK * 32 : b0p;
-#pragma unroll
-      for (int k = 0; k < NK; ++k) {
-        accK[k] += ld_stream(b0p + 32 * (3 * k)) * z0.x + ld_stream(b0p + 32 * (3 * k + 1)) * z0.y +
-                   ld_stream(b0p + 32 * (3 * k + 2)) * z0.z;
-        if (ok1)
-          accK[k] += ld_stream(b1p + 32 * (3 * k)) * z1.x + ld_stream(b1p + 32 * (3 * k + 1)) * z1.y +
-                     ld_stream(b1p + 32 * (3 * k + 2)) * z1.z;
-      }
-    }
-    if (ok0) {
-      const double w0 = a[0] * z0.x + a[1] * z0.y + a[2] * z0.z;
-      const double w1 = a[1] * z0.x + a[3] * z0.y + a[4] * z0.z;
-      const double w2 = a[2] * z0.x + a[4] * z0.y + a[5] * z0.z;
-      const double X0 = a[6], X1 = a[7], X2 = a[8];
-      acc[0] += 2.0 * (X1 * w2 - X2 * w1);
-      acc[1] += 2.0 * (X2 * w0 - X0 * w2);
-      acc[2] += 2.0 * (X0 * w1 - X1 * w0);
-      acc[3] += w0;
-      acc[4] += w1;
-      acc[5] += w2;
-    }
-    if (ok1) {
-      const double w0 = c[0] * z1.x + c[1] * z1.y + c[2] * z1.z;
-      const double w1 = c[1] * z1.x + c[3] * z1.y + c[4] * z1.z;
-      const double w2 = c[2] * z1.x + c[4] * z1.y + c[5] * z1.z;
-      const double X0 = c[6], X1 = c[7], X2 = c[8];
-      acc[0] += 2.0 * (X1 * w2 - X2 * w1);
-      acc[1] += 2.0 * (X2 * w0 - X0 * w2);
-      acc[2] += 2.0 * (X0 * w1 - X1 * w0);
-      acc[3] += w0;
-      acc[4] += w1;
-      acc[5] += w2;
-    }
+    X = Xn; z = zn; xy = xyn; pt_nxt = pt_nn;
   }
 #pragma unroll
   for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
   if (lane < 6) {
-    const double4 q4c = ld_rec32(cam_rec + (size_t)cam * kCamRec);
-    const double4 t4c = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
     const int mask = (int)(__double_as_longlong(t4c.w) & 0xff);
     const double q[4] = {q4c.x, q4c.y, q4c.z, q4c.w};
     double R[9];
     quat_to_R(q, R);
-    const int blk = lane / 3, r = lane % 3;
-    const bool fixed = blk == 0 ? (mask & 1) : (mask & 2);
-    const double s = R[3 * r] * acc[3 * blk] + R[3 * r + 1] * acc[3 * blk + 1] + R[3 * r + 2] * acc[3 * blk + 2];
+    const int bl = lane / 3, r = lane % 3;
+    const bool fixed = bl == 0 ? (mask & 1) : (mask & 2);
+    const double s = R[3 * r] * acc[3 * bl] + R[3 * r + 1] * acc[3 * bl + 1] + R[3 * r + 2] * acc[3 * bl + 2];
     if (!fixed && s != 0.0) atomicAdd(&y[(size_t)cam * 6 + lane], -s);
   }
   if (NK > 0) {
-    const size_t kb = (size_t)(v2.C + v.seg_intr[warp]);
+    const size_t kb = (size_t)(v2.C + blk);
 #pragma unroll
     for (int k = 0; k < NK; ++k) {
       const double sk = warp_sum(accK[k]);

@@ -79,13 +79,6 @@ __global__ void k_fill_segs(int n_buckets, int VC, int smul, const int* __restri
     seg_end[s] = min(i + kSeg, e);
   }
 }
-// padded length (multiple of 32 rows) of every segment -> scanned into seg_row0
-__global__ void k_seg_padded_len(int n_segs, const int* __restrict__ seg_begin, const int* __restrict__ seg_end,
-                                 int* __restrict__ out) {
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  if (s < n_segs) out[s] = (seg_end[s] - seg_begin[s] + 31) & ~31;
-  if (s == n_segs) out[s] = 0;
-}
 __global__ void k_gather_camorder(int Nv, const int* __restrict__ camord_obs, const int* __restrict__ obs_pt,
                                   const double2* __restrict__ obs_xy, int* __restrict__ pt_c,
                                   double2* __restrict__ xy_c) {
@@ -147,7 +140,7 @@ struct b200sfm_ba_problem {
   long long N = 0;
   int Nv = 0, n_tiles = 0, n_segs = 0, min_views = 3;
   int seg_mid = 0;   // first camera-order segment of a camera >= C / 2 (split all-reduce of the multi-GPU mat-vec)
-  int n_slices = 1, slice_pts = 0;   // camera-order rows are grouped by point slices of slice_pts points (create())
+  int n_slices = 1, slice_pts = 0;   // camera-order observations are grouped by point slices of slice_pts points (create())
   long long n_obs_used = 0;
 
   // structure
@@ -155,8 +148,7 @@ struct b200sfm_ba_problem {
   // known rigs (S > 0): see BAView
   int S = 0;
   DevBuf<unsigned short> obs_sensor;
-  DevBuf<int> seg_sensor, seg_intr, sensor_intr, seg_row0;
-  long long n_rows_padded = 0;   // v2 camera-order rows incl. the per-segment padding to 32
+  DevBuf<int> seg_sensor, seg_intr, sensor_intr;
   DevBuf<double> sensor_rec;
   DevBuf<double2> obs_xy, xy_c;
   DevBuf<int4> tile_desc;
@@ -196,16 +188,16 @@ struct b200sfm_ba_problem {
     e.sensor = S > 0 ? ell_sensor.p : nullptr; e.A = ell_A.p; e.B = kfast ? ell_B.p : nullptr;
     return e;
   }
-  DevBuf<double> Jc, z4, xq, bpart, bpart2;
+  DevBuf<double> z4, pts4, xq, bpart, bpart2;
   size_t smem_k3v2 = 0;
   // stored-row intrinsics path (ba_kernels_v2.cuh): <= 2 variable parameters per camera, no unknown cam_from_rig
   bool kfast = false;
   int nk = 0;
-  DevBuf<double> ell_B, Bc, Ufk;
+  DevBuf<double> ell_B, Ufk;
   b200::BAViewV2 view2() {
     b200::BAViewV2 w;
-    w.Ap = W.p; w.Ac = Jc.p; w.z4 = z4.p;
-    w.Bc = kfast ? Bc.p : nullptr; w.Ufk = kfast ? Ufk.p : nullptr; w.ivar = ivar.p; w.C = C;
+    w.Ap = W.p; w.z4 = z4.p; w.pts4 = pts4.p;
+    w.Ufk = kfast ? Ufk.p : nullptr; w.ivar = ivar.p; w.C = C;
     return w;
   }
   int cur = 0;
@@ -228,7 +220,7 @@ struct b200sfm_ba_problem {
     v.C = C; v.P = P; v.K = K; v.N = N; v.n_tiles = n_tiles; v.n_segs = n_segs; v.min_views = min_views;
     v.obs_cam = obs_cam.p; v.obs_pt = obs_pt.p; v.obs_xy = obs_xy.p; v.pt_begin = pt_begin.p;
     v.tile_pt_begin = tile_pt_begin.p; v.tile_desc = tile_desc.p; v.camord_obs = camord_obs.p; v.pt_c = pt_c.p; v.xy_c = xy_c.p;
-    v.seg_cam = seg_cam.p; v.seg_begin = seg_begin.p; v.seg_end = seg_end.p; v.seg_row0 = seg_row0.p;
+    v.seg_cam = seg_cam.p; v.seg_begin = seg_begin.p; v.seg_end = seg_end.p;
     v.S = S; v.obs_sensor = obs_sensor.p; v.seg_sensor = seg_sensor.p; v.seg_intr = seg_intr.p; v.sensor_rec = sensor_rec.p;
     v.W = W.p; v.V = V.p; v.Vinv = Vinv.p; v.gp = gp.p; v.U = U(); v.gc = gc(); v.Sd = Sd.p; v.Minv = Minv.p;
     v.jscale_c = jscale_c.p; v.jscale_p = jscale_p.p; v.Dc = Dc.p;
@@ -400,24 +392,6 @@ struct b200sfm_ba_problem {
                 S > 0 ? sensor_intr.p : nullptr, seg_cam.p, seg_sensor.p, seg_intr.p, seg_begin.p, seg_end.p);
     if (Nv > 0)
       B200_LAUNCH(ctx, k_gather_camorder, cdiv(Nv, 256), 256, 0, Nv, camord_obs.p, obs_pt.p, obs_xy.p, pt_c.p, xy_c.p);
-    // v2 camera-order rows: every segment starts on a 32-row group boundary
-    {
-      DevBuf<int> padded;
-      padded.alloc((size_t)n_segs + 1);
-      seg_row0.alloc((size_t)n_segs + 1);
-      B200_LAUNCH(ctx, k_seg_padded_len, cdiv(n_segs + 1, 256), 256, 0, n_segs, seg_begin.p, seg_end.p, padded.p);
-      size_t need = 0;
-      cub::DeviceScan::ExclusiveSum(nullptr, need, padded.p, seg_row0.p, n_segs + 1, s);
-      DevBuf<unsigned char> tmp2;
-      tmp2.alloc(need + 16);
-      size_t tb2 = tmp2.bytes();
-      cub::DeviceScan::ExclusiveSum(tmp2.p, tb2, padded.p, seg_row0.p, n_segs + 1, s);
-      ctx->launches += 1;
-      int h_rows = 0;
-      B200_CUDA_OK(cudaMemcpyAsync(&h_rows, seg_row0.p + n_segs, sizeof(int), cudaMemcpyDeviceToHost, s));
-      B200_CUDA_OK(cudaStreamSynchronize(s));
-      n_rows_padded = h_rows;
-    }
 
     // ELL-32 point-order structure (ba_kernels_v3.cuh): windows of 1024 points sorted by track length, 32 per group
     {
@@ -487,7 +461,7 @@ struct b200sfm_ba_problem {
     B200_CUDA_OK(cudaFuncSetAttribute(ba2_pass_a<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_k3v2));
     B200_CUDA_OK(cudaFuncSetAttribute(ba2_pass_a<0>, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
     B200_CUDA_OK(cudaFuncSetAttribute(ba2_pass_a<2>, cudaFuncAttributePreferredSharedMemoryCarveout, carve));
-    Jc.alloc((size_t)std::max<long long>(n_rows_padded, 32) * kJcDoubles); z4.alloc((size_t)P * 4); xq.alloc((size_t)C * kXqStride);
+    z4.alloc((size_t)P * 4); pts4.alloc((size_t)P * 4); xq.alloc((size_t)C * kXqStride);
     bpart.alloc((size_t)std::max(std::max(n_tiles, ell_bpart_rows), 1) * 4);
     bpart2.alloc(296 * 4);
     B200_CUDA_OK(cudaStreamSynchronize(s));   // temporaries go out of scope
@@ -624,16 +598,16 @@ struct b200sfm_ba_problem {
       const int sgrid = cdiv((long long)n_segs * 32, 128);
       if (kfast) {
         Ufk.zero(s);
-        B200_LAUNCH(ctx, ba2_pad_points, cdiv(P, 256), 256, 0, P, points[cur].p, z4.p);
-        if (nk == 2) B200_LAUNCH(ctx, ba2_linearize_cams<2>, sgrid, 128, 0, v, view2(), cam_rec.p, intr_rec.p, points[cur].p, huber_a);
-        else B200_LAUNCH(ctx, ba2_linearize_cams<1>, sgrid, 128, 0, v, view2(), cam_rec.p, intr_rec.p, points[cur].p, huber_a);
+        B200_LAUNCH(ctx, ba2_pad_points, cdiv(P, 256), 256, 0, P, points[cur].p, pts4.p);
+        if (nk == 2) B200_LAUNCH(ctx, ba2_linearize_cams<2>, sgrid, 128, 0, v, view2(), cam_rec.p, intr_rec.p, huber_a);
+        else B200_LAUNCH(ctx, ba2_linearize_cams<1>, sgrid, 128, 0, v, view2(), cam_rec.p, intr_rec.p, huber_a);
       } else if (ext) {
         B200_LAUNCH(ctx, bax_linearize_blocks<0>, sgrid, 128, 0, v, ext_view(), cam_rec.p, intr_rec.p, points[cur].p, huber_a);
         if (ext_k) B200_LAUNCH(ctx, bax_linearize_blocks<1>, sgrid, 128, 0, v, ext_view(), cam_rec.p, intr_rec.p, points[cur].p, huber_a);
         if (ext_s) B200_LAUNCH(ctx, bax_linearize_blocks<2>, sgrid, 128, 0, v, ext_view(), cam_rec.p, intr_rec.p, points[cur].p, huber_a);
       } else if (use_v2) {
-        B200_LAUNCH(ctx, ba2_pad_points, cdiv(P, 256), 256, 0, P, points[cur].p, z4.p);   // z4 is idle until the mat-vec
-        B200_LAUNCH(ctx, ba2_linearize_cams<0>, sgrid, 128, 0, v, view2(), cam_rec.p, intr_rec.p, points[cur].p, huber_a);
+        B200_LAUNCH(ctx, ba2_pad_points, cdiv(P, 256), 256, 0, P, points[cur].p, pts4.p);
+        B200_LAUNCH(ctx, ba2_linearize_cams<0>, sgrid, 128, 0, v, view2(), cam_rec.p, intr_rec.p, huber_a);
       } else {
         B200_LAUNCH(ctx, ba_linearize_cams, sgrid, 128, 0, v, cam_rec.p, intr_rec.p, points[cur].p, huber_a);
       }
@@ -801,14 +775,18 @@ struct b200sfm_ba_problem {
     }
   }
 
-  void launch_pass_b(const b200::BAView& v, double* y, const b200::PcgCtl* ctl, int seg_lo = 0, int seg_hi = -1) {
+  void launch_pass_b(const b200::BAView& v, double huber_a, double* y, const b200::PcgCtl* ctl, int seg_lo = 0,
+                     int seg_hi = -1) {
     using namespace b200;
     if (seg_hi < 0) seg_hi = n_segs;
     if (seg_hi <= seg_lo) return;
     const int grid = cdiv((long long)(seg_hi - seg_lo) * 32, 128);
-    if (kfast && nk == 2) B200_LAUNCH(ctx, ba2_pass_b<2>, grid, 128, 0, v, view2(), cam_rec.p, y, ctl, seg_lo, seg_hi);
-    else if (kfast) B200_LAUNCH(ctx, ba2_pass_b<1>, grid, 128, 0, v, view2(), cam_rec.p, y, ctl, seg_lo, seg_hi);
-    else B200_LAUNCH(ctx, ba2_pass_b<0>, grid, 128, 0, v, view2(), cam_rec.p, y, ctl, seg_lo, seg_hi);
+#define B200_PASS_B(NKV) \
+  B200_LAUNCH(ctx, ba2_pass_b<NKV>, grid, 128, 0, v, view2(), cam_rec.p, intr_rec.p, huber_a, y, ctl, seg_lo, seg_hi)
+    if (kfast && nk == 2) B200_PASS_B(2);
+    else if (kfast) B200_PASS_B(1);
+    else B200_PASS_B(0);
+#undef B200_PASS_B
   }
   void launch_pass_a0(const b200::BAView& v, double radius, const b200::PcgCtl* ctl) {
     using namespace b200;
@@ -861,14 +839,14 @@ struct b200sfm_ba_problem {
       if (split_ar) {
         // cameras below C/2 are complete after the first half of the (camera-sorted) segments: their all-reduce
         // runs on the second stream while pass B works through the upper half
-        launch_pass_b(v, y, ctl, 0, seg_mid);
+        launch_pass_b(v, o.thres_loss_function, y, ctl, 0, seg_mid);
         B200_CUDA_OK(cudaEventRecord(ctx->ev_half, s));
         B200_CUDA_OK(cudaStreamWaitEvent(ctx->comm_stream, ctx->ev_half, 0));
         ctx->allreduce_sum_on(ctx->comm_stream, y, (size_t)(C / 2) * 6);
         B200_CUDA_OK(cudaEventRecord(ctx->ev_comm, ctx->comm_stream));
-        launch_pass_b(v, y, ctl, seg_mid, n_segs);
+        launch_pass_b(v, o.thres_loss_function, y, ctl, seg_mid, n_segs);
       } else if (n_segs > 0) {
-        launch_pass_b(v, y, ctl);
+        launch_pass_b(v, o.thres_loss_function, y, ctl);
       }
     } else {
       B200_LAUNCH(ctx, ba_schur_pass<0>, n_tiles, kTile, smem_k3, v, x, y, nullptr, nullptr, radius, nullptr, nullptr,
@@ -897,14 +875,16 @@ struct b200sfm_ba_problem {
     double* yrhs = Sd.p + (size_t)CB * 21;   // W Vinv g_p accumulates next to Sd so that both share one all-reduce
     Sd.zero(s);
     if (schur_jacobi && n_segs > 0) {
-      if (use_v2) B200_LAUNCH(ctx, ba2_schur_diag, cdiv((long long)n_segs * 32, 128), 128, 0, v, view2(), cam_rec.p);
+      if (use_v2)
+        B200_LAUNCH(ctx, ba2_schur_diag, cdiv((long long)n_segs * 32, 128), 128, 0, v, view2(), cam_rec.p, intr_rec.p,
+                    o.thres_loss_function);
       else B200_LAUNCH(ctx, ba_schur_diag, cdiv((long long)n_segs * 32, 128), 128, 0, v);
     }
     if (points_var) {
       if (use_v2) {
         B200_LAUNCH(ctx, ba2_point_rhs_z, cdiv(P, 256), 256, 0, v, view2());
         if (recomp) ext_matvec(nullptr, yrhs, o.thres_loss_function, radius, true, nullptr);
-        else if (n_segs > 0) launch_pass_b(v, yrhs, nullptr);
+        else if (n_segs > 0) launch_pass_b(v, o.thres_loss_function, yrhs, nullptr);
       } else {
         B200_LAUNCH(ctx, ba_schur_pass<1>, n_tiles, kTile, smem_k3, v, nullptr, yrhs, nullptr, nullptr, radius, nullptr);
       }
@@ -1079,8 +1059,6 @@ struct b200sfm_ba_problem {
     if (kfast) {
       const size_t cells = (size_t)std::max<long long>(ell_rows, 1) * 32;
       if (ell_B.n < cells * 3 * nk) ell_B.alloc(cells * 3 * nk);
-      const size_t crow = (size_t)std::max<long long>(n_rows_padded, 32) * 3 * nk;
-      if (Bc.n < crow) Bc.alloc(crow);
       if (Ufk.n < (size_t)C * 6 * nk) Ufk.alloc((size_t)C * 6 * nk);
     }
   }
@@ -1091,7 +1069,8 @@ struct b200sfm_ba_problem {
   }
 
   // A step that is not accepted: compute_step ended by building the records of the candidate (for its cost); the next
-  // step works on the same linearisation, whose stored rows and Jacobians belong to the current state's records.
+  // step works on the same linearisation, whose stored rows and Jacobians belong to the current state's records (and
+  // the camera-order kernels rebuild A_o from those records and pts4, which still holds points[cur]).
   void reject_step() { build_records(cur); }
 
   // The LM loop, Ceres order of checks (see oracle/ceres_lm.py).

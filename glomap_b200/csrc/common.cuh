@@ -24,11 +24,8 @@ namespace b200 {
 #ifndef B200_LC_MIN_CTAS   // v2 camera-order linearisation
 #define B200_LC_MIN_CTAS 3   // the register-pipelined kernel needs ~168 registers without spills (3 CTAs); 4 CTAs was slower on H100
 #endif
-#ifndef B200_PB_PREFETCH   // v2 pass B: load all point indices of a segment before the gathers (one latency per iteration)
-#define B200_PB_PREFETCH 1
-#endif
 #ifndef B200_PB_MIN_CTAS
-#define B200_PB_MIN_CTAS 7   // H100 config-4 sweep: 5 and 9 within 2 % of 7
+#define B200_PB_MIN_CTAS 4   // pass B rebuilds A_o per observation: 124 registers at 4; 5 and 6 spill and were slower (DESIGN §6)
 #endif
 #ifndef B200_E1_MIN_CTAS   // ELL point-side linearisation (one thread per point): CTAs of 128 threads per SM
 #define B200_E1_MIN_CTAS 4   // with the register pipeline: ~122 registers, no spills, 16 warps / SM (H100 sweep: 3 equal, 5 slower)
