@@ -6,7 +6,7 @@ import ctypes as ct
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("B200SFM_LIB", os.path.join(_HERE, "libb200sfm.so"))   # env override: kernel-tuning sweeps only
+LIB_PATH = os.environ.get("B200SFM_LIB", os.path.join(_HERE, "libb200sfm.so"))   # env override: tuning builds, other revisions, test doubles
 
 INTR_STRIDE = 12
 NCCL_ID_BYTES = 128
@@ -110,6 +110,8 @@ PROTOTYPES = {
     "b200sfm_tracks_establish": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_double, P(c_void_p),
                                            P(c_int64), P(c_int64), P(c_int64)]),
     "b200sfm_tracks_get": (c_int32, [c_void_p] * 5),
+    "b200sfm_image_pairs_inlier_count": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                                   c_int64] + [c_void_p] * 9 + [c_double] * 3 + [c_void_p] * 3),
     "b200sfm_tracks_free": (None, [c_void_p]),
     "b200sfm_gp_default_opts": (None, [P(GPOpts)]),
     "b200sfm_gp_solve": (c_int32, [c_void_p, P(GPOpts), c_int32, c_int32, c_int64] + [c_void_p] * 8 + [P(LMStats)]),
@@ -149,8 +151,16 @@ TEST_PROTOTYPES = {
 _lib = None
 
 
+def _not_exported(name: str):
+    def call(*_args):
+        raise RuntimeError(f"{name} is not exported by {LIB_PATH}")
+    return call
+
+
 def load() -> ct.CDLL:
-    """Load libb200sfm.so and bind every prototype (the test probe's included).  Raises if missing."""
+    """Load libb200sfm.so and bind every prototype (the test probe's included).  Raises if the library is missing, or
+    if the shipped library lacks an entry point.  A library named by B200SFM_LIB (a tuning build, another revision, a
+    host-side test double) may implement part of the ABI: an entry it does not export raises when it is called."""
     global _lib
     if _lib is not None:
         return _lib
@@ -159,7 +169,11 @@ def load() -> ct.CDLL:
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(glomap_b200 has no CPU fallback)")
     lib = ct.CDLL(LIB_PATH)
+    override = "B200SFM_LIB" in os.environ
     for name, (res, args) in PROTOTYPES.items():
+        if override and not hasattr(lib, name):
+            setattr(lib, name, _not_exported(name))
+            continue
         fn = getattr(lib, name)      # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args

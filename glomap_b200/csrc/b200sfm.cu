@@ -6,6 +6,7 @@
 #include "ba_solver.cuh"
 #include "context.cuh"
 #include "gp_solver.cuh"
+#include "pair_kernels.cuh"
 #include "ra_solver.cuh"
 #include "track_kernels.cuh"
 
@@ -568,6 +569,55 @@ int b200sfm_ba_solve(b200sfm_ctx* ctx, const b200sfm_ba_opts* opts, int32_t C, i
     if (e) cudaEventDestroy(e);
   if (stats) *stats = st;
   return rc;
+}
+
+// ---- image pair inliers ----------------------------------------------------------
+int b200sfm_image_pairs_inlier_count(b200sfm_ctx* ctx, int32_t num_images, const int64_t* feature_begin, const double* features,
+                                     const int32_t* image_intr, int32_t K, const int32_t* intr_model, const double* intr_params,
+                                     int64_t num_pairs, const int32_t* pair_image1, const int32_t* pair_image2,
+                                     const int32_t* pair_config, const double* pair_quat_xyzw, const double* pair_trans,
+                                     const double* pair_F, const double* pair_H, const int64_t* match_begin, const int32_t* matches,
+                                     double max_epipolar_error_E, double max_epipolar_error_F, double max_epipolar_error_H,
+                                     uint8_t* is_inlier, int32_t* num_inliers, double* score) {
+  if (!ctx || num_images < 0 || K < 0 || num_pairs < 0) return B200SFM_ERR_INVALID_ARG;
+  if (num_pairs == 0) return B200SFM_OK;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (!feature_begin || (num_images > 0 && !image_intr) || (K > 0 && (!intr_model || !intr_params)) || !pair_image1 ||
+      !pair_image2 || !pair_config || !pair_quat_xyzw || !pair_trans || !pair_F || !pair_H || !match_begin || !num_inliers || !score)
+    return invalid("null argument");
+  if (feature_begin[0] != 0) return invalid("feature_begin[0] must be 0");
+  for (int32_t i = 0; i < num_images; ++i)
+    if (feature_begin[i + 1] < feature_begin[i]) return invalid("feature_begin must be non-decreasing");
+  const long long nf = feature_begin[num_images];
+  if (nf > 0 && !features) return invalid("null features");
+  if (match_begin[0] != 0) return invalid("match_begin[0] must be 0");
+  std::vector<unsigned char> need(num_images, 0);   // images with features_undist: the images of a CALIBRATED pair
+  for (int64_t e = 0; e < num_pairs; ++e) {
+    if (match_begin[e + 1] < match_begin[e]) return invalid("match_begin must be non-decreasing");
+    const int32_t a = pair_image1[e], b = pair_image2[e];
+    if (a < 0 || a >= num_images || b < 0 || b >= num_images) return invalid("pair image index out of range");
+    if (pair_config[e] != B200SFM_TWO_VIEW_CALIBRATED) continue;
+    for (int32_t i : {a, b}) {
+      if (image_intr[i] < 0 || image_intr[i] >= K) return invalid("image_intr index out of range");
+      const int32_t m = intr_model[image_intr[i]];
+      if (m < B200SFM_SIMPLE_PINHOLE || m > B200SFM_RADIAL) {
+        ctx->err = "camera model " + std::to_string(m) + " of a CALIBRATED pair is not supported";
+        return B200SFM_ERR_UNSUPPORTED;
+      }
+      need[i] = 1;
+    }
+  }
+  const long long M = match_begin[num_pairs];
+  if (M > 0 && (!matches || !is_inlier)) return invalid("null matches / is_inlier");
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    if (!b200::image_pairs_inlier_count(ctx, num_images, nf, feature_begin, features, image_intr, K, intr_model, intr_params, num_pairs,
+                                        pair_image1, pair_image2, pair_config, pair_quat_xyzw, pair_trans, pair_F, pair_H, match_begin,
+                                        matches, max_epipolar_error_E, max_epipolar_error_F, max_epipolar_error_H, need.data(), is_inlier,
+                                        num_inliers, score))
+      throw b200::InvalidInput{"match feature index out of range of its image"};
+    return (int)B200SFM_OK;
+  });
 }
 
 // ---- track establishment ----------------------------------------------------------

@@ -86,17 +86,9 @@ __global__ void proc_scale_shift3(long long n, double scale, double t0, double t
   y[3 * i + 2] = scale * y[3 * i + 2] + t2;
 }
 
-// unit bearing of every observation (caller's point-order indexing), from the CURRENT intrinsics
-__global__ void proc_undistort(long long N, int S, const int* __restrict__ obs_cam, const unsigned short* __restrict__ obs_sensor,
-                               const int* __restrict__ cam_intr, const int* __restrict__ sensor_intr,
-                               const int* __restrict__ intr_model, const double* __restrict__ intr /*[K][12]*/,
-                               const double2* __restrict__ obs_xy, double* __restrict__ out) {
-  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= N) return;
-  const int blk = S > 0 ? sensor_intr[obs_sensor[o]] : cam_intr[obs_cam[o]];
-  const double* p = intr + (size_t)blk * 12;
-  const int m = intr_model[blk];
-  const double2 xy = obs_xy[o];
+// CamFromImg(xy).homogeneous().normalized() of one pixel for camera model m (0-3) with parameters p; writes out[0..2].
+// Shared by UndistortImages below and the per-feature bearings of ImagePairsInlierCount (pair_kernels.cuh).
+__device__ __forceinline__ void bearing_from_pixel(int m, const double* __restrict__ p, double2 xy, double* __restrict__ out) {
   double u, v;
   if (m == 0) {          // SIMPLE_PINHOLE f cx cy
     u = (xy.x - p[1]) / p[0]; v = (xy.y - p[2]) / p[0];
@@ -113,9 +105,20 @@ __global__ void proc_undistort(long long N, int S, const int* __restrict__ obs_c
     }
   }
   const double inv = 1.0 / sqrt(u * u + v * v + 1.0);
-  out[3 * o] = u * inv;
-  out[3 * o + 1] = v * inv;
-  out[3 * o + 2] = inv;
+  out[0] = u * inv;
+  out[1] = v * inv;
+  out[2] = inv;
+}
+
+// unit bearing of every observation (caller's point-order indexing), from the CURRENT intrinsics
+__global__ void proc_undistort(long long N, int S, const int* __restrict__ obs_cam, const unsigned short* __restrict__ obs_sensor,
+                               const int* __restrict__ cam_intr, const int* __restrict__ sensor_intr,
+                               const int* __restrict__ intr_model, const double* __restrict__ intr /*[K][12]*/,
+                               const double2* __restrict__ obs_xy, double* __restrict__ out) {
+  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= N) return;
+  const int blk = S > 0 ? sensor_intr[obs_sensor[o]] : cam_intr[obs_cam[o]];
+  bearing_from_pixel(intr_model[blk], intr + (size_t)blk * 12, obs_xy[o], out + 3 * o);
 }
 
 }  // namespace b200

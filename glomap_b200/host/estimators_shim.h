@@ -22,6 +22,7 @@
 #include <set>
 #include <random>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/b200sfm.h"
@@ -803,6 +804,105 @@ class RotationEstimator {
 
  private:
   const RotationEstimatorOptions& options_;   // the reference stores a const& too (.h:140)
+};
+
+// ---------------------------------------------------------------------------
+struct InlierThresholdOptions {   // glomap/types.h:18-32
+  double max_angle_error = 1.;
+  double max_reprojection_error = 1e-2;
+  double min_triangulation_angle = 1.;
+  double max_epipolar_error_E = 1.;
+  double max_epipolar_error_F = 4.;
+  double max_epipolar_error_H = 4.;
+  double min_inlier_num = 30;
+  double min_inlier_ratio = 0.25;
+  double max_rotation_error = 10.;
+};
+
+// ImagePairsInlierCount (processors/image_pair_inliers.cc:200-213) on the device: the pairs whose inliers are cleared
+// (all, or with clean_inliers = false only those without inliers) and of those the valid ones are scored.  Images,
+// cameras and pairs are flattened in sorted-id order; ImagePair::inliers is rewritten in ascending row order.
+// A template over the view graph and the options so that, inside a glomap build, the caller's own
+// glomap::InlierThresholdOptions (glomap/types.h, not an estimator header the shim replaces) is accepted as it is.
+template <class ViewGraphT, class InlierOptions>
+void ImagePairsInlierCount(ViewGraphT& view_graph, const std::unordered_map<camera_t, Camera>& cameras,
+                           const std::unordered_map<image_t, Image>& images, const InlierOptions& options, bool clean_inliers) {
+  using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
+  std::map<image_pair_t, Pair*> psorted;
+  for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
+  std::vector<Pair*> scored;
+  for (auto& [id, pr] : psorted) {
+    if (!clean_inliers && pr->inliers.size() > 0) continue;
+    pr->inliers.clear();
+    if (pr->is_valid) scored.push_back(pr);
+  }
+  if (scored.empty()) return;
+  b200sfm_ctx* ctx = DefaultContext();
+  if (!ctx) return;
+  std::map<camera_t, int> cidx;
+  for (auto& [id, c] : cameras) cidx[id] = 0;
+  std::vector<int32_t> intr_model;
+  std::vector<double> intr(cidx.size() * B200SFM_INTR_STRIDE, 0.0);
+  for (auto& [id, k] : cidx) {
+    k = (int)intr_model.size();
+    const Camera& c = cameras.at(id);
+    intr_model.push_back(static_cast<int32_t>(c.model_id));
+    for (size_t j = 0; j < c.params.size() && j < B200SFM_INTR_STRIDE; ++j) intr[(size_t)k * B200SFM_INTR_STRIDE + j] = c.params[j];
+  }
+  std::map<image_t, const Image*> isorted;
+  for (auto& [id, im] : images) isorted[id] = &im;
+  std::map<image_t, int> iidx;
+  std::vector<int64_t> feature_begin(1, 0);
+  std::vector<double> features;
+  std::vector<int32_t> image_intr;
+  for (auto& [id, im] : isorted) {
+    iidx[id] = (int)image_intr.size();
+    auto c = cidx.find(im->camera_id);
+    image_intr.push_back(c == cidx.end() ? -1 : c->second);
+    for (const auto& f : im->features) { features.push_back(f[0]); features.push_back(f[1]); }
+    feature_begin.push_back((int64_t)features.size() / 2);
+  }
+  const int64_t E = (int64_t)scored.size();
+  std::vector<int32_t> img1, img2, config, matches;
+  std::vector<double> quat, trans, F, H;
+  std::vector<int64_t> match_begin(1, 0);
+  for (Pair* pr : scored) {
+    auto a = iidx.find(pr->image_id1), b = iidx.find(pr->image_id2);
+    if (a == iidx.end() || b == iidx.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return; }
+    img1.push_back(a->second); img2.push_back(b->second); config.push_back(pr->config);
+    for (int k = 0; k < 4; ++k) quat.push_back(pr->cam2_from_cam1.rotation.coeffs().data()[k]);
+    for (int k = 0; k < 3; ++k) trans.push_back(pr->cam2_from_cam1.translation[k]);
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) { F.push_back(pr->F(r, c)); H.push_back(pr->H(r, c)); }
+    for (long k = 0; k < (long)pr->matches.rows(); ++k) { matches.push_back(pr->matches(k, 0)); matches.push_back(pr->matches(k, 1)); }
+    match_begin.push_back((int64_t)matches.size() / 2);
+  }
+  std::vector<uint8_t> is_inlier(match_begin.back());
+  std::vector<int32_t> num_inliers(E);
+  std::vector<double> score(E);
+  const int rc = b200sfm_image_pairs_inlier_count(
+      ctx, (int32_t)image_intr.size(), feature_begin.data(), features.data(), image_intr.data(), (int32_t)intr_model.size(),
+      intr_model.data(), intr.data(), E, img1.data(), img2.data(), config.data(), quat.data(), trans.data(), F.data(), H.data(),
+      match_begin.data(), matches.data(), options.max_epipolar_error_E, options.max_epipolar_error_F, options.max_epipolar_error_H,
+      is_inlier.data(), num_inliers.data(), score.data());
+  if (rc != B200SFM_OK) { std::fprintf(stderr, "b200sfm: ImagePairsInlierCount failed: %s\n", b200sfm_last_error(ctx)); return; }
+  for (int64_t e = 0; e < E; ++e)
+    for (int64_t k = match_begin[e]; k < match_begin[e + 1]; ++k)
+      if (is_inlier[k]) scored[e]->inliers.push_back((int)(k - match_begin[e]));
+}
+
+// processors/relpose_filter.{h,cc}: the two inlier filters the mapper runs after ImagePairsInlierCount (global_mapper.cc:67-70)
+struct RelPoseFilter {
+  template <class ViewGraphT>
+  static void FilterInlierNum(ViewGraphT& view_graph, int min_inlier_num) {   // relpose_filter.cc:35-48
+    for (auto& [id, pr] : view_graph.image_pairs)
+      if (pr.is_valid && pr.inliers.size() < (size_t)min_inlier_num) pr.is_valid = false;   // size_t comparison as in the reference
+  }
+  template <class ViewGraphT>
+  static void FilterInlierRatio(ViewGraphT& view_graph, double min_inlier_ratio) {   // relpose_filter.cc:50-65
+    for (auto& [id, pr] : view_graph.image_pairs)   // 0 matches: NaN, not below the threshold -- the pair stays valid
+      if (pr.is_valid && pr.inliers.size() / double(pr.matches.rows()) < min_inlier_ratio) pr.is_valid = false;
+  }
 };
 
 }  // namespace b200sfm_shim

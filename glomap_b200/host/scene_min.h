@@ -130,12 +130,24 @@ struct Track {
   std::vector<std::pair<image_t, feature_t>> observations;
   bool is_initialized = false;
 };
+struct Matrix3 {   // Eigen::Matrix3d: the shim reads M(r, c)
+  double m[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  double operator()(int r, int c) const { return m[3 * r + c]; }
+};
+struct MatchMatrix {   // Eigen::MatrixXi with two columns: (k, 0) feature in image 1, (k, 1) feature in image 2
+  std::vector<std::array<int, 2>> rows_;
+  long rows() const { return (long)rows_.size(); }
+  int operator()(long r, int c) const { return rows_[r][c]; }
+};
 struct ImagePair {
   image_t image_id1 = 0, image_id2 = 0;
   bool is_valid = true;
   double weight = -1;
   std::vector<int> inliers;                      // scene/image_pair.h: indices of the inlier matches
   Rigid3d cam2_from_cam1;
+  int config = 0;                                // colmap::TwoViewGeometry::ConfigurationType
+  Matrix3 F, H;
+  MatchMatrix matches;
 };
 struct ViewGraph {
   std::unordered_map<image_pair_t, ImagePair> image_pairs;

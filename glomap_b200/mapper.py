@@ -24,6 +24,12 @@ class InlierThresholdOptions:
     max_reprojection_error: float = 1e-2    # normalised image plane, bundle adjustment
     min_triangulation_angle: float = 1.0    # degrees
     max_rotation_error: float = 10.0        # degrees, rotation averaging
+    # image pairs (image_pair_inliers.py)
+    max_epipolar_error_E: float = 1.0       # pixels, converted with the mean focal of the two cameras
+    max_epipolar_error_F: float = 4.0       # pixels
+    max_epipolar_error_H: float = 4.0       # pixels
+    min_inlier_num: float = 30              # RelPoseFilter::FilterInlierNum (takes it as an int)
+    min_inlier_ratio: float = 0.25          # RelPoseFilter::FilterInlierRatio
 
 
 @dataclasses.dataclass

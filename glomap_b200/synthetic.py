@@ -375,23 +375,25 @@ def bearings_from_scene(scene: Scene) -> np.ndarray:
         mk = ci == k
         if not mk.any():
             continue
-        m = int(scene.intr_model[k])
-        p = scene.intr_params[k]
-        xy = scene.obs_xy[mk]
-        if m == SIMPLE_PINHOLE:
-            u, v = (xy[:, 0] - p[1]) / p[0], (xy[:, 1] - p[2]) / p[0]
-        elif m == PINHOLE:
-            u, v = (xy[:, 0] - p[2]) / p[0], (xy[:, 1] - p[3]) / p[1]
-        else:
-            ud, vd = (xy[:, 0] - p[1]) / p[0], (xy[:, 1] - p[2]) / p[0]
-            u, v = ud.copy(), vd.copy()
-            for _ in range(50):
-                r2 = u * u + v * v
-                dd = 1 + p[3] * r2 + (p[4] * r2 * r2 if m == RADIAL else 0.0)
-                u, v = ud / dd, vd / dd
-        b = np.stack([u, v, np.ones_like(u)], 1)
-        out[mk] = b / np.linalg.norm(b, axis=1, keepdims=True)
+        out[mk] = bearings_from_pixels(int(scene.intr_model[k]), scene.intr_params[k], scene.obs_xy[mk])
     return out
+
+
+def bearings_from_pixels(m: int, p: np.ndarray, xy: np.ndarray) -> np.ndarray:
+    """``CamFromImg(xy).homogeneous().normalized()`` of [n,2] pixels of one camera (model ``m``, parameters ``p``)."""
+    if m == SIMPLE_PINHOLE:
+        u, v = (xy[:, 0] - p[1]) / p[0], (xy[:, 1] - p[2]) / p[0]
+    elif m == PINHOLE:
+        u, v = (xy[:, 0] - p[2]) / p[0], (xy[:, 1] - p[3]) / p[1]
+    else:
+        ud, vd = (xy[:, 0] - p[1]) / p[0], (xy[:, 1] - p[2]) / p[0]
+        u, v = ud.copy(), vd.copy()
+        for _ in range(50):
+            r2 = u * u + v * v
+            dd = 1 + p[3] * r2 + (p[4] * r2 * r2 if m == RADIAL else 0.0)
+            u, v = ud / dd, vd / dd
+    b = np.stack([u, v, np.ones_like(u)], 1)
+    return b / np.linalg.norm(b, axis=1, keepdims=True)
 
 
 # ---------------------------------------------------------------------------
@@ -584,3 +586,117 @@ def read_flat_problem(path: str) -> Scene:
         trans = np.fromfile(f, np.float64, 3 * C).reshape(C, 3)
         pts = np.fromfile(f, np.float64, 3 * P).reshape(P, 3)
     return Scene(quat, trans, pts, ptb, cam, xy, ci, im, intr)
+
+
+# ---------------------------------------------------------------------------
+# Image pairs with matches (input of ImagePairsInlierCount)
+# ---------------------------------------------------------------------------
+def _pinhole_K(model: int, p: np.ndarray) -> np.ndarray:
+    fx, fy, cx, cy = (p[0], p[1], p[2], p[3]) if model == PINHOLE else (p[0], p[0], p[1], p[2])
+    return np.array([[fx, 0.0, cx], [0.0, fy, cy], [0.0, 0.0, 1.0]])
+
+
+def _fit_homography(x1: np.ndarray, x2: np.ndarray) -> np.ndarray:
+    """Least-squares homography x2 ~ H x1 (normalised DLT)."""
+    def norm(x):
+        c = x.mean(0)
+        s = np.sqrt(2.0) / max(np.linalg.norm(x - c, axis=1).mean(), 1e-12)
+        return np.array([[s, 0, -s * c[0]], [0, s, -s * c[1]], [0, 0, 1.0]])
+    T1, T2 = norm(x1), norm(x2)
+    a = x1 @ T1[:2, :2].T + T1[:2, 2]
+    b = x2 @ T2[:2, :2].T + T2[:2, 2]
+    z, o = np.zeros(len(a)), np.ones(len(a))
+    A = np.concatenate([np.stack([a[:, 0], a[:, 1], o, z, z, z, -b[:, 0] * a[:, 0], -b[:, 0] * a[:, 1], -b[:, 0]], 1),
+                        np.stack([z, z, z, a[:, 0], a[:, 1], o, -b[:, 1] * a[:, 0], -b[:, 1] * a[:, 1], -b[:, 1]], 1)])
+    Hn = np.linalg.svd(A)[2][-1].reshape(3, 3)
+    H = np.linalg.inv(T2) @ Hn @ T1
+    return H / H[2, 2]
+
+
+def make_pair_matches(scene: Scene, seed: int = 1, outlier_frac: float = 0.2, config_weights=(0.8, 0.15, 0.05)) -> dict:
+    """Flat image-pair match set from the tracks of ``scene``: feature f of image i is the f-th observation of camera i
+    (in observation order); every pair of observations inside a track is a match of the pair (i < j) of their cameras;
+    ``outlier_frac`` of the final matches are random feature pairs of the same image pairs.  Each pair is CALIBRATED,
+    UNCALIBRATED or PLANAR with the probabilities ``config_weights`` and carries the true cam2_from_cam1 (unit
+    translation), the F of the
+    pinhole part of the two cameras and, for PLANAR pairs, the least-squares homography of its true matches (the infinite
+    homography K2 R K1^-1 when it has fewer than 4).  Arrays (the layout of
+    b200sfm_image_pairs_inlier_count): feature_begin [C+1], features [nf,2], image_intr [C], intr_model, intr_params,
+    img1/img2/config [E], quat [E,4], trans [E,3], F/H [E,9], match_begin [E+1], matches [M,2] int32, is_true [M]."""
+    rng = np.random.default_rng([seed, 77])
+    C = scene.C
+    counts = np.bincount(scene.obs_cam, minlength=C)
+    feature_begin = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64)
+    order = np.argsort(scene.obs_cam, kind="stable")
+    feat_of_obs = np.empty(scene.N, np.int64)
+    feat_of_obs[order] = np.arange(scene.N) - feature_begin[scene.obs_cam[order]]
+    lens = np.diff(scene.pt_obs_begin)
+    us, vs = [], []
+    for L in np.unique(lens[lens >= 2]):
+        starts = scene.pt_obs_begin[:-1][lens == L]
+        a, b = np.triu_indices(int(L), 1)
+        us.append((starts[:, None] + a[None, :]).ravel())
+        vs.append((starts[:, None] + b[None, :]).ravel())
+    u, v = np.concatenate(us), np.concatenate(vs)
+    ci, cj = scene.obs_cam[u].astype(np.int64), scene.obs_cam[v].astype(np.int64)
+    fu, fv = feat_of_obs[u], feat_of_obs[v]
+    swap = ci > cj
+    ci, cj, fu, fv = np.where(swap, cj, ci), np.where(swap, ci, cj), np.where(swap, fv, fu), np.where(swap, fu, fv)
+    del u, v, swap
+    n_out = int(round(len(ci) * outlier_frac / (1.0 - outlier_frac)))
+    src = rng.integers(0, len(ci), n_out)
+    oi, oj = ci[src], cj[src]
+    of1 = (rng.random(n_out) * counts[oi]).astype(np.int64)
+    of2 = (rng.random(n_out) * counts[oj]).astype(np.int64)
+    is_true = np.concatenate([np.ones(len(ci), bool), np.zeros(n_out, bool)])
+    key = np.concatenate([ci * C + cj, oi * C + oj])
+    f1, f2 = np.concatenate([fu, of1]), np.concatenate([fv, of2])
+    del ci, cj, fu, fv, oi, oj, of1, of2, src
+    perm = np.lexsort((rng.random(len(key)), key))             # by pair; true and outlier matches interleaved
+    key, is_true = key[perm], is_true[perm]
+    matches = np.stack([f1[perm], f2[perm]], 1).astype(np.int32)
+    del f1, f2, perm
+    heads = np.concatenate([[0], np.nonzero(np.diff(key))[0] + 1]) if len(key) else np.zeros(0, np.int64)
+    match_begin = np.concatenate([heads, [len(key)]]).astype(np.int64)
+    img1, img2 = (key[heads] // C).astype(np.int32), (key[heads] % C).astype(np.int32)
+    E = len(heads)
+    config = rng.choice(np.array([2, 3, 4], np.int32), size=E, p=np.asarray(config_weights, float) / np.sum(config_weights))
+    R = geo.quat_xyzw_to_rotmat(scene.quat)
+    R_rel = R[img2] @ np.swapaxes(R[img1], -1, -2)
+    t_rel = scene.trans[img2] - np.einsum("nij,nj->ni", R_rel, scene.trans[img1])
+    t_rel /= np.linalg.norm(t_rel, axis=1, keepdims=True)     # unit baseline, as relative pose estimation returns it
+    Kinv = np.array([np.linalg.inv(_pinhole_K(int(m), p)) for m, p in zip(scene.intr_model, scene.intr_params)])
+    Kb = np.array([_pinhole_K(int(m), p) for m, p in zip(scene.intr_model, scene.intr_params)])
+    K1i, K2i = Kinv[scene.cam_intr[img1]], Kinv[scene.cam_intr[img2]]
+    tx = np.zeros((E, 3, 3))
+    tx[:, 0, 1], tx[:, 0, 2], tx[:, 1, 2] = -t_rel[:, 2], t_rel[:, 1], -t_rel[:, 0]
+    tx[:, 1, 0], tx[:, 2, 0], tx[:, 2, 1] = t_rel[:, 2], -t_rel[:, 1], t_rel[:, 0]
+    F = np.swapaxes(K2i, -1, -2) @ tx @ R_rel @ K1i
+    F /= np.linalg.norm(F.reshape(E, 9), axis=1)[:, None, None]
+    H = Kb[scene.cam_intr[img2]] @ R_rel @ K1i
+    feats = scene.obs_xy[order]
+    for e in np.nonzero(config == 4)[0]:     # PLANAR: the DLT homography of the pair's true matches, where there are 4
+        m = matches[match_begin[e]:match_begin[e + 1]][is_true[match_begin[e]:match_begin[e + 1]]]
+        if len(m) >= 4:
+            H[e] = _fit_homography(feats[feature_begin[img1[e]] + m[:, 0]], feats[feature_begin[img2[e]] + m[:, 1]])
+    return dict(feature_begin=feature_begin, features=np.ascontiguousarray(scene.obs_xy[order]),
+                image_intr=scene.cam_intr.astype(np.int32), intr_model=scene.intr_model.astype(np.int32),
+                intr_params=scene.intr_params, img1=img1, img2=img2, config=config.astype(np.int32),
+                quat=geo.rotmat_to_quat_xyzw_fast(R_rel), trans=t_rel, F=F.reshape(E, 9), H=H.reshape(E, 9),
+                match_begin=match_begin, matches=matches, is_true=is_true)
+
+
+def pairs_from_match_arrays(d: dict):
+    """(features, cameras, pairs) of ``make_pair_matches`` arrays for the object-level API (image_pair_inliers.py): image
+    ids are the camera indices, every image has its own camera object, pairs carry no inliers."""
+    from .image_pair_inliers import Camera
+    from .track_establishment import ImagePairMatches
+    C = len(d["image_intr"])
+    fb = d["feature_begin"]
+    features = {i: d["features"][fb[i]:fb[i + 1]] for i in range(C)}
+    cameras = {i: Camera(int(d["intr_model"][d["image_intr"][i]]), d["intr_params"][d["image_intr"][i]]) for i in range(C)}
+    mb = d["match_begin"]
+    pairs = [ImagePairMatches(int(d["img1"][e]), int(d["img2"][e]), d["matches"][mb[e]:mb[e + 1]], np.zeros(0, np.int64),
+                              config=int(d["config"][e]), quat_xyzw=d["quat"][e], trans=d["trans"][e],
+                              F=d["F"][e].reshape(3, 3), H=d["H"][e].reshape(3, 3)) for e in range(len(d["img1"]))]
+    return features, cameras, pairs

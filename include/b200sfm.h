@@ -254,6 +254,46 @@ int b200sfm_tracks_get(b200sfm_tracks* t, uint64_t* track_ids /*[T]*/, int64_t* 
                        uint32_t* obs_feature /*[n]*/);
 void b200sfm_tracks_free(b200sfm_tracks* t);
 
+/* ---- image pair inliers ------------------------------------------------------------------------------------------------
+ * ImagePairsInlierCount (glomap/processors/image_pair_inliers.cc:200-213), the scorers ScoreErrorEssential / Fundamental /
+ * Homography (:20-198) and the two-view arithmetic they call (glomap/math/two_view_geometry.cc:5-93), run by
+ * GlobalMapper::Solve after the relative poses (controllers/global_mapper.cc:64-65).  Every pair passed in is scored by
+ * its config: PLANAR / PANORAMIC / PLANAR_OR_PANORAMIC against H (max_epipolar_error_H px), UNCALIBRATED against F
+ * (max_epipolar_error_F px, orientation-signum majority), CALIBRATED against E = [t]x R of cam2_from_cam1 on the unit
+ * bearings of the features (features_undist; computed here once per feature from the image's camera, as UndistortImages
+ * does), with threshold max_epipolar_error_E * (1/f1 + 1/f2) / 2, cheirality and the 3-degree epipole cones; any other
+ * config gives no inliers.  The caller selects the pairs (valid pairs, minus those it keeps under clean_inliers = false).
+ *   feature_begin [I+1]   CSR over the features of the I images (int64); features [nf][2] distorted pixels
+ *   image_intr [I]        camera block of each image; intr_model [K] / intr_params [K][B200SFM_INTR_STRIDE] -- only the
+ *                         cameras of CALIBRATED pairs are read (models 0-3, else B200SFM_ERR_UNSUPPORTED)
+ *   pair_image1/2 [E]     image indices; pair_config [E] b200sfm_two_view_config; pair_quat_xyzw [E][4] / pair_trans [E][3]
+ *                         cam2_from_cam1; pair_F / pair_H [E][9] row-major
+ *   match_begin [E+1]     CSR over matches [M][2] (feature index in image 1, in image 2); an index outside its image's
+ *                         features gives B200SFM_ERR_INVALID_ARG (checked on the device, never dereferenced)
+ *   is_inlier [M]         1 = inlier (ImagePair::inliers are its set rows in ascending order); num_inliers [E]; score [E]
+ *                         the scorer's return value (the reference's caller discards it).
+ * num_pairs == 0 returns B200SFM_OK and writes nothing.  No collectives: on a distributed context each rank scores the
+ * pairs it is given. */
+/* colmap::TwoViewGeometry::ConfigurationType (colmap/estimators/two_view_geometry.h, un-vendored; UPSTREAM-UNVERIFIED) */
+typedef enum {
+  B200SFM_TWO_VIEW_UNDEFINED = 0,
+  B200SFM_TWO_VIEW_DEGENERATE = 1,
+  B200SFM_TWO_VIEW_CALIBRATED = 2,
+  B200SFM_TWO_VIEW_UNCALIBRATED = 3,
+  B200SFM_TWO_VIEW_PLANAR = 4,
+  B200SFM_TWO_VIEW_PANORAMIC = 5,
+  B200SFM_TWO_VIEW_PLANAR_OR_PANORAMIC = 6,
+  B200SFM_TWO_VIEW_WATERMARK = 7,
+  B200SFM_TWO_VIEW_MULTIPLE = 8
+} b200sfm_two_view_config;
+int b200sfm_image_pairs_inlier_count(b200sfm_ctx* ctx, int32_t num_images, const int64_t* feature_begin, const double* features,
+                                     const int32_t* image_intr, int32_t K, const int32_t* intr_model, const double* intr_params,
+                                     int64_t num_pairs, const int32_t* pair_image1, const int32_t* pair_image2,
+                                     const int32_t* pair_config, const double* pair_quat_xyzw, const double* pair_trans,
+                                     const double* pair_F, const double* pair_H, const int64_t* match_begin, const int32_t* matches,
+                                     double max_epipolar_error_E, double max_epipolar_error_F, double max_epipolar_error_H,
+                                     uint8_t* is_inlier, int32_t* num_inliers, double* score);
+
 /* ---- (ii) global positioning (BATA) ----------------------------------------- */
 /* Mirror of GlobalPositionerOptions (global_positioning.h:9-54) + inherited
  * solver options (optimization_base.h:18-23) + PCG knobs.  Only the
