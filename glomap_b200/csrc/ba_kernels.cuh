@@ -87,34 +87,75 @@ __device__ __forceinline__ void huber(double s, double a, double& rho0, double& 
   }
 }
 
-// Pixel projection with the generic radial form (pinhole models have k = 0,
-// simple models fx = fy).  J = d(px,py)/d(Xc) row-major 2x3.
-__device__ __forceinline__ void project_jac(const double* __restrict__ ir, double x, double y, double z, double& px,
-                                            double& py, double J[6]) {
+// Values of an intrinsics record (fx fy cx cy k1 k2 model).  The camera-order kernels load it once per segment.
+struct Intr {
+  double fx, fy, cx, cy, k1, k2;
+  int model;
+};
+__device__ __forceinline__ Intr ld_intr(const double* __restrict__ ir) {
+  return Intr{ir[0], ir[1], ir[2], ir[3], ir[4], ir[5], (int)ir[6]};
+}
+
+// Projection Jacobian in factored form:  d(px,py)/d(Xc) = iz M [I | -(u, v)^T],  M = d(pixel)/d(u, v)  (2x2;
+// diag(fx, fy) for the pinhole models).
+struct ProjJac {
+  double iz, u, v, m00, m01, m10, m11;
+};
+
+// Pixel projection.  Records with k1 == k2 == 0 (SIMPLE_PINHOLE, PINHOLE) take the pinhole form; the others the
+// generic radial form (simple models have fx = fy).  project_only computes the pixel with the same instructions.
+__device__ __forceinline__ void project_jac(const Intr& in, double x, double y, double z, double& px, double& py,
+                                            ProjJac& pj) {
   const double iz = 1.0 / z;
   const double u = x * iz, v = y * iz;
-  const double fx = ir[0], fy = ir[1], cx = ir[2], cy = ir[3], k1 = ir[4], k2 = ir[5];
-  const double r2 = u * u + v * v;
-  const double d = 1.0 + r2 * (k1 + k2 * r2);
-  const double dd = k1 + 2.0 * k2 * r2;
-  px = fx * u * d + cx;
-  py = fy * v * d + cy;
-  const double a00 = d + 2.0 * u * u * dd, a01 = 2.0 * u * v * dd, a11 = d + 2.0 * v * v * dd;
-  J[0] = fx * a00 * iz;
-  J[1] = fx * a01 * iz;
-  J[2] = -fx * iz * (a00 * u + a01 * v);
-  J[3] = fy * a01 * iz;
-  J[4] = fy * a11 * iz;
-  J[5] = -fy * iz * (a01 * u + a11 * v);
+  pj.iz = iz;
+  pj.u = u;
+  pj.v = v;
+  if (in.k1 == 0.0 && in.k2 == 0.0) {
+    px = in.fx * u + in.cx;
+    py = in.fy * v + in.cy;
+    pj.m00 = in.fx; pj.m01 = 0.0; pj.m10 = 0.0; pj.m11 = in.fy;
+  } else {
+    const double r2 = u * u + v * v;
+    const double d = 1.0 + r2 * (in.k1 + in.k2 * r2);
+    const double dd = in.k1 + 2.0 * in.k2 * r2;
+    px = in.fx * u * d + in.cx;
+    py = in.fy * v * d + in.cy;
+    const double a00 = d + 2.0 * u * u * dd, a01 = 2.0 * u * v * dd, a11 = d + 2.0 * v * v * dd;
+    pj.m00 = in.fx * a00; pj.m01 = in.fx * a01; pj.m10 = in.fy * a01; pj.m11 = in.fy * a11;
+  }
+}
+__device__ __forceinline__ void project_only(const Intr& in, double x, double y, double z, double& px, double& py) {
+  const double iz = 1.0 / z;
+  const double u = x * iz, v = y * iz;
+  if (in.k1 == 0.0 && in.k2 == 0.0) {
+    px = in.fx * u + in.cx;
+    py = in.fy * v + in.cy;
+  } else {
+    const double r2 = u * u + v * v;
+    const double d = 1.0 + r2 * (in.k1 + in.k2 * r2);
+    px = in.fx * u * d + in.cx;
+    py = in.fy * v * d + in.cy;
+  }
+}
+// J = d(px,py)/d(Xc) row-major 2x3 from the factored form
+__device__ __forceinline__ void proj_jac_rows(const ProjJac& pj, double J[6]) {
+  J[0] = pj.m00 * pj.iz;
+  J[1] = pj.m01 * pj.iz;
+  J[2] = -(J[0] * pj.u + J[1] * pj.v);
+  J[3] = pj.m10 * pj.iz;
+  J[4] = pj.m11 * pj.iz;
+  J[5] = -(J[3] * pj.u + J[4] * pj.v);
+}
+__device__ __forceinline__ void project_jac(const double* __restrict__ ir, double x, double y, double z, double& px,
+                                            double& py, double J[6]) {
+  ProjJac pj;
+  project_jac(ld_intr(ir), x, y, z, px, py, pj);
+  proj_jac_rows(pj, J);
 }
 __device__ __forceinline__ void project_only(const double* __restrict__ ir, double x, double y, double z, double& px,
                                              double& py) {
-  const double iz = 1.0 / z;
-  const double u = x * iz, v = y * iz;
-  const double r2 = u * u + v * v;
-  const double d = 1.0 + r2 * (ir[4] + ir[5] * r2);
-  px = ir[0] * u * d + ir[2];
-  py = ir[1] * v * d + ir[3];
+  project_only(ld_intr(ir), x, y, z, px, py);
 }
 
 // Everything one observation contributes.  Jc = [Jrot(2x3) | Jtrn(2x3)] and
@@ -217,16 +258,19 @@ __device__ __forceinline__ void linearize_obs(const double4& q4, const double4& 
 //   e   = pixel residual, rho0 = rho(|e|^2), rho1 = rho'(|e|^2)  (Huber; corrector with rho'' <= 0 => rows * sqrt(rho'))
 //   RX  = R X (the rotated point, for the rotation block), R = R(q)
 // valid == false (point behind the camera): the observation contributes nothing (ObsLin convention).
+//   pj  = the factored projection Jacobian (camera-order kernels work with it in the camera frame; J is then dead code)
 struct ObsCore {
   double J[6], e[2], rho0, rho1, RX[3], R[9];
   double uv[2];   // normalised image coordinates (only read by the intrinsics rows: dead code elsewhere)
+  ProjJac pj;
   bool valid;
 };
-__device__ __forceinline__ void obs_core(const double4& q4, const double4& t4, const double* __restrict__ ir,
-                                         const double* __restrict__ sr, double X0, double X1, double X2, double2 xy,
-                                         double huber_a, ObsCore& o) {
-  const double q[4] = {q4.x, q4.y, q4.z, q4.w};
-  quat_to_R(q, o.R);
+// R = R(q) of the camera (frame) record, computed by the caller (once per segment in camera order)
+__device__ __forceinline__ void obs_core_R(const double R[9], const double4& t4, const Intr& in,
+                                           const double* __restrict__ sr, double X0, double X1, double X2, double2 xy,
+                                           double huber_a, ObsCore& o) {
+#pragma unroll
+  for (int k = 0; k < 9; ++k) o.R[k] = R[k];
   o.RX[0] = o.R[0] * X0 + o.R[1] * X1 + o.R[2] * X2;
   o.RX[1] = o.R[3] * X0 + o.R[4] * X1 + o.R[5] * X2;
   o.RX[2] = o.R[6] * X0 + o.R[7] * X1 + o.R[8] * X2;
@@ -240,10 +284,12 @@ __device__ __forceinline__ void obs_core(const double4& q4, const double4& t4, c
     o.rho0 = 0.0;
     o.rho1 = 0.0;
     o.uv[0] = o.uv[1] = 0.0;
+    o.pj = ProjJac{0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     return;
   }
   double px, py;
-  project_jac(ir, xc, yc, zc, px, py, o.J);
+  project_jac(in, xc, yc, zc, px, py, o.pj);
+  proj_jac_rows(o.pj, o.J);
   o.uv[0] = xc / zc;
   o.uv[1] = yc / zc;
   if (sr) {   // chain through the constant cam_from_rig rotation: J <- J R_cr
@@ -267,6 +313,14 @@ __device__ __forceinline__ void obs_core(const double4& q4, const double4& t4, c
     o.rho0 = s;
     o.rho1 = 1.0;
   }
+}
+__device__ __forceinline__ void obs_core(const double4& q4, const double4& t4, const double* __restrict__ ir,
+                                         const double* __restrict__ sr, double X0, double X1, double X2, double2 xy,
+                                         double huber_a, ObsCore& o) {
+  const double q[4] = {q4.x, q4.y, q4.z, q4.w};
+  double R[9];
+  quat_to_R(q, R);
+  obs_core_R(R, t4, ld_intr(ir), sr, X0, X1, X2, xy, huber_a, o);
 }
 // point block J_pt = J R (2x3, unscaled) -> A = rho' J_pt^T J_pt (packed symmetric), b = rho' J_pt^T e
 __device__ __forceinline__ void obs_point_blocks(const ObsCore& o, double Jp[6], double A[6], double b[3]) {
@@ -1031,14 +1085,13 @@ struct IntrVarRec {   // per intrinsics block
 };
 
 // d(px,py)/d(param pidx), scaled by w = sqrt(rho')
-__device__ __forceinline__ void intr_param_jac(const double* __restrict__ ir, int pidx, double u, double v, double w,
+__device__ __forceinline__ void intr_param_jac(const Intr& in, int pidx, double u, double v, double w,
                                                double& jx, double& jy) {
-  const int model = (int)ir[6];
   const double r2 = u * u + v * v;
-  const double d = 1.0 + r2 * (ir[4] + ir[5] * r2);
+  const double d = 1.0 + r2 * (in.k1 + in.k2 * r2);
   jx = 0.0;
   jy = 0.0;
-  if (model == 1) {                       // PINHOLE fx fy cx cy
+  if (in.model == 1) {                    // PINHOLE fx fy cx cy
     if (pidx == 0) jx = u;
     else if (pidx == 1) jy = v;
     else if (pidx == 2) jx = 1.0;
@@ -1047,8 +1100,8 @@ __device__ __forceinline__ void intr_param_jac(const double* __restrict__ ir, in
     if (pidx == 0) { jx = u * d; jy = v * d; }
     else if (pidx == 1) jx = 1.0;
     else if (pidx == 2) jy = 1.0;
-    else if (pidx == 3) { jx = ir[0] * u * r2; jy = ir[1] * v * r2; }
-    else { jx = ir[0] * u * r2 * r2; jy = ir[1] * v * r2 * r2; }
+    else if (pidx == 3) { jx = in.fx * u * r2; jy = in.fy * v * r2; }
+    else { jx = in.fx * u * r2 * r2; jy = in.fy * v * r2 * r2; }
   }
   jx *= w;
   jy *= w;

@@ -94,7 +94,7 @@ __device__ __forceinline__ void obs_full(const double4& q4, const double4& t4, c
   if (WK) {
 #pragma unroll
     for (int j = 0; j < kMaxBlockDof; ++j)
-      if (j < iv.mb) intr_param_jac(ir, iv.pidx[j], u, v, w, o.Jk[0][j], o.Jk[WK ? 1 : 0][j]);
+      if (j < iv.mb) intr_param_jac(ld_intr(ir), iv.pidx[j], u, v, w, o.Jk[0][j], o.Jk[WK ? 1 : 0][j]);
   }
   if (sr) {   // chain through the cam_from_rig rotation: J <- J R_cr
 #pragma unroll

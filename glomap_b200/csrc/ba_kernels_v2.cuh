@@ -13,10 +13,11 @@
 //     pass B (camera order): y_c -= R-rotated sum_o [2 X x (A_o z_p) ; A_o z_p]  gathers X_p (pts4) and z_p (32 B each)
 //                            one warp per <= 256-observation segment of ONE camera: register
 //                            accumulation, shuffle reduction, 6 atomics per segment.
-// In camera order the segment's camera, intrinsics and sensor records are warp-uniform, so pass B (and the Schur-Jacobi
-// diagonal) rebuild A_o from them, the pixel and the point with the linearisation's own arithmetic (obs_core +
-// obs_point_blocks) instead of streaming a stored camera-order row: about 160 FP64 instructions per observation in
-// place of 72 B of HBM traffic, the cheaper side on an H100.  All arithmetic stays FP64.
+// In camera order the segment's camera, intrinsics and sensor records are warp-uniform and held in registers, so pass B
+// (and the Schur-Jacobi diagonal) recompute each observation's residual with the linearisation's own arithmetic
+// (obs_core_R) instead of streaming a stored camera-order row, and apply its Jacobian in the camera frame without
+// forming A_o (see "Camera-frame form" below): about 80 FP64 instructions per pinhole observation in place of 72 B of
+// HBM traffic, the cheaper side on an H100.  All arithmetic stays FP64.
 // Algorithmic bytes per mat-vec: 52 N + 80 P (A) + 20 N + 64 P (B, point records gathered from L2: see the slices of
 // BAProblem::create).
 #pragma once
@@ -49,19 +50,77 @@ struct BAViewV2 {
 // so the per-iteration cost over the constant-intrinsics path is 24 NK bytes per observation of streamed rows.
 // ---------------------------------------------------------------------------
 template <int NK>
-__device__ __forceinline__ void obs_intr_rows(const ObsCore& o, const double* __restrict__ ir, const IntrVarRec& iv,
-                                              const double Jp[6], double Jk[2][NK > 0 ? NK : 1],
-                                              double B[NK > 0 ? 3 * NK : 1]) {
+__device__ __forceinline__ void obs_intr_jac(const ObsCore& o, const Intr& in, const IntrVarRec& iv,
+                                             double Jk[2][NK > 0 ? NK : 1]) {
 #pragma unroll
   for (int j = 0; j < NK; ++j) {
     double jx = 0.0, jy = 0.0;
-    if (j < iv.mb) intr_param_jac(ir, iv.pidx[j], o.uv[0], o.uv[1], 1.0, jx, jy);
+    if (j < iv.mb) intr_param_jac(in, iv.pidx[j], o.uv[0], o.uv[1], 1.0, jx, jy);
     if (!o.valid) jx = jy = 0.0;
     Jk[0][j] = jx;
     Jk[1][j] = jy;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) B[3 * j + c] = o.rho1 * (Jp[c] * jx + Jp[3 + c] * jy);
   }
+}
+template <int NK>
+__device__ __forceinline__ void obs_intr_rows(const ObsCore& o, const Intr& in, const IntrVarRec& iv,
+                                              const double Jp[6], double Jk[2][NK > 0 ? NK : 1],
+                                              double B[NK > 0 ? 3 * NK : 1]) {
+  obs_intr_jac<NK>(o, in, iv, Jk);
+#pragma unroll
+  for (int j = 0; j < NK; ++j)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) B[3 * j + c] = o.rho1 * (Jp[c] * Jk[0][j] + Jp[3 + c] * Jk[1][j]);
+}
+
+// ---------------------------------------------------------------------------
+// Camera-frame form of the camera-order kernels.  With Rs = R_cr R (R for a trivial frame, R_cr = cam_from_rig of a
+// known rig), P = R_cr R X (the rotated point in the sensor-camera frame) and J_pi = iz M [I | -(u, v)^T] the
+// projection Jacobian (ProjJac),
+//     J_pt = J_pi Rs,   J_cam = J_pi [ -2 [P]x | I ] B,   B = blockdiag(R_cr, R_cr)
+// so every per-segment sum is taken in the sensor-camera frame and conjugated by B once at the end of the segment
+// (B = I for a trivial frame).  No world-frame J_pt or A_o is formed.  Only R is held in registers: the R_cr factor of
+// a known rig is applied from its sensor record (a branch the trivial frames never take).
+// ---------------------------------------------------------------------------
+// the segment's warp-uniform records, in registers
+struct SegRec {
+  double R[9];
+  double4 t4;
+  Intr in;
+  const double* sr;   // sensor record (known rig) or nullptr
+};
+__device__ __forceinline__ void seg_records(const BAView& v, int seg, int cam, const double* __restrict__ cam_rec,
+                                            const double* __restrict__ intr_rec, SegRec& s) {
+  const double4 q4 = ld_rec32(cam_rec + (size_t)cam * kCamRec);
+  s.t4 = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
+  s.in = ld_intr(intr_rec + (size_t)v.seg_intr[seg] * kIntrRec);
+  s.sr = sensor_of_seg(v, seg);
+  const double q[4] = {q4.x, q4.y, q4.z, q4.w};
+  quat_to_R(q, s.R);
+}
+// x <- R_cr x  (nothing for a trivial frame)
+__device__ __forceinline__ void to_sensor(const double* __restrict__ sr, double x[3]) {
+  if (!sr) return;
+  const double x0 = x[0], x1 = x[1], x2 = x[2];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) x[k] = sr[3 * k] * x0 + sr[3 * k + 1] * x1 + sr[3 * k + 2] * x2;
+}
+// a = rho' J_pi r  and  w = J_pi^T a
+__device__ __forceinline__ void cam_frame_jac(const ObsCore& o, const double r[3], double a[2], double w[3]) {
+  const ProjJac& p = o.pj;
+  const double t0 = r[0] - p.u * r[2], t1 = r[1] - p.v * r[2];
+  const double c = o.rho1 * p.iz;
+  a[0] = c * (p.m00 * t0 + p.m01 * t1);
+  a[1] = c * (p.m10 * t0 + p.m11 * t1);
+  const double s0 = p.iz * (p.m00 * a[0] + p.m10 * a[1]), s1 = p.iz * (p.m01 * a[0] + p.m11 * a[1]);
+  w[0] = s0;
+  w[1] = s1;
+  w[2] = -(p.u * s0 + p.v * s1);
+}
+// x <- R_cr^T x  (the B^T of a known-rig segment)
+__device__ __forceinline__ void rig_to_frame(const double* __restrict__ sr, double x[3]) {
+  const double x0 = x[0], x1 = x[1], x2 = x[2];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) x[k] = sr[k] * x0 + sr[3 + k] * x1 + sr[6 + k] * x2;
 }
 
 // xp[c] = { R^T x_r , R^T x_t, pad, pad }: 64-B rows, so pass A gathers a camera with three 128-bit
@@ -141,16 +200,14 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
   if (warp >= v.n_segs) return;
   const int cam = v.seg_cam[warp];
   const int b = v.seg_begin[warp], e = v.seg_end[warp];
-  const double4 q4c = ld_rec32(cam_rec + (size_t)cam * kCamRec);
-  const double4 t4c = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
-  const double* irc = intr_rec + (size_t)v.seg_intr[warp] * kIntrRec;
-  const double* src = sensor_of_seg(v, warp);
+  SegRec sg;
+  seg_records(v, warp, cam, cam_rec, intr_rec, sg);
   double U[21], g[6];
 #pragma unroll
   for (int k = 0; k < 21; ++k) U[k] = 0.0;
 #pragma unroll
   for (int k = 0; k < 6; ++k) g[k] = 0.0;
-  const int cmask = (int)(__double_as_longlong(t4c.w) & 0xff);
+  const int cmask = (int)(__double_as_longlong(sg.t4.w) & 0xff);
   const bool tvar = !(cmask & 2), rvar = !(cmask & 1);
   // stored-row intrinsics path: U_kk / g_k of the segment's intrinsics block and the image's 6 x NK cross block
   constexpr int NKK = NK > 0 ? NK : 1;
@@ -192,9 +249,7 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
     if (i + 64 < e) pt_nn = ld_stream(v.pt_c + i + 64);
     const double X0 = Xc.x, X1 = Xc.y, X2 = Xc.z;
     ObsCore o;
-    obs_core(q4c, t4c, irc, src, X0, X1, X2, xy, huber_a, o);
-    double Jp[6], A[6], bo[3];
-    obs_point_blocks(o, Jp, A, bo);
+    obs_core_R(sg.R, sg.t4, sg.in, sg.sr, X0, X1, X2, xy, huber_a, o);
     // camera blocks: J_t = J, J_r = J (-2 [R X]x)  (EigenQuaternionManifold: left perturbation of angle 2|d|), masked;
     // U += rho' Jc^T Jc, g += rho' Jc^T e
     double Jc[2][6];
@@ -218,8 +273,8 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
       g[i2] += Jc[0][i2] * e0 + Jc[1][i2] * e1;
     }
     if (NK > 0) {
-      double Jk[2][NKK], Bo[3 * NKK];
-      obs_intr_rows<NK>(o, irc, iv, Jp, Jk, Bo);
+      double Jk[2][NKK];
+      obs_intr_jac<NK>(o, sg.in, iv, Jk);
       int ik = 0;
 #pragma unroll
       for (int a = 0; a < NK; ++a) {
@@ -265,23 +320,22 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
 }
 
 // ---------------------------------------------------------------------------
-// Schur-Jacobi diagonal in camera order, accumulated in the world
-// frame:  Sd_c = Rb ( sum_o Gh^T N Gh ) Rb^T,  N = A_o Vinv_p A_o,
-//         Gh = [ -2 [X]x | I ],  Rb = blockdiag(R, R)
-// A_o is recomputed as in pass B; per observation the kernel gathers the point (pts4, 32 B) and Vinv_p (48 B).
+// Schur-Jacobi diagonal in camera order, accumulated in the sensor-camera frame (per observation, W_o Vinv_p W_o^T):
+//   Sd_c = B^T ( sum_o Gh^T N Gh ) B,   N = J_pi^T Q J_pi,   Q = rho'^2 L Vinv_p L^T,   L = J_pi Rs,
+//   Gh = [ -2 [P]x | I ]
+// with Q = (rho' iz^2)^2 K Q' K, Q' = L' Vinv L'^T, L' = [I | -(u, v)^T] Rs, K = M^T M.  Per observation the kernel
+// gathers the point (pts4, 32 B) and Vinv_p (48 B).
 // ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) ba2_schur_diag(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec,
-                                                      const double* __restrict__ intr_rec, double huber_a) {
+__global__ void __launch_bounds__(128, B200_SD_MIN_CTAS) ba2_schur_diag(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec,
+                                                                        const double* __restrict__ intr_rec, double huber_a) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (warp >= v.n_segs) return;
   const int cam = v.seg_cam[warp];
   const int b = v.seg_begin[warp], e = v.seg_end[warp];
-  const double4 q4c = ld_rec32(cam_rec + (size_t)cam * kCamRec);
-  const double4 t4c = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
-  const double* irc = intr_rec + (size_t)v.seg_intr[warp] * kIntrRec;
-  const double* src = sensor_of_seg(v, warp);
-  // world-frame accumulators: RR (sym 6), RT (full 9), TT (sym 6)
+  SegRec sg;
+  seg_records(v, warp, cam, cam_rec, intr_rec, sg);
+  // accumulators: RR (sym 6), RT (full 9), TT (sym 6)
   double RR[6] = {0, 0, 0, 0, 0, 0}, RT[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}, TT[6] = {0, 0, 0, 0, 0, 0};
   // register pipeline of ba2_linearize_cams: the index of iteration + 2 and the point / pixel / Vinv of iteration + 1
   // are in flight while iteration + 0 is computed
@@ -308,28 +362,45 @@ __global__ void __launch_bounds__(128) ba2_schur_diag(BAView v, BAViewV2 v2, con
       van = vp[0]; vbn = vp[1]; vcn = vp[2];
     }
     if (i + 64 < e) pt_nn = ld_stream(v.pt_c + i + 64);
-    const double X[3] = {Xc.x, Xc.y, Xc.z};
     ObsCore o;
-    obs_core(q4c, t4c, irc, src, X[0], X[1], X[2], xy, huber_a, o);
-    double Jp[6], A[6], bo[3];
-    obs_point_blocks(o, Jp, A, bo);
+    obs_core_R(sg.R, sg.t4, sg.in, sg.sr, Xc.x, Xc.y, Xc.z, xy, huber_a, o);
+    double X[3] = {o.RX[0], o.RX[1], o.RX[2]};
+    to_sensor(sg.sr, X);
+    const ProjJac& pj = o.pj;
     const double vi[6] = {va.x, va.y, vb.x, vb.y, vc.x, vc.y};
-    // T = Vinv A (columns), N = A T (symmetric 3x3)
-    const double Ac0[3] = {A[0], A[1], A[2]}, Ac1[3] = {A[1], A[3], A[4]}, Ac2[3] = {A[2], A[4], A[5]};
-    double T0[3], T1[3], T2[3];
-    sym3_mul(vi, Ac0, T0);
-    sym3_mul(vi, Ac1, T1);
-    sym3_mul(vi, Ac2, T2);
-    double N[3][3];
-    {
-      double c0[3], c1[3], c2[3];
-      sym3_mul(A, T0, c0);
-      sym3_mul(A, T1, c1);
-      sym3_mul(A, T2, c2);
+    // Q' = L' Vinv L'^T,  L' = E Rs = (E R_cr) R,  E = [I | -(u, v)^T]
+    double e0[3] = {1.0, 0.0, -pj.u}, e1[3] = {0.0, 1.0, -pj.v};
+    if (sg.sr) {
 #pragma unroll
-      for (int r = 0; r < 3; ++r) { N[r][0] = c0[r]; N[r][1] = c1[r]; N[r][2] = c2[r]; }
+      for (int c = 0; c < 3; ++c) {
+        e0[c] = sg.sr[c] - pj.u * sg.sr[6 + c];
+        e1[c] = sg.sr[3 + c] - pj.v * sg.sr[6 + c];
+      }
     }
-    // P = 2 [X]x N  (rows: 2 X x N_col);  rr = -2 P [X]x;  rt = P;  tt = N
+    double l0[3], l1[3], t0[3], t1[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      l0[c] = e0[0] * sg.R[c] + e0[1] * sg.R[3 + c] + e0[2] * sg.R[6 + c];
+      l1[c] = e1[0] * sg.R[c] + e1[1] * sg.R[3 + c] + e1[2] * sg.R[6 + c];
+    }
+    sym3_mul(vi, l0, t0);
+    sym3_mul(vi, l1, t1);
+    const double q00 = l0[0] * t0[0] + l0[1] * t0[1] + l0[2] * t0[2];
+    const double q01 = l0[0] * t1[0] + l0[1] * t1[1] + l0[2] * t1[2];
+    const double q11 = l1[0] * t1[0] + l1[1] * t1[1] + l1[2] * t1[2];
+    // H = (rho' iz^2)^2 K Q' K  (J_pi^T Q J_pi = [I | -(u, v)^T]^T H [I | -(u, v)^T])
+    const double k00 = pj.m00 * pj.m00 + pj.m10 * pj.m10, k01 = pj.m00 * pj.m01 + pj.m10 * pj.m11,
+                 k11 = pj.m01 * pj.m01 + pj.m11 * pj.m11;
+    const double a00 = k00 * q00 + k01 * q01, a01 = k00 * q01 + k01 * q11;
+    const double a10 = k01 * q00 + k11 * q01, a11 = k01 * q01 + k11 * q11;
+    const double sc = o.rho1 * pj.iz * pj.iz, c2 = sc * sc;
+    const double h00 = c2 * (a00 * k00 + a01 * k01), h01 = c2 * (a00 * k01 + a01 * k11), h11 = c2 * (a10 * k01 + a11 * k11);
+    double N[3][3];
+    N[0][0] = h00; N[0][1] = N[1][0] = h01; N[1][1] = h11;
+    N[0][2] = N[2][0] = -(h00 * pj.u + h01 * pj.v);
+    N[1][2] = N[2][1] = -(h01 * pj.u + h11 * pj.v);
+    N[2][2] = -(N[0][2] * pj.u + N[1][2] * pj.v);
+    // P = 2 [X]x N  (rows: 2 X x N_col);  rr = -2 P [X]x;  rt = P;  tt = N   (X: the camera-frame point)
     double P[3][3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
@@ -362,11 +433,14 @@ __global__ void __launch_bounds__(128) ba2_schur_diag(BAView v, BAViewV2 v2, con
 #pragma unroll
   for (int k = 0; k < 6; ++k) TT[k] = warp_sum(TT[k]);
   if (lane == 0) {
-    const int mask = (int)(__double_as_longlong(t4c.w) & 0xff);
-    const double q[4] = {q4c.x, q4c.y, q4c.z, q4c.w};
-    double R[9];
-    quat_to_R(q, R);
-    // full 6x6 in the world frame, then S = Rb M Rb^T
+    const int mask = (int)(__double_as_longlong(sg.t4.w) & 0xff);
+    // R = R_cr^T of a known rig (identity for a trivial frame): S = Rb M Rb^T = B^T M B
+    double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    if (sg.sr) {
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) R[3 * r + c] = sg.sr[3 * c + r];
+    }
+    // full 6x6 in the sensor-camera frame, then S = Rb M Rb^T
     double M[6][6];
     const double rr[3][3] = {{RR[0], RR[1], RR[2]}, {RR[1], RR[3], RR[4]}, {RR[2], RR[4], RR[5]}};
     const double tt[3][3] = {{TT[0], TT[1], TT[2]}, {TT[1], TT[3], TT[4]}, {TT[2], TT[4], TT[5]}};
@@ -595,10 +669,10 @@ __global__ void ba2_point_rhs_z(BAView v, BAViewV2 v2) {
 }
 
 // ---------------------------------------------------------------------------
-// pass B (camera order): y_c -= [ 2 R sum (X x w) ; R sum w ],  w = A_o z_p   (NK > 0: y_k -= sum B_o^T z_p)
-// A_o (and B_o) are rebuilt per observation from the segment's camera / intrinsics / sensor records, the pixel and the
-// point, by the arithmetic of the linearisations (obs_core, obs_point_blocks, obs_intr_rows); per observation the
-// kernel streams the index and the pixel (20 B) and gathers two 32-B point records, X_p (pts4) and z_p (z4).
+// pass B (camera order): y_c -= B^T [ 2 sum P x v ; sum v ],  v = J_pi^T a,  a = rho' J_pi Rs z_p
+//                        (= [ 2 R sum (X x w) ; R sum w ] with w = A_o z_p;  NK > 0: y_k -= sum J_k^T a = sum B_o^T z_p)
+// Per observation the kernel recomputes the residual (obs_core_R), streams the index and the pixel (20 B) and gathers
+// two 32-B point records, X_p (pts4) and z_p (z4).
 // ---------------------------------------------------------------------------
 template <int NK>
 __global__ void __launch_bounds__(128, B200_PB_MIN_CTAS) ba2_pass_b(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec,
@@ -611,15 +685,13 @@ __global__ void __launch_bounds__(128, B200_PB_MIN_CTAS) ba2_pass_b(BAView v, BA
   if (warp >= seg_hi) return;
   const int cam = v.seg_cam[warp];
   const int b = v.seg_begin[warp], e = v.seg_end[warp];
-  const double4 q4c = ld_rec32(cam_rec + (size_t)cam * kCamRec);
-  const double4 t4c = ld_rec32(cam_rec + (size_t)cam * kCamRec + 4);
   const int blk = v.seg_intr[warp];
-  const double* irc = intr_rec + (size_t)blk * kIntrRec;
-  const double* src = sensor_of_seg(v, warp);
+  SegRec sg;
+  seg_records(v, warp, cam, cam_rec, intr_rec, sg);
   constexpr int NKK = NK > 0 ? NK : 1;
   IntrVarRec iv{};
   if (NK > 0) iv = v2.ivar[blk];
-  double acc[6] = {0, 0, 0, 0, 0, 0};
+  double acc[6] = {0, 0, 0, 0, 0, 0};   // sensor-camera frame: sum P x w, sum w
   double accK[NKK];
 #pragma unroll
   for (int k = 0; k < NKK; ++k) accK[k] = 0.0;
@@ -648,37 +720,42 @@ __global__ void __launch_bounds__(128, B200_PB_MIN_CTAS) ba2_pass_b(BAView v, BA
     }
     if (i + 64 < e) pt_nn = ld_stream(v.pt_c + i + 64);
     ObsCore o;
-    obs_core(q4c, t4c, irc, src, X.x, X.y, X.z, xy, huber_a, o);
-    double Jp[6], a[6], bo[3];
-    obs_point_blocks(o, Jp, a, bo);
-    const double w0 = a[0] * z.x + a[1] * z.y + a[2] * z.z;
-    const double w1 = a[1] * z.x + a[3] * z.y + a[4] * z.z;
-    const double w2 = a[2] * z.x + a[4] * z.y + a[5] * z.z;
-    acc[0] += 2.0 * (X.y * w2 - X.z * w1);
-    acc[1] += 2.0 * (X.z * w0 - X.x * w2);
-    acc[2] += 2.0 * (X.x * w1 - X.y * w0);
-    acc[3] += w0;
-    acc[4] += w1;
-    acc[5] += w2;
-    if (NK > 0) {
-      double Jk[2][NKK], Bo[3 * NKK];
-      obs_intr_rows<NK>(o, irc, iv, Jp, Jk, Bo);
+    obs_core_R(sg.R, sg.t4, sg.in, sg.sr, X.x, X.y, X.z, xy, huber_a, o);
+    double P[3] = {o.RX[0], o.RX[1], o.RX[2]};
+    to_sensor(sg.sr, P);
+    // R w = J^T rho' J (R z) and R (X x w) = (R X) x (R w): w = A_o z_p is never formed in the world frame
+    double r[3] = {sg.R[0] * z.x + sg.R[1] * z.y + sg.R[2] * z.z,
+                   sg.R[3] * z.x + sg.R[4] * z.y + sg.R[5] * z.z,
+                   sg.R[6] * z.x + sg.R[7] * z.y + sg.R[8] * z.z};
+    to_sensor(sg.sr, r);
+    double a[2], w[3];
+    cam_frame_jac(o, r, a, w);
+    acc[0] += P[1] * w[2] - P[2] * w[1];
+    acc[1] += P[2] * w[0] - P[0] * w[2];
+    acc[2] += P[0] * w[1] - P[1] * w[0];
+    acc[3] += w[0];
+    acc[4] += w[1];
+    acc[5] += w[2];
+    if (NK > 0) {   // B_o^T z_p = J_k^T a
+      double Jk[2][NKK];
+      obs_intr_jac<NK>(o, sg.in, iv, Jk);
 #pragma unroll
-      for (int k = 0; k < NK; ++k) accK[k] += Bo[3 * k] * z.x + Bo[3 * k + 1] * z.y + Bo[3 * k + 2] * z.z;
+      for (int k = 0; k < NK; ++k) accK[k] += Jk[0][k] * a[0] + Jk[1][k] * a[1];
     }
     X = Xn; z = zn; xy = xyn; pt_nxt = pt_nn;
   }
 #pragma unroll
   for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
-  if (lane < 6) {
-    const int mask = (int)(__double_as_longlong(t4c.w) & 0xff);
-    const double q[4] = {q4c.x, q4c.y, q4c.z, q4c.w};
-    double R[9];
-    quat_to_R(q, R);
-    const int bl = lane / 3, r = lane % 3;
-    const bool fixed = bl == 0 ? (mask & 1) : (mask & 2);
-    const double s = R[3 * r] * acc[3 * bl] + R[3 * r + 1] * acc[3 * bl + 1] + R[3 * r + 2] * acc[3 * bl + 2];
-    if (!fixed && s != 0.0) atomicAdd(&y[(size_t)cam * 6 + lane], -s);
+  if (sg.sr) {
+    rig_to_frame(sg.sr, acc);
+    rig_to_frame(sg.sr, acc + 3);
+  }
+  const int mask = (int)(__double_as_longlong(sg.t4.w) & 0xff);
+#pragma unroll
+  for (int k = 0; k < 6; ++k) {
+    const double s = k < 3 ? 2.0 * acc[k] : acc[k];
+    const bool fixed = k < 3 ? (mask & 1) : (mask & 2);
+    if (lane == k && !fixed && s != 0.0) atomicAdd(&y[(size_t)cam * 6 + k], -s);
   }
   if (NK > 0) {
     const size_t kb = (size_t)(v2.C + blk);

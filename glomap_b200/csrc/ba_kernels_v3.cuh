@@ -183,7 +183,7 @@ __global__ void __launch_bounds__(kEllThreads, NK > 0 ? 3 : B200_E1_MIN_CTAS) ba
         if (NK > 0) {   // B_o = rho' J_pt^T J_k next to A_o
           constexpr int NKK = NK > 0 ? NK : 1;
           double Jk[2][NKK], Bo[3 * NKK];
-          obs_intr_rows<NK>(o, ir, ivar[blk], Jp, Jk, Bo);
+          obs_intr_rows<NK>(o, ld_intr(ir), ivar[blk], Jp, Jk, Bo);
           double* rowB = ell.B + ((size_t)r0 + j) * (3 * NK * 32) + lane;
 #pragma unroll
           for (int k = 0; k < 3 * NK; ++k) st_stream(rowB + 32 * k, Bo[k]);
@@ -223,7 +223,7 @@ __global__ void __launch_bounds__(kEllThreads, NK > 0 ? 3 : B200_E1_MIN_CTAS) ba
         if (NK > 0) {
           constexpr int NKK = NK > 0 ? NK : 1;
           double Jk[2][NKK], Bo[3 * NKK];
-          obs_intr_rows<NK>(o, ir, ivar[blk], Jp, Jk, Bo);
+          obs_intr_rows<NK>(o, ld_intr(ir), ivar[blk], Jp, Jk, Bo);
           double* rowB = ell.B + ((size_t)r0 + j) * (3 * NK * 32) + lane;
 #pragma unroll
           for (int k = 0; k < 3 * NK; ++k) st_stream(rowB + 32 * k, Bo[k]);

@@ -25,7 +25,10 @@ namespace b200 {
 #define B200_LC_MIN_CTAS 3   // the register-pipelined kernel needs ~168 registers without spills (3 CTAs); 4 CTAs was slower on H100
 #endif
 #ifndef B200_PB_MIN_CTAS
-#define B200_PB_MIN_CTAS 4   // pass B rebuilds A_o per observation: 124 registers at 4; 5 and 6 spill and were slower (DESIGN §6)
+#define B200_PB_MIN_CTAS 4   // pass B recomputes each observation: 126 registers at 4; 5 and 6 spilled and were slower (DESIGN §6)
+#endif
+#ifndef B200_SD_MIN_CTAS   // v2 camera-order Schur-Jacobi diagonal: 168 registers, no spills, 12 warps / SM
+#define B200_SD_MIN_CTAS 3
 #endif
 #ifndef B200_E1_MIN_CTAS   // ELL point-side linearisation (one thread per point): CTAs of 128 threads per SM
 #define B200_E1_MIN_CTAS 4   // with the register pipeline: ~122 registers, no spills, 16 warps / SM (H100 sweep: 3 equal, 5 slower)
