@@ -66,6 +66,17 @@ class RAOpts(ct.Structure):
     ]
 
 
+class VGCOpts(ct.Structure):
+    _fields_ = [
+        ("max_num_iterations", c_int32), ("max_num_line_search_step_size_iterations", c_int32),
+        ("thres_loss_function", c_double), ("function_tolerance", c_double), ("gradient_tolerance", c_double),
+        ("parameter_tolerance", c_double), ("thres_lower_ratio", c_double), ("thres_higher_ratio", c_double),
+        ("thres_two_view_error", c_double),
+        ("pcg_max_iterations", c_int32), ("pcg_min_iterations", c_int32), ("pcg_rel_tolerance", c_double),
+        ("profile_kernels", c_int32), ("reserved0", c_int32),
+    ]
+
+
 class RAStats(ct.Structure):
     _fields_ = [
         ("l1_iterations", c_int32), ("irls_iterations", c_int32), ("admm_iterations", c_int32), ("usable", c_int32),
@@ -128,6 +139,9 @@ PROTOTYPES = {
     "b200sfm_ra_default_opts": (None, [P(RAOpts)]),
     "b200sfm_ra_solve": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int64] + [c_void_p] * 4 + [c_int32, c_void_p, P(RAStats)]),
     "b200sfm_ra_solve_rig": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int32, c_int64] + [c_void_p] * 8 + [c_int32, c_void_p, P(RAStats)]),
+    "b200sfm_vgc_default_opts": (None, [P(VGCOpts)]),
+    "b200sfm_view_graph_calibrate": (c_int32, [c_void_p, P(VGCOpts), c_int32, c_void_p, c_void_p, c_void_p, c_int64]
+                                     + [c_void_p] * 6 + [P(LMStats)]),
     "b200sfm_ra_solve_gravity": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int64] + [c_void_p] * 5 + [c_int32, c_void_p, P(RAStats)]),
 }
 

@@ -9,6 +9,7 @@
 #include "pair_kernels.cuh"
 #include "ra_solver.cuh"
 #include "track_kernels.cuh"
+#include "vgc_solver.cuh"
 
 namespace {
 
@@ -618,6 +619,84 @@ int b200sfm_image_pairs_inlier_count(b200sfm_ctx* ctx, int32_t num_images, const
       throw b200::InvalidInput{"match feature index out of range of its image"};
     return (int)B200SFM_OK;
   });
+}
+
+// ---- view-graph calibration -------------------------------------------------------
+void b200sfm_vgc_default_opts(b200sfm_vgc_opts* o) {
+  if (!o) return;
+  *o = b200sfm_vgc_opts{};
+  o->max_num_iterations = 100;
+  o->max_num_line_search_step_size_iterations = 20;
+  o->thres_loss_function = 1e-2;
+  o->function_tolerance = 1e-5;
+  o->gradient_tolerance = 1e-10;
+  o->parameter_tolerance = 1e-8;
+  o->thres_lower_ratio = 0.1;
+  o->thres_higher_ratio = 10.0;
+  o->thres_two_view_error = 2.0;
+  o->pcg_max_iterations = 1000;
+  o->pcg_min_iterations = 0;
+  o->pcg_rel_tolerance = 1e-12;
+}
+
+int b200sfm_view_graph_calibrate(b200sfm_ctx* ctx, const b200sfm_vgc_opts* opts, int32_t K, const double* principal_point,
+                                 double* focal, const uint8_t* focal_constant, int64_t E, const int32_t* cam1,
+                                 const int32_t* cam2, const double* F, uint8_t* pair_valid, uint8_t* cam_accepted,
+                                 double* pair_residual, b200sfm_lm_stats* stats) {
+  if (!ctx || !opts || K < 0 || E < 0) return B200SFM_ERR_INVALID_ARG;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (E > 0 && (!principal_point || !focal || !cam1 || !cam2 || !F || !pair_valid || !cam_accepted))
+    return invalid("null argument");
+  if (E > 0x7fffffffLL) return invalid("more than 2^31 - 1 pairs");
+  if (ctx->world > 1) {
+    ctx->err = "view-graph calibration runs on a single-rank context";
+    return B200SFM_ERR_UNSUPPORTED;
+  }
+  b200sfm_lm_stats st{};
+  st.usable = 1;
+  st.num_observations = E;
+  // cameras with a parameter block (used by a pair) and the variable ones among them (.cc:105-120)
+  std::vector<uint8_t> has_block(K, 0), var(K, 0);
+  for (int64_t e = 0; e < E; ++e) {
+    const int32_t a = cam1[e], b = cam2[e];
+    if (a < 0 || a >= K || b < 0 || b >= K) return invalid("pair camera index out of range [0, K)");
+    has_block[a] = has_block[b] = 1;
+  }
+  int n_var = 0;
+  for (int32_t k = 0; k < K; ++k) {
+    var[k] = has_block[k] && !(focal_constant && focal_constant[k]);
+    n_var += var[k];
+  }
+  if (n_var == 0) {   // E == 0 included: "No cameras to optimize", return true (.cc:30-35)
+    if (stats) *stats = st;
+    return B200SFM_OK;
+  }
+  const int rc = guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    b200::VgcSolver sv;
+    std::vector<double> f0(focal, focal + K);
+    double ms_h2d = 0, ms_d2h = 0;
+    sv.create(ctx, K, E, principal_point, focal, var.data(), cam1, cam2, F, &ms_h2d);
+    sv.solve(*opts, st);
+    sv.finish(opts->thres_two_view_error, focal, pair_valid, pair_residual, &ms_d2h);
+    st.ms_h2d = ms_h2d;
+    st.ms_d2h = ms_d2h;
+    st.h2d_bytes = E * (9 * 8 + 2 * 4) + (int64_t)K * (3 * 8 + 1);
+    st.d2h_bytes = E * (1 + (pair_residual ? 16 : 0)) + (int64_t)K * 8;
+    // CopyBackResults (.cc:122-148): a camera whose estimate is out of [lower, higher] x its focal keeps its parameters
+    for (int32_t k = 0; k < K; ++k) {
+      if (!has_block[k]) {
+        focal[k] = f0[k];
+        cam_accepted[k] = 0;
+        continue;
+      }
+      const double ratio = focal[k] / f0[k];
+      cam_accepted[k] = (ratio > opts->thres_higher_ratio || ratio < opts->thres_lower_ratio) ? 0 : 1;
+    }
+    return (int)B200SFM_OK;
+  });
+  if (stats) *stats = st;
+  return rc;
 }
 
 // ---- track establishment ----------------------------------------------------------

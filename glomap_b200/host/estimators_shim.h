@@ -905,4 +905,138 @@ struct RelPoseFilter {
   }
 };
 
+
+// ---------------------------------------------------------------------------
+struct ViewGraphCalibratorOptions : public OptimizationBaseOptions {   // view_graph_calibration.h:10-29
+  double thres_lower_ratio = 0.1;
+  double thres_higher_ratio = 10;
+  double thres_two_view_error = 2.;
+  int max_num_line_search_step_size_iterations = 20;   // Ceres default
+  // PCG knobs of the device solver (the reference factors the normal matrix exactly, view_graph_calibration.cc:21-24)
+  int pcg_max_iterations = 1000;
+  double pcg_rel_tolerance = 1e-12;
+  ViewGraphCalibratorOptions() { thres_loss_function = 1e-2; }
+};
+
+// The camera accessors the calibrator needs: glomap::Camera's own inside a glomap build (scene/camera.h:22-33 and
+// colmap::Camera::FocalLengthIdxs), the COLMAP parameter layout of models 0-3 over scene_min.h otherwise.  Templates, so
+// that a glomap build which never calls the calibrator does not need these members.
+#ifdef B200SFM_WITH_GLOMAP
+template <class CameraT>
+double VgcFocal(const CameraT& c) { return c.Focal(); }
+template <class CameraT>
+void VgcPrincipalPoint(const CameraT& c, double* pp) {
+  const auto p = c.PrincipalPoint();
+  pp[0] = p(0);
+  pp[1] = p(1);
+}
+template <class CameraT>
+std::vector<size_t> VgcFocalLengthIdxs(const CameraT& c) {
+  std::vector<size_t> out;
+  for (const size_t idx : c.FocalLengthIdxs()) out.push_back(idx);
+  return out;
+}
+#else
+template <class CameraT>
+bool VgcIsPinhole(const CameraT& c) { return static_cast<int>(c.model_id) == B200SFM_PINHOLE; }
+template <class CameraT>
+double VgcFocal(const CameraT& c) { return VgcIsPinhole(c) ? (c.params[0] + c.params[1]) / 2.0 : c.params[0]; }
+template <class CameraT>
+void VgcPrincipalPoint(const CameraT& c, double* pp) {
+  const size_t o = VgcIsPinhole(c) ? 2 : 1;
+  pp[0] = c.params[o];
+  pp[1] = c.params[o + 1];
+}
+template <class CameraT>
+std::vector<size_t> VgcFocalLengthIdxs(const CameraT& c) {
+  return VgcIsPinhole(c) ? std::vector<size_t>{0, 1} : std::vector<size_t>{0};
+}
+#endif
+
+// ViewGraphCalibrator (view_graph_calibration.{h,cc}) on the device: the valid CALIBRATED / UNCALIBRATED pairs are
+// flattened in sorted pair-id order and the cameras in sorted camera-id order; CopyBackResults sets every
+// FocalLengthIdxs() entry and has_refined_focal_length of the cameras the ratio test accepts, FilterImagePairs
+// invalidates the pairs above thres_two_view_error.  Returns summary.IsSolutionUsable(); false also when the device call
+// fails (message on stderr).  A template over the view graph and the scene maps so that it takes glomap's own ImagePair
+// and Camera.
+class ViewGraphCalibrator {
+ public:
+  explicit ViewGraphCalibrator(const ViewGraphCalibratorOptions& options) : options_(options) {}
+
+  template <class ViewGraphT, class CameraMap, class ImageMap>
+  bool Solve(ViewGraphT& view_graph, CameraMap& cameras, ImageMap& images) {
+    using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
+    using Cam = typename CameraMap::mapped_type;
+    std::map<image_pair_t, Pair*> psorted;
+    for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
+    std::map<camera_t, Cam*> csorted;
+    for (auto& [id, c] : cameras) csorted[id] = &c;
+    std::map<camera_t, int> cidx;
+    std::vector<Cam*> cams;
+    std::vector<double> pp, focal;
+    std::vector<uint8_t> prior;
+    for (auto& [id, c] : csorted) {
+      cidx[id] = (int)cams.size();
+      cams.push_back(c);
+      double p[2];
+      VgcPrincipalPoint(*c, p);
+      pp.push_back(p[0]); pp.push_back(p[1]);
+      focal.push_back(VgcFocal(*c));
+      prior.push_back(c->has_prior_focal_length ? 1 : 0);
+    }
+    std::vector<Pair*> qual;
+    std::vector<int32_t> cam1, cam2;
+    std::vector<double> F;
+    for (auto& [id, pr] : psorted) {
+      if (pr->config != B200SFM_TWO_VIEW_CALIBRATED && pr->config != B200SFM_TWO_VIEW_UNCALIBRATED) continue;
+      if (!pr->is_valid) continue;
+      auto a = images.find(pr->image_id1), b = images.find(pr->image_id2);
+      if (a == images.end() || b == images.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return false; }
+      auto ca = cidx.find(a->second.camera_id), cb = cidx.find(b->second.camera_id);
+      if (ca == cidx.end() || cb == cidx.end()) { std::fprintf(stderr, "b200sfm: image with an unknown camera\n"); return false; }
+      qual.push_back(pr);
+      cam1.push_back(ca->second);
+      cam2.push_back(cb->second);
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) F.push_back(pr->F(r, c));
+    }
+    const int32_t K = (int32_t)cams.size();
+    const int64_t E = (int64_t)qual.size();
+    b200sfm_vgc_opts o;
+    b200sfm_vgc_default_opts(&o);
+    o.max_num_iterations = options_.solver_options.max_num_iterations;
+    o.max_num_line_search_step_size_iterations = options_.max_num_line_search_step_size_iterations;
+    o.thres_loss_function = options_.thres_loss_function;
+    o.function_tolerance = options_.solver_options.function_tolerance;
+    o.gradient_tolerance = options_.solver_options.gradient_tolerance;
+    o.parameter_tolerance = options_.solver_options.parameter_tolerance;
+    o.thres_lower_ratio = options_.thres_lower_ratio;
+    o.thres_higher_ratio = options_.thres_higher_ratio;
+    o.thres_two_view_error = options_.thres_two_view_error;
+    o.pcg_max_iterations = options_.pcg_max_iterations;
+    o.pcg_rel_tolerance = options_.pcg_rel_tolerance;
+    b200sfm_ctx* ctx = DefaultContext();
+    if (!ctx) return false;
+    std::vector<uint8_t> valid(E, 1), accepted(K, 0);
+    b200sfm_lm_stats st{};
+    const int rc = b200sfm_view_graph_calibrate(ctx, &o, K, pp.data(), focal.data(), prior.data(), E, cam1.data(), cam2.data(),
+                                                F.data(), valid.data(), accepted.data(), nullptr, &st);
+    if (rc != B200SFM_OK) {
+      std::fprintf(stderr, "b200sfm: ViewGraphCalibrator failed: %s\n", b200sfm_last_error(ctx));
+      return false;
+    }
+    for (int32_t k = 0; k < K; ++k) {
+      if (!accepted[k]) continue;
+      cams[k]->has_refined_focal_length = true;
+      for (const size_t idx : VgcFocalLengthIdxs(*cams[k])) cams[k]->params[idx] = focal[k];
+    }
+    for (int64_t e = 0; e < E; ++e)
+      if (!valid[e]) qual[e]->is_valid = false;
+    return st.usable != 0;
+  }
+
+ private:
+  ViewGraphCalibratorOptions options_;
+};
+
 }  // namespace b200sfm_shim

@@ -70,6 +70,7 @@ struct Camera {
   int model_id = 0;                  // colmap::CameraModelId
   std::vector<double> params;
   bool has_prior_focal_length = true;
+  bool has_refined_focal_length = false;   // set by ViewGraphCalibrator
 };
 struct Rig {   // colmap::Rig: one reference sensor (identity) + non-reference sensors, calibrated (cam_from_rig) or not yet
   rig_t rig_id = 0;

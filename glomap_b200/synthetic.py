@@ -700,3 +700,45 @@ def pairs_from_match_arrays(d: dict):
                               config=int(d["config"][e]), quat_xyzw=d["quat"][e], trans=d["trans"][e],
                               F=d["F"][e].reshape(3, 3), H=d["H"][e].reshape(3, 3)) for e in range(len(d["img1"]))]
     return features, cameras, pairs
+
+
+# ---------------------------------------------------------------------------
+# Fundamental matrices of camera pairs (input of ViewGraphCalibrator)
+# ---------------------------------------------------------------------------
+def make_vgc_pairs(scene: Scene, pairs, seed: int = 1, f_noise: float = 0.0, outlier_frac: float = 0.0,
+                   F_sigma: float = 0.0) -> dict:
+    """F of the image pairs ``pairs`` ([E, 2] image indices) of ``scene``, without matches: F = K2^-T [t]x R K1^-1 of the
+    true poses and the pinhole part of the true intrinsics (the camera of image i is intrinsics block cam_intr[i]),
+    normalised to unit Frobenius norm.  ``F_sigma`` multiplies every entry by 1 + N(0, F_sigma^2); ``outlier_frac`` of the
+    pairs get a random unit-norm F instead (``is_outlier``).  ``focal_init`` [K] is Camera::Focal() of each block times
+    (1 + U(-f_noise, f_noise)).  Arrays: img1, img2, cam1, cam2 [E] int32, F [E, 9], principal_point [K, 2], focal_true,
+    focal_init [K], is_outlier [E]."""
+    rng = np.random.default_rng([seed, 91])
+    pr = np.asarray(pairs, np.int64).reshape(-1, 2)
+    img1, img2 = pr[:, 0], pr[:, 1]
+    E = len(pr)
+    R = geo.quat_xyzw_to_rotmat(scene.quat)
+    R_rel = R[img2] @ np.swapaxes(R[img1], -1, -2)
+    t_rel = scene.trans[img2] - np.einsum("nij,nj->ni", R_rel, scene.trans[img1])
+    t_rel /= np.linalg.norm(t_rel, axis=1, keepdims=True)
+    Kinv = np.array([np.linalg.inv(_pinhole_K(int(m), p)) for m, p in zip(scene.intr_model, scene.intr_params)])
+    cam1, cam2 = scene.cam_intr[img1].astype(np.int32), scene.cam_intr[img2].astype(np.int32)
+    tx = np.zeros((E, 3, 3))
+    tx[:, 0, 1], tx[:, 0, 2], tx[:, 1, 2] = -t_rel[:, 2], t_rel[:, 1], -t_rel[:, 0]
+    tx[:, 1, 0], tx[:, 2, 0], tx[:, 2, 1] = t_rel[:, 2], -t_rel[:, 1], t_rel[:, 0]
+    F = (np.swapaxes(Kinv[cam2], -1, -2) @ tx @ R_rel @ Kinv[cam1]).reshape(E, 9)
+    F /= np.linalg.norm(F, axis=1, keepdims=True)
+    if F_sigma > 0:
+        F *= 1.0 + rng.normal(scale=F_sigma, size=F.shape)
+    is_outlier = rng.random(E) < outlier_frac
+    n_out = int(is_outlier.sum())
+    Fo = rng.normal(size=(n_out, 9))
+    F[is_outlier] = Fo / np.linalg.norm(Fo, axis=1, keepdims=True)
+    p = scene.intr_params
+    pinhole = scene.intr_model == PINHOLE
+    focal_true = np.where(pinhole, (p[:, 0] + p[:, 1]) / 2.0, p[:, 0])
+    principal_point = np.where(pinhole[:, None], p[:, 2:4], p[:, 1:3])
+    focal_init = focal_true * (1.0 + rng.uniform(-f_noise, f_noise, size=len(focal_true)))
+    return dict(img1=img1.astype(np.int32), img2=img2.astype(np.int32), cam1=cam1, cam2=cam2, F=np.ascontiguousarray(F),
+                principal_point=np.ascontiguousarray(principal_point), focal_true=focal_true, focal_init=focal_init,
+                is_outlier=is_outlier)

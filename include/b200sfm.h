@@ -440,6 +440,54 @@ int b200sfm_ra_solve_rig(b200sfm_ctx* ctx, const b200sfm_ra_opts* opts, int32_t 
                          const double* edge_w, const int32_t* cam_frames_begin, const int32_t* cam_frames,
                          int32_t fixed_frame, double* theta, b200sfm_ra_stats* stats);
 
+/* ---- view-graph calibration ---------------------------------------------------------------------------------------
+ * ViewGraphCalibrator::Solve (glomap/estimators/view_graph_calibration.cc:11-185), stage 1 of GlobalMapper::Solve
+ * (controllers/global_mapper.cc:41-50): one focal length per camera refined from the fundamental matrices of the image
+ * pairs with FetzerFocalLengthCost / FetzerFocalLengthSameCameraCost (glomap/estimators/cost_function.h:138-310) under
+ * CauchyLoss(thres_loss_function), lower bound 1e-3 on every focal (.cc:105-120).  Field-for-field mirror of
+ * ViewGraphCalibratorOptions (view_graph_calibration.h:10-29) + the inherited solver options (optimization_base.h:18-23)
+ * + the PCG knobs of this implementation (the reference factors the normal matrix exactly, .cc:21-24). */
+typedef struct {
+  int32_t max_num_iterations;                        /* 100 */
+  int32_t max_num_line_search_step_size_iterations;  /* Ceres default 20 (bounded problem) */
+  double thres_loss_function;                        /* Cauchy scale, 1e-2 (view_graph_calibration.h:23) */
+  double function_tolerance;                         /* 1e-5 */
+  double gradient_tolerance;                         /* Ceres default 1e-10 */
+  double parameter_tolerance;                        /* Ceres default 1e-8 */
+  double thres_lower_ratio;                          /* 0.1 */
+  double thres_higher_ratio;                         /* 10 */
+  double thres_two_view_error;                       /* 2 */
+  int32_t pcg_max_iterations;                        /* default 1000 */
+  int32_t pcg_min_iterations;                        /* default 0 */
+  double pcg_rel_tolerance;                          /* ||r_k|| <= tol * ||r_0||, default 1e-12 */
+  int32_t profile_kernels;                           /* 1: time the linearisation / mat-vec kernels with CUDA events */
+  int32_t reserved0;
+} b200sfm_vgc_opts;
+
+void b200sfm_vgc_default_opts(b200sfm_vgc_opts* opts);
+
+/* The caller passes the qualifying pairs only: valid pairs whose config is CALIBRATED or UNCALIBRATED (.cc:71-79).
+ *   principal_point [K][2]   Camera::PrincipalPoint()
+ *   focal [K]                in: Camera::Focal() = (fx + fy) / 2; out: the estimate of every camera used by a pair
+ *                            (those of the others are left as they are)
+ *   focal_constant [K]       nonzero: has_prior_focal_length, the focal is held constant (.cc:113-116); may be NULL
+ *   cam1, cam2 [E]           camera of image_id1 / image_id2; cam1 == cam2 uses the same-camera cost
+ *   F [E][9]                 ImagePair::F (i1_F_i0), row-major
+ *   pair_valid [E]           out: 0 = |r|^2 > thres_two_view_error^2 at the final focals (FilterImagePairs, .cc:150-185),
+ *                            the unlossed residuals evaluated with the estimate even where the ratio test rejected it
+ *   cam_accepted [K]         out: 1 = a camera used by a pair whose estimate lies within [thres_lower_ratio,
+ *                            thres_higher_ratio] times its initial focal: CopyBackResults (.cc:122-148) sets
+ *                            has_refined_focal_length and every FocalLengthIdxs() entry to the estimate; 0 otherwise
+ *   pair_residual [E][2]     out: the unlossed residuals at the final focals; may be NULL
+ * E == 0 or no variable camera: B200SFM_OK with stats->usable = 1 and nothing written (the early return, .cc:30-35).
+ * stats->num_observations is E.  A non-finite F leaves the focals as they were and gives usable = 0, as the failed
+ * evaluation makes Ceres' solution unusable.  A camera index outside [0, K) gives B200SFM_ERR_INVALID_ARG; a context with
+ * more than one rank B200SFM_ERR_UNSUPPORTED. */
+int b200sfm_view_graph_calibrate(b200sfm_ctx* ctx, const b200sfm_vgc_opts* opts, int32_t K, const double* principal_point,
+                                 double* focal, const uint8_t* focal_constant, int64_t E, const int32_t* cam1,
+                                 const int32_t* cam2, const double* F, uint8_t* pair_valid, uint8_t* cam_accepted,
+                                 double* pair_residual, b200sfm_lm_stats* stats);
+
 #ifdef __cplusplus
 }
 #endif
