@@ -87,6 +87,16 @@ class RAStats(ct.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+class PruneStats(ct.Structure):
+    _fields_ = [
+        ("covisible_pairs", c_int64), ("pairs_min5", c_int64), ("visibility_edges", c_int64), ("strong_threshold", c_double),
+        ("clustering_iterations", c_int32), ("largest_component_frames", c_int32),
+    ]
+
+    def as_dict(self):
+        return {f: getattr(self, f) for f, _ in self._fields_}
+
+
 # name -> (restype, argtypes); every symbol include/b200sfm.h declares
 PROTOTYPES = {
     "b200sfm_version": (c_int32, []),
@@ -142,6 +152,8 @@ PROTOTYPES = {
     "b200sfm_vgc_default_opts": (None, [P(VGCOpts)]),
     "b200sfm_view_graph_calibrate": (c_int32, [c_void_p, P(VGCOpts), c_int32, c_void_p, c_void_p, c_void_p, c_int64]
                                      + [c_void_p] * 6 + [P(LMStats)]),
+    "b200sfm_prune_weakly_connected": (c_int32, [c_void_p, c_int32, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_int64]
+                                       + [c_void_p] * 3 + [P(PruneStats)]),
     "b200sfm_ra_solve_gravity": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int64] + [c_void_p] * 5 + [c_int32, c_void_p, P(RAStats)]),
 }
 

@@ -221,20 +221,26 @@ def scene_from_model(cameras, images, points) -> tuple[S.Scene, ModelIndex]:
     return scene, index
 
 
+def default_index(scene: S.Scene) -> ModelIndex:
+    """Synthesised ids / feature tables: image i has exactly its observed features, in scene order."""
+    C, P, K = scene.C, scene.P, len(scene.intr_model)
+    order = np.argsort(scene.obs_cam, kind="stable")
+    feat = np.empty(scene.N, np.int64)
+    counts = np.bincount(scene.obs_cam, minlength=C)
+    starts = np.concatenate([[0], np.cumsum(counts)])
+    feat[order] = np.arange(scene.N) - np.repeat(starts[:-1], counts)
+    xy_sorted = scene.obs_xy[order]
+    return ModelIndex(np.arange(1, K + 1), np.zeros((K, 2), np.int64), np.arange(1, C + 1),
+                      [f"image_{i + 1:06d}.jpg" for i in range(C)],
+                      [xy_sorted[starts[i]:starts[i + 1]] for i in range(C)], np.arange(1, P + 1, dtype=np.uint64),
+                      np.zeros((P, 3), np.uint8), feat)
+
+
 def model_from_scene(scene: S.Scene, index: ModelIndex | None = None, min_supports: int = 2):
     """ConvertGlomapToColmap (colmap_converter.cc:22-133) for trivial frames."""
     C, P, K = scene.C, scene.P, len(scene.intr_model)
-    if index is None:   # synthesise ids / feature tables: image i has exactly its observed features, in scene order
-        order = np.argsort(scene.obs_cam, kind="stable")
-        feat = np.empty(scene.N, np.int64)
-        counts = np.bincount(scene.obs_cam, minlength=C)
-        starts = np.concatenate([[0], np.cumsum(counts)])
-        feat[order] = np.arange(scene.N) - np.repeat(starts[:-1], counts)
-        xy_sorted = scene.obs_xy[order]
-        index = ModelIndex(np.arange(1, K + 1), np.zeros((K, 2), np.int64), np.arange(1, C + 1),
-                           [f"image_{i + 1:06d}.jpg" for i in range(C)],
-                           [xy_sorted[starts[i]:starts[i + 1]] for i in range(C)], np.arange(1, P + 1, dtype=np.uint64),
-                           np.zeros((P, 3), np.uint8), feat)
+    if index is None:
+        index = default_index(scene)
     cameras = {}
     for k in range(K):
         m = int(scene.intr_model[k])
@@ -272,19 +278,67 @@ def model_from_scene(scene: S.Scene, index: ModelIndex | None = None, min_suppor
     return cameras, images, points
 
 
+def write_clustered_model(out_dir: str, scene: S.Scene, index: ModelIndex | None, cluster_id, registered) -> list:
+    """WriteGlomapReconstruction (io/colmap_io.cc:8-66) with the cluster filter of ConvertGlomapToColmap
+    (colmap_converter.cc:22-131), trivial frames: ``cluster_id`` / ``registered`` [C] per image (the output of
+    ``reconstruction_pruning.prune_weakly_connected_images``).  A model holds the images that stay registered in it:
+    the reference deregisters every other frame before writing (colmap_converter.cc:122-128), and its tracks skip the
+    images of those frames (:55-58, :86-90).  So if every id is -1, ``out_dir/0`` holds the registered images; otherwise
+    ``out_dir/c`` holds the images of cluster c (all registered).  Track elements are restricted to the images written,
+    points left with fewer than 2 elements are dropped, and every model keeps all cameras.  Camera models 0-3 only, as
+    ``model_from_scene`` recomputes each point's mean reprojection error.  Returns the directories written."""
+    from .mapper import compact_observations
+    index = index if index is not None else default_index(scene)
+    cid = np.asarray(cluster_id, np.int64)
+    reg = np.asarray(registered, bool)
+    img_ids = np.asarray(index.image_ids)
+    if cid.max(initial=-1) == -1:
+        jobs = [(os.path.join(out_dir, "0"), reg, reg)]
+    else:
+        jobs = [(os.path.join(out_dir, str(c)), cid == c, cid == c) for c in range(int(cid.max()) + 1)]
+    written = []
+    for path, keep_obs_img, keep_img in jobs:
+        keep = keep_obs_img[scene.obs_cam]
+        sub = compact_observations(scene, keep)
+        sub_index = dataclasses.replace(index, obs_feature=np.asarray(index.obs_feature)[keep])
+        cameras, images, points = model_from_scene(sub, sub_index)
+        images = {int(i): images[int(i)] for i in img_ids[keep_img]}
+        write_model(path, cameras, images, points)
+        written.append(path)
+    return written
+
+
 # ---------------------------------------------------------------------------- command line
 def _main(argv=None):
     """``python -m glomap_b200.colmap_io to-flat MODEL_DIR FLAT.bin`` converts a COLMAP sparse model into the flat
     binary problem of ``b200sfm_cli ba|gp`` (mapper_resume-style entry, exe/global_mapper.cc:110);
-    ``from-flat MODEL_DIR FLAT.bin OUT_DIR`` writes the solved state back as a COLMAP model."""
+    ``from-flat MODEL_DIR FLAT.bin OUT_DIR`` writes the solved state back as a COLMAP model;
+    ``prune MODEL_DIR OUT_DIR [--min_num_observations N]`` splits a model into its covisibility clusters on the GPU
+    (PruneWeaklyConnectedImages, the ``mapper_resume --skip_pruning 0`` analogue for trivial frames) and writes one model
+    per cluster to OUT_DIR/0, OUT_DIR/1, ...  Every subcommand reads camera models 0-3 (SIMPLE_PINHOLE, PINHOLE,
+    SIMPLE_RADIAL, RADIAL) only: the flat problem holds those, and ``prune`` recomputes the points' reprojection errors of
+    the models it writes.  The pruning itself does not read the intrinsics."""
     import argparse
     ap = argparse.ArgumentParser(prog="glomap_b200.colmap_io")
     sub = ap.add_subparsers(dest="cmd", required=True)
     a = sub.add_parser("to-flat"); a.add_argument("model"); a.add_argument("flat")
     b = sub.add_parser("from-flat"); b.add_argument("model"); b.add_argument("flat"); b.add_argument("out")
+    c = sub.add_parser("prune", help="split into covisibility clusters (camera models 0-3)")
+    c.add_argument("model"); c.add_argument("out")
+    c.add_argument("--min_num_observations", type=int, default=0)
     args = ap.parse_args(argv)
-    scene, index = scene_from_model(*read_model(args.model))
-    if args.cmd == "to-flat":
+    try:
+        scene, index = scene_from_model(*read_model(args.model))
+    except ValueError as e:
+        raise SystemExit(f"{args.cmd}: {e} (colmap_io reads camera models 0-3 only)")
+    if args.cmd == "prune":
+        from .reconstruction_pruning import prune_weakly_connected_images
+        out = prune_weakly_connected_images(scene.pt_obs_begin, scene.obs_cam, scene.C,
+                                            min_num_observations=args.min_num_observations)
+        for path in write_clustered_model(args.out, scene, index, out["cluster_id"], out["is_registered"]):
+            print(f"wrote {path}")
+        print(f"{out['num_clusters']} clusters, {int(out['is_registered'].sum())} of {scene.C} images registered")
+    elif args.cmd == "to-flat":
         S.write_flat_problem(args.flat, scene)
         print(f"{scene.C} images, {scene.P} points, {scene.N} observations -> {args.flat}")
     else:

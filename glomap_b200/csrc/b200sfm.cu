@@ -7,6 +7,7 @@
 #include "context.cuh"
 #include "gp_solver.cuh"
 #include "pair_kernels.cuh"
+#include "prune_kernels.cuh"
 #include "ra_solver.cuh"
 #include "track_kernels.cuh"
 #include "vgc_solver.cuh"
@@ -696,6 +697,47 @@ int b200sfm_view_graph_calibrate(b200sfm_ctx* ctx, const b200sfm_vgc_opts* opts,
     return (int)B200SFM_OK;
   });
   if (stats) *stats = st;
+  return rc;
+}
+
+// ---- reconstruction pruning -------------------------------------------------------
+int b200sfm_prune_weakly_connected(b200sfm_ctx* ctx, int32_t num_frames, int64_t num_tracks, const int64_t* track_begin,
+                                   const int32_t* obs_frame, const uint8_t* frame_self_loop, int32_t min_num_observations,
+                                   int64_t max_pair_keys_per_pass, int32_t* cluster_id, uint8_t* is_registered,
+                                   int32_t* num_clusters, b200sfm_prune_stats* stats) {
+  if (!ctx || num_frames < 0 || num_tracks < 0 || !track_begin || !num_clusters || (num_frames > 0 && (!cluster_id || !is_registered)))
+    return B200SFM_ERR_INVALID_ARG;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (num_tracks > 0x7ffffffeLL) return invalid("more than 2^31 - 2 tracks");
+  if (track_begin[0] != 0) return invalid("track_begin[0] must be 0");
+  for (int64_t t = 0; t < num_tracks; ++t)
+    if (track_begin[t + 1] < track_begin[t]) return invalid("track_begin must be non-decreasing");
+  const long long n = track_begin[num_tracks];
+  if (n > 0 && !obs_frame) return invalid("null obs_frame");
+  if (ctx->world > 1) {
+    ctx->err = "reconstruction pruning runs on a single-rank context";
+    return B200SFM_ERR_UNSUPPORTED;
+  }
+  const long long max_keys = max_pair_keys_per_pass <= 0 ? (1LL << 27) : std::min<long long>(max_pair_keys_per_pass, 1LL << 30);
+  b200::PruneStats st;
+  const int rc = guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    b200::PruneRunner r(ctx);
+    static_assert(sizeof(long long) == sizeof(int64_t), "track_begin is 64-bit");
+    if (!r.run(num_frames, (int)num_tracks, n, reinterpret_cast<const long long*>(track_begin), obs_frame, frame_self_loop,
+               min_num_observations, max_keys, cluster_id, is_registered, num_clusters, st))
+      throw b200::InvalidInput{"obs_frame outside [0, num_frames)"};
+    B200_CUDA_OK(cudaGetLastError());   // a failed launch of this call is reported here, not left pending for the next caller
+    return (int)B200SFM_OK;
+  });
+  if (stats) {
+    stats->covisible_pairs = st.covisible_pairs;
+    stats->pairs_min5 = st.pairs_min5;
+    stats->visibility_edges = st.visibility_edges;
+    stats->strong_threshold = st.strong_threshold;
+    stats->clustering_iterations = st.clustering_iterations;
+    stats->largest_component_frames = st.largest_component_frames;
+  }
   return rc;
 }
 

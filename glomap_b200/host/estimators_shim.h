@@ -1039,4 +1039,67 @@ class ViewGraphCalibrator {
   ViewGraphCalibratorOptions options_;
 };
 
+// ---------------------------------------------------------------------------
+// PruneWeaklyConnectedImages (processors/reconstruction_pruning.{h,cc}), stage 8 of GlobalMapper::Solve, on the device:
+// frames are flattened in sorted frame-id order and tracks in sorted track-id order, each observation becomes the frame
+// index of its image; a frame with >= 2 images present gets a self-loop (its intra-frame edges, :63-104).  Writes
+// is_registered and cluster_id of every frame back and returns the number of clusters.  min_num_images has no effect,
+// as in the reference (EstablishStrongClusters calls MarkConnectedComponents with its default -1).  Returns 0 and
+// changes nothing when the device call fails or an observation names an unknown image or frame (message on stderr).
+template <class FrameMap, class ImageMap, class TrackMap>
+image_t PruneWeaklyConnectedImages(FrameMap& frames, ImageMap& images, TrackMap& tracks, int min_num_images = 2,
+                                   int min_num_observations = 0) {
+  (void)min_num_images;
+  using Frm = typename FrameMap::mapped_type;
+  using Trk = typename TrackMap::mapped_type;
+  std::map<frame_t, Frm*> fsorted;
+  for (auto& [id, f] : frames) fsorted[id] = &f;
+  std::map<frame_t, int32_t> fidx;
+  std::vector<Frm*> fr;
+  for (auto& [id, f] : fsorted) {
+    fidx[id] = (int32_t)fr.size();
+    fr.push_back(f);
+  }
+  const int32_t F = (int32_t)fr.size();
+  std::vector<int32_t> images_of(F, 0);
+  for (auto& [id, im] : images) {
+    auto it = fidx.find(im.frame_id);
+    if (it != fidx.end()) ++images_of[it->second];
+  }
+  std::vector<uint8_t> self_loop(F), reg(F);
+  for (int32_t f = 0; f < F; ++f) {
+    self_loop[f] = images_of[f] >= 2 ? 1 : 0;
+    reg[f] = fr[f]->is_registered ? 1 : 0;
+  }
+  std::map<track_t, const Trk*> tsorted;
+  for (auto& [id, t] : tracks) tsorted[id] = &t;
+  std::vector<int64_t> begin{0};
+  std::vector<int32_t> obs_frame;
+  for (auto& [id, t] : tsorted) {
+    for (const auto& ob : t->observations) {
+      auto im = images.find(ob.first);
+      if (im == images.end()) { std::fprintf(stderr, "b200sfm: track observation of an unknown image\n"); return 0; }
+      auto f = fidx.find(im->second.frame_id);
+      if (f == fidx.end()) { std::fprintf(stderr, "b200sfm: image of an unknown frame\n"); return 0; }
+      obs_frame.push_back(f->second);
+    }
+    begin.push_back((int64_t)obs_frame.size());
+  }
+  b200sfm_ctx* ctx = DefaultContext();
+  if (!ctx) return 0;
+  std::vector<int32_t> cluster(F, -1);
+  int32_t num_clusters = 0;
+  const int rc = b200sfm_prune_weakly_connected(ctx, F, (int64_t)tsorted.size(), begin.data(), obs_frame.data(), self_loop.data(),
+                                                min_num_observations, 0, cluster.data(), reg.data(), &num_clusters, nullptr);
+  if (rc != B200SFM_OK) {
+    std::fprintf(stderr, "b200sfm: PruneWeaklyConnectedImages failed: %s\n", b200sfm_last_error(ctx));
+    return 0;
+  }
+  for (int32_t f = 0; f < F; ++f) {
+    fr[f]->is_registered = reg[f] != 0;
+    fr[f]->cluster_id = cluster[f];
+  }
+  return (image_t)num_clusters;
+}
+
 }  // namespace b200sfm_shim

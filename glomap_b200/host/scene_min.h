@@ -108,6 +108,7 @@ struct Frame {
   rig_t rig_id = 0;
   rig_t RigId() const { return rig_id; }
   bool is_registered = true;
+  int cluster_id = -1;                 // set by PruneWeaklyConnectedImages
   Rigid3d rig_from_world;
   Rigid3d& RigFromWorld() { return rig_from_world; }
   const Rigid3d& RigFromWorld() const { return rig_from_world; }

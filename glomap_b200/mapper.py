@@ -2,19 +2,21 @@
 (glomap/controllers/global_mapper.cc:79-276) on the flat SoA scene -- rotation averaging (run twice, with
 ``RelPoseFilter::FilterRotations`` and the largest connected component in between), global positioning followed by the
 three track filters and ``NormalizeReconstruction``, then the staged bundle adjustment loop (positions only, then
-rotations too; normalise; reprojection filters with the tightening threshold ``max(3 - ite, 1) * thr``).
+rotations too; normalise; reprojection filters with the tightening threshold ``max(3 - ite, 1) * thr``), and, with
+``skip_pruning = False``, stage 8: ``PruneWeaklyConnectedImages`` over the final tracks (``frame_cluster_id`` /
+``frame_registered`` of the mapper; ``colmap_io.write_clustered_model`` writes one model per cluster).
 
 It mirrors the reference's control flow so that the GPU solvers are exercised in the order, and with the option
 mutations, the real mapper uses; it is host glue (as in the reference) and owns no numerics: every solve and every
 filter goes through ``libb200sfm.so``.  Trivial frames only.  Not covered (they are COLMAP / PoseLib code in the
-reference): view-graph calibration, relative-pose estimation, track establishment, retriangulation, pruning."""
+reference): view-graph calibration, relative-pose estimation, track establishment, retriangulation."""
 from __future__ import annotations
 
 import dataclasses
 
 import numpy as np
 
-from . import estimators as E, geometry as geo, processors as PR, synthetic as S
+from . import estimators as E, geometry as geo, processors as PR, reconstruction_pruning as RP, synthetic as S
 
 
 @dataclasses.dataclass
@@ -43,6 +45,7 @@ class GlobalMapperOptions:
     skip_rotation_averaging: bool = False
     skip_global_positioning: bool = False
     skip_bundle_adjustment: bool = False
+    skip_pruning: bool = True                # global_mapper.h:41; --skip_pruning 0 turns stage 8 on
 
 
 def compact_observations(scene: S.Scene, keep: np.ndarray) -> S.Scene:
@@ -87,6 +90,8 @@ class GlobalMapper:
         self.options_ = options or GlobalMapperOptions()
         self.ctx = ctx
         self.log: list[str] = []
+        self.frame_cluster_id: np.ndarray | None = None   # stage 8: cluster of every frame (-1: none)
+        self.frame_registered: np.ndarray | None = None   # stage 8: frames of the largest visibility component
 
     # -- helpers ------------------------------------------------------------------------------------
     def _filters(self, scene: S.Scene, what) -> S.Scene:
@@ -174,4 +179,9 @@ class GlobalMapper:
                 ite += 1
             scene = self._filters(scene, [("reprojection", thr.max_reprojection_error),
                                           ("triangulation", thr.min_triangulation_angle)])
+        # 8. reconstruction pruning (:340-353): trivial frames, so the tracks' frames are their images
+        if not o.skip_pruning:
+            out = RP.prune_weakly_connected_images(scene.pt_obs_begin, scene.obs_cam, scene.C, ctx=self.ctx)
+            self.frame_cluster_id, self.frame_registered = out["cluster_id"], out["is_registered"]
+            self.log.append(f"pruning: {out['num_clusters']} clusters, threshold {out['stats']['strong_threshold']:g}")
         return True, scene

@@ -742,3 +742,53 @@ def make_vgc_pairs(scene: Scene, pairs, seed: int = 1, f_noise: float = 0.0, out
     return dict(img1=img1.astype(np.int32), img2=img2.astype(np.int32), cam1=cam1, cam2=cam2, F=np.ascontiguousarray(F),
                 principal_point=np.ascontiguousarray(principal_point), focal_true=focal_true, focal_init=focal_init,
                 is_outlier=is_outlier)
+
+
+# ---------------------------------------------------------------------------
+# Covisibility clusters (input of PruneWeaklyConnectedImages)
+# ---------------------------------------------------------------------------
+def make_cluster_tracks(group_sizes, tracks_per_window: int = 40, bridges=(), seed: int = 1, shuffle: bool = True) -> dict:
+    """Frame groups with dense internal tracks plus bridge tracks of set covisibility counts.
+
+    Group g of n_g >= 4 frames gets ``tracks_per_window`` = K tracks over every window of 3 consecutive frames of the
+    group, so its adjacent frame pairs are seen together 2K times (K at the two ends) and the pairs two apart K times.
+    With fewer than 3 bridges per group the median edge weight is K and the MAD 0, so the strong-cluster threshold is
+    thr = max(K, 20): the interior adjacent pairs are strong edges and the end frames join through their two weaker ones,
+    so each group is one cluster.  A bridge (a, b, c) (global frame indices before shuffling, c >= 2) adds tracks
+    [a, a, b] (2 counts of (a, b) each; one [a, a, a, b] when c is odd) and no other pair, so two groups merge when
+    c > thr, or when two bridges between them both have 0.75 thr <= c.
+
+    ``shuffle`` relabels the frames with a random permutation and shuffles the tracks and the observations inside each
+    track.  Returns dict(track_begin [T+1] int64, obs_frame [N] int32, num_frames, group [F] int32 (group of every frame
+    after relabelling), threshold = max(K, 20))."""
+    rng = np.random.default_rng([seed, 97])
+    sizes = [int(n) for n in group_sizes]
+    if min(sizes) < 4:
+        raise ValueError("groups need >= 4 frames")
+    F = sum(sizes)
+    start = np.concatenate([[0], np.cumsum(sizes)])
+    tracks = []
+    for g, n in enumerate(sizes):
+        for i in range(n - 2):
+            tracks += [[start[g] + i, start[g] + i + 1, start[g] + i + 2]] * tracks_per_window
+    for a, b, c in bridges:
+        c = int(c)
+        if c < 2:
+            raise ValueError("a bridge count must be >= 2")
+        if c % 2:
+            tracks.append([a, a, a, b])
+            c -= 3
+        tracks += [[a, a, b]] * (c // 2)
+    group = np.repeat(np.arange(len(sizes)), sizes).astype(np.int32)
+    perm = rng.permutation(F) if shuffle else np.arange(F)
+    tracks = [list(perm[np.asarray(t)]) for t in tracks]
+    if shuffle:
+        order = rng.permutation(len(tracks))
+        tracks = [list(rng.permutation(tracks[k])) for k in order]
+    new_group = np.empty(F, np.int32)
+    new_group[perm] = group
+    lens = np.array([len(t) for t in tracks], np.int64)
+    track_begin = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    obs_frame = np.concatenate([np.asarray(t, np.int64) for t in tracks]).astype(np.int32) if tracks else np.zeros(0, np.int32)
+    return dict(track_begin=track_begin, obs_frame=obs_frame, num_frames=F, group=new_group,
+                threshold=max(float(tracks_per_window), 20.0))

@@ -488,6 +488,58 @@ int b200sfm_view_graph_calibrate(b200sfm_ctx* ctx, const b200sfm_vgc_opts* opts,
                                  const int32_t* cam2, const double* F, uint8_t* pair_valid, uint8_t* cam_accepted,
                                  double* pair_residual, b200sfm_lm_stats* stats);
 
+/* ---- reconstruction pruning ---------------------------------------------------------------------------------------
+ * PruneWeaklyConnectedImages (glomap/processors/reconstruction_pruning.cc:6-131), stage 8 of GlobalMapper::Solve
+ * (controllers/global_mapper.cc:340-353, on with --skip_pruning 0), in frame space: frames 0..F-1 in sorted frame-id
+ * order, a track is the frame index of each of its observations.
+ *   1. covisibility (:14-36): tracks of <= 2 observations are skipped; every observation of another track adds 1 to its
+ *      frame's observation count, every index pair i < j of it whose frames differ adds 1 to the unordered frame pair
+ *      (multiplicities count: frames [a, a, b] add 2 to (a, b))
+ *   2. visibility edges (:38-61): a pair counted >= 5 times (pairs_min5) is an edge of weight = count unless either frame's
+ *      observation count is below min_num_observations
+ *   3. intra-frame edges (:63-104) join the first image of a frame to its other images: in frame space they are
+ *      self-loops, whose only effect is that such a frame belongs to the frame adjacency list (and so is a component of
+ *      its own) even without another edge.  frame_self_loop[f] != 0 marks a frame with >= 2 images present
+ *   4. threshold (:106-127): median = w[E / 2] of the sorted weights, MAD = the same of |w - median|,
+ *      strong_threshold = max(median - MAD, 20)
+ *   5. EstablishStrongClusters (processors/view_graph_manipulation.cc:70-176): KeepLargestConnectedComponents
+ *      (scene/view_graph.cc:56-97) sets is_registered; frames of the edges with weight > thr are united; then up to 10
+ *      passes count the edges with weight >= 0.75 thr between two sets and unite every pair of sets counted >= 2 times,
+ *      repeating while a pass found such a pair (clustering_iterations is the reference's `iteration` at exit, 1..11);
+ *      edges between sets are dropped and MarkConnectedComponents (view_graph.cc:99-126, min_num_img = -1: every
+ *      component gets an id) numbers the components of the rest by size, descending.
+ * Where the reference depends on hash-map order or is undefined:
+ *   (i)   between equally large components in 5a, the one with the smallest frame index is kept;
+ *   (ii)  equally large clusters are numbered by their smallest frame index, ascending;
+ *   (iii) with no visibility edge (the reference indexes an empty vector) the call returns B200SFM_OK with num_clusters = 0,
+ *         every cluster_id = -1 and is_registered as it was.
+ *   track_begin [T + 1]         CSR of the tracks over obs_frame; track_begin[0] = 0, non-decreasing
+ *   obs_frame [track_begin[T]]  frame of every observation; outside [0, F) gives B200SFM_ERR_INVALID_ARG (checked on the
+ *                               device, never dereferenced)
+ *   frame_self_loop [F]         may be NULL (trivial frames)
+ *   max_pair_keys_per_pass      covisibility keys sorted at once (8 B each, ~36 B of device memory per key); <= 0: 2^27,
+ *                               at most 2^30.  The distinct frame pairs of all passes together must stay below 2^31
+ *                               (B200SFM_ERR_INVALID_ARG otherwise; a larger pass size gives fewer)
+ *   cluster_id [F]              out: component of every frame, -1 outside every component
+ *   is_registered [F]           in/out: 1 = in the largest component of the visibility graph
+ *   num_clusters                out: the return value of PruneWeaklyConnectedImages
+ *   stats                       may be NULL
+ * All counting is integer work on the device; the result does not depend on the pass size.  A context with more than one
+ * rank gives B200SFM_ERR_UNSUPPORTED; a kernel launch that fails gives B200SFM_ERR_CUDA (checked before the call returns). */
+typedef struct {
+  int64_t covisible_pairs;           /* distinct frame pairs seen together in a track longer than 2 */
+  int64_t pairs_min5;                /* of these, counted >= 5 times (the reference's `counter`) */
+  int64_t visibility_edges;          /* of these, passing the min_num_observations filter */
+  double strong_threshold;           /* max(median - MAD, 20); 0 when there is no visibility edge */
+  int32_t clustering_iterations;     /* 0 when there is no visibility edge */
+  int32_t largest_component_frames;  /* frames registered by KeepLargestConnectedComponents */
+} b200sfm_prune_stats;
+
+int b200sfm_prune_weakly_connected(b200sfm_ctx* ctx, int32_t num_frames, int64_t num_tracks, const int64_t* track_begin,
+                                   const int32_t* obs_frame, const uint8_t* frame_self_loop, int32_t min_num_observations,
+                                   int64_t max_pair_keys_per_pass, int32_t* cluster_id, uint8_t* is_registered,
+                                   int32_t* num_clusters, b200sfm_prune_stats* stats);
+
 #ifdef __cplusplus
 }
 #endif
