@@ -97,6 +97,25 @@ class PruneStats(ct.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+class GravityOpts(ct.Structure):
+    _fields_ = [
+        ("max_outlier_ratio", c_double), ("max_gravity_error", c_double), ("min_num_neighbors", c_int32),
+        ("max_num_iterations", c_int32), ("function_tolerance", c_double), ("gradient_tolerance", c_double),
+        ("parameter_tolerance", c_double), ("reserved", c_int32 * 4),
+    ]
+
+
+class GravityStats(ct.Structure):
+    _fields_ = [
+        ("error_prone_frames", c_int32), ("rectified_frames", c_int32), ("too_few_terms", c_int32),
+        ("max_lm_iterations", c_int32), ("lm_iterations", c_int64), ("ms_total", c_double), ("ms_h2d", c_double),
+        ("ms_error_test", c_double), ("ms_csr", c_double), ("ms_refine", c_double),
+    ]
+
+    def as_dict(self):
+        return {f: getattr(self, f) for f, _ in self._fields_}
+
+
 # name -> (restype, argtypes); every symbol include/b200sfm.h declares
 PROTOTYPES = {
     "b200sfm_version": (c_int32, []),
@@ -155,6 +174,9 @@ PROTOTYPES = {
     "b200sfm_prune_weakly_connected": (c_int32, [c_void_p, c_int32, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_int64]
                                        + [c_void_p] * 3 + [P(PruneStats)]),
     "b200sfm_ra_solve_gravity": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int64] + [c_void_p] * 5 + [c_int32, c_void_p, P(RAStats)]),
+    "b200sfm_gravity_default_opts": (None, [P(GravityOpts)]),
+    "b200sfm_gravity_refine": (c_int32, [c_void_p, P(GravityOpts), c_int32, c_void_p, c_void_p, c_int64] + [c_void_p] * 5
+                               + [P(GravityStats)]),
 }
 
 

@@ -6,6 +6,7 @@
 #include "ba_solver.cuh"
 #include "context.cuh"
 #include "gp_solver.cuh"
+#include "gravity_kernels.cuh"
 #include "pair_kernels.cuh"
 #include "prune_kernels.cuh"
 #include "ra_solver.cuh"
@@ -737,6 +738,66 @@ int b200sfm_prune_weakly_connected(b200sfm_ctx* ctx, int32_t num_frames, int64_t
     stats->strong_threshold = st.strong_threshold;
     stats->clustering_iterations = st.clustering_iterations;
     stats->largest_component_frames = st.largest_component_frames;
+  }
+  return rc;
+}
+
+// ---- gravity refinement -----------------------------------------------------------
+void b200sfm_gravity_default_opts(b200sfm_gravity_opts* o) {
+  if (!o) return;
+  *o = b200sfm_gravity_opts{};
+  o->max_outlier_ratio = 0.5;
+  o->max_gravity_error = 1.0;
+  o->min_num_neighbors = 7;
+  o->max_num_iterations = 100;
+  o->function_tolerance = 1e-5;
+  o->gradient_tolerance = 1e-10;
+  o->parameter_tolerance = 1e-8;
+}
+
+int b200sfm_gravity_refine(b200sfm_ctx* ctx, const b200sfm_gravity_opts* opts, int32_t F, const double* R_align,
+                           const uint8_t* has_gravity, int64_t E, const int32_t* frame1, const int32_t* frame2,
+                           const double* M, double* gravity, uint8_t* status, b200sfm_gravity_stats* stats) {
+  if (!ctx || !opts || F < 0 || E < 0) return B200SFM_ERR_INVALID_ARG;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (E > 0 && (!R_align || !has_gravity || !frame1 || !frame2 || !M || !gravity || !status)) return invalid("null argument");
+  if (E >= (1LL << 30)) return invalid("2^30 or more pairs");
+  if (ctx->world > 1) {
+    ctx->err = "gravity refinement runs on a single-rank context";
+    return B200SFM_ERR_UNSUPPORTED;
+  }
+  const auto t0 = std::chrono::steady_clock::now();
+  b200::GravityStats st;
+  int rc = B200SFM_OK;
+  if (E > 0 && F > 0) {
+    rc = guarded(ctx, [&]() {
+      B200_CUDA_OK(cudaSetDevice(ctx->device));
+      const b200::GravityParams prm{opts->max_outlier_ratio,  opts->max_gravity_error,  opts->min_num_neighbors,
+                                    opts->max_num_iterations, opts->function_tolerance, opts->gradient_tolerance,
+                                    opts->parameter_tolerance};
+      b200::GravityRunner r(ctx);
+      const int bad = r.run(prm, F, R_align, has_gravity, E, frame1, frame2, M, gravity, status, st);
+      B200_CUDA_OK(cudaGetLastError());   // a failed launch of this call is reported here, not left pending for the next caller
+      if (bad & 1) throw b200::InvalidInput{"frame index outside [0, F)"};
+      if (bad & 2) throw b200::InvalidInput{"a frame with gravity has a non-finite or zero gravity"};
+      if (bad & 4) throw b200::InvalidInput{"a pair has a non-finite M"};
+      return (int)B200SFM_OK;
+    });
+  } else if (E > 0) {
+    rc = invalid("frame index outside [0, F)");   // F == 0: every index is out of range
+  }
+  if (stats) {
+    *stats = b200sfm_gravity_stats{};
+    stats->error_prone_frames = st.error_prone;
+    stats->rectified_frames = st.rectified;
+    stats->too_few_terms = st.too_few;
+    stats->max_lm_iterations = st.max_lm_iterations;
+    stats->lm_iterations = st.lm_iterations;
+    stats->ms_total = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    stats->ms_h2d = st.ms_h2d;
+    stats->ms_error_test = st.ms_error_test;
+    stats->ms_csr = st.ms_csr;
+    stats->ms_refine = st.ms_refine;
   }
   return rc;
 }

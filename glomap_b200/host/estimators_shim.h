@@ -1102,4 +1102,226 @@ image_t PruneWeaklyConnectedImages(FrameMap& frames, ImageMap& images, TrackMap&
   return (image_t)num_clusters;
 }
 
+// ---------------------------------------------------------------------------
+// GravityRefiner (estimators/gravity_refinement.{h,cc}), run by `rotation_averager --refine_gravity 1`, on the device
+// (b200sfm_gravity_refine): frames in sorted frame-id order, valid pairs in sorted pair-id order whose two images have
+// gravity (a frame prior and, off the rig's reference sensor, a known cam_from_rig), M = R_c2^T R_rel R_c1.  Accepted
+// frames get gravity_info.SetGravity(g); their rig_from_world is left alone, as in the reference.  Every error-prone
+// frame is refined against the priors as they were on entry (include/b200sfm.h states the rules).
+// Weak, so that a host linked against a libb200sfm without these entries (an older build, a test double) still links;
+// RefineGravity then reports the missing entry and changes nothing.
+extern "C" {
+void b200sfm_gravity_default_opts(b200sfm_gravity_opts* opts) __attribute__((weak));
+int b200sfm_gravity_refine(b200sfm_ctx* ctx, const b200sfm_gravity_opts* opts, int32_t F, const double* R_align,
+                           const uint8_t* has_gravity, int64_t E, const int32_t* frame1, const int32_t* frame2,
+                           const double* M, double* gravity, uint8_t* status, b200sfm_gravity_stats* stats) __attribute__((weak));
+}
+
+struct GravityRefinerOptions : public OptimizationBaseOptions {   // gravity_refinement.h:12-26
+  double max_outlier_ratio = 0.5;
+  double max_gravity_error = 1.;
+  int min_num_neighbors = 7;
+};
+
+class GravityRefiner {
+ public:
+  explicit GravityRefiner(const GravityRefinerOptions& options) : options_(options) {}
+  b200sfm_gravity_stats summary{};
+
+  template <class ViewGraphT, class FrameMap, class ImageMap>
+  void RefineGravity(const ViewGraphT& view_graph, FrameMap& frames, ImageMap& images) {
+    using Frm = typename FrameMap::mapped_type;
+    std::map<frame_t, Frm*> fsorted;
+    for (auto& [id, f] : frames) fsorted[id] = &f;
+    std::map<frame_t, int32_t> fidx;
+    std::vector<Frm*> fr;
+    for (auto& [id, f] : fsorted) { fidx[id] = (int32_t)fr.size(); fr.push_back(f); }
+    const int32_t F = (int32_t)fr.size();
+    std::vector<double> R_align(9 * (size_t)F, 0.0);
+    std::vector<uint8_t> has(F, 0);
+    for (int32_t f = 0; f < F; ++f) {
+      has[f] = fr[f]->HasGravity() ? 1 : 0;
+      if (has[f]) b200host_adapt::RAlignRowMajor(*fr[f], &R_align[9 * (size_t)f]);
+    }
+    // an image's cam_from_rig rotation (identity for a trivial frame); false: the image has no gravity (image.h:78-84)
+    auto cam_rot = [&](const auto& im, int32_t f, double R[9]) {
+      if (!has[f]) return false;
+      double q[4] = {0, 0, 0, 1};
+      if (!im.HasTrivialFrame() && !b200host_adapt::FrameCamFromRig(*fr[f], im.camera_id, q)) return false;
+      QuatToR(q, R);
+      return true;
+    };
+    using Pair = std::remove_reference_t<decltype(view_graph.image_pairs.begin()->second)>;
+    std::vector<int32_t> f1, f2;
+    std::vector<double> M;
+    std::map<image_pair_t, const Pair*> order;
+    for (const auto& [id, pr] : view_graph.image_pairs)
+      if (pr.is_valid) order[id] = &pr;
+    for (const auto& [id, pp] : order) {
+      const Pair& pr = *pp;
+      const auto i1 = images.find(pr.image_id1), i2 = images.find(pr.image_id2);
+      if (i1 == images.end() || i2 == images.end()) continue;
+      const auto a = fidx.find(i1->second.frame_id), b = fidx.find(i2->second.frame_id);
+      if (a == fidx.end() || b == fidx.end()) continue;
+      double Rc1[9], Rc2[9], R[9], T[9], Me[9];
+      if (!cam_rot(i1->second, a->second, Rc1) || !cam_rot(i2->second, b->second, Rc2)) continue;   // .cc:62-64,149
+      QuatToR(pr.cam2_from_cam1.rotation.coeffs().data(), R);
+      for (int r = 0; r < 3; ++r)   // R Rc1
+        for (int c = 0; c < 3; ++c) T[3 * r + c] = R[3 * r] * Rc1[c] + R[3 * r + 1] * Rc1[3 + c] + R[3 * r + 2] * Rc1[6 + c];
+      for (int r = 0; r < 3; ++r)   // Rc2^T (R Rc1)
+        for (int c = 0; c < 3; ++c) Me[3 * r + c] = Rc2[r] * T[c] + Rc2[3 + r] * T[3 + c] + Rc2[6 + r] * T[6 + c];
+      f1.push_back(a->second);
+      f2.push_back(b->second);
+      M.insert(M.end(), Me, Me + 9);
+    }
+    if (f1.empty()) { std::fprintf(stderr, "Adjacency list not established\n"); return; }   // .cc:14-17
+    if (!b200sfm_gravity_refine || !b200sfm_gravity_default_opts) {
+      std::fprintf(stderr, "b200sfm: this libb200sfm has no b200sfm_gravity_refine\n");
+      return;
+    }
+    b200sfm_ctx* ctx = DefaultContext();
+    if (!ctx) return;
+    b200sfm_gravity_opts o;
+    b200sfm_gravity_default_opts(&o);
+    o.max_outlier_ratio = options_.max_outlier_ratio;
+    o.max_gravity_error = options_.max_gravity_error;
+    o.min_num_neighbors = options_.min_num_neighbors;
+    o.max_num_iterations = options_.solver_options.max_num_iterations;
+    o.function_tolerance = options_.solver_options.function_tolerance;
+    o.gradient_tolerance = options_.solver_options.gradient_tolerance;
+    o.parameter_tolerance = options_.solver_options.parameter_tolerance;
+    std::vector<double> g(3 * (size_t)F, 0.0);
+    std::vector<uint8_t> status(F, 0);
+    const int rc = b200sfm_gravity_refine(ctx, &o, F, R_align.data(), has.data(), (int64_t)f1.size(), f1.data(), f2.data(),
+                                          M.data(), g.data(), status.data(), &summary);
+    if (rc != B200SFM_OK) {
+      std::fprintf(stderr, "b200sfm: RefineGravity failed: %s\n", b200sfm_last_error(ctx));
+      return;
+    }
+    for (int32_t f = 0; f < F; ++f)
+      if (status[f] == 2) b200host_adapt::SetFrameGravity(*fr[f], &g[3 * (size_t)f]);   // .cc:119-123
+    std::fprintf(stderr, "Number of rectified frames: %d / %d\n", summary.rectified_frames, summary.error_prone_frames);
+  }
+
+ private:
+  GravityRefinerOptions options_;
+};
+
+// ViewGraph::KeepLargestConnectedComponents (scene/view_graph.cc:56-97) over frames: the frames of the largest component
+// of the valid pairs stay registered, every other frame is deregistered and the pairs that leave the component become
+// invalid.  Equally large components: the one with the smallest frame id.  Returns the number of images registered.
+template <class ViewGraphT, class FrameMap, class ImageMap>
+int KeepLargestConnectedComponents(ViewGraphT& view_graph, FrameMap& frames, ImageMap& images) {
+  std::map<frame_t, std::vector<frame_t>> adj;
+  for (auto& [id, pr] : view_graph.image_pairs) {
+    if (!pr.is_valid) continue;
+    const auto i1 = images.find(pr.image_id1), i2 = images.find(pr.image_id2);
+    if (i1 == images.end() || i2 == images.end()) continue;
+    adj[i1->second.frame_id].push_back(i2->second.frame_id);
+    adj[i2->second.frame_id].push_back(i1->second.frame_id);
+  }
+  std::map<frame_t, int> comp;
+  std::vector<size_t> size;
+  for (auto& [s, _] : adj) {
+    if (comp.count(s)) continue;
+    const int c = (int)size.size();
+    size.push_back(0);
+    std::queue<frame_t> q;
+    q.push(s);
+    comp[s] = c;
+    while (!q.empty()) {
+      const frame_t u = q.front();
+      q.pop();
+      ++size[c];
+      for (frame_t v : adj[u])
+        if (!comp.count(v)) { comp[v] = c; q.push(v); }
+    }
+  }
+  int best = -1;
+  for (int c = 0; c < (int)size.size(); ++c)
+    if (best < 0 || size[c] > size[best]) best = c;
+  for (auto& [id, f] : frames) {
+    const auto it = comp.find(id);
+    f.is_registered = it != comp.end() && it->second == best;
+  }
+  for (auto& [id, pr] : view_graph.image_pairs) {
+    const auto i1 = images.find(pr.image_id1), i2 = images.find(pr.image_id2);
+    if (i1 == images.end() || i2 == images.end()) { pr.is_valid = false; continue; }
+    const auto a = comp.find(i1->second.frame_id), b = comp.find(i2->second.frame_id);
+    if (a == comp.end() || b == comp.end() || a->second != best || b->second != best) pr.is_valid = false;
+  }
+  int n = 0;
+  for (auto& [id, im] : images) {
+    const auto it = comp.find(im.frame_id);
+    n += it != comp.end() && it->second == best;
+  }
+  return n;
+}
+
+// SolveRotationAveraging (controllers/rotation_averager.{h,cc}:8-63,183-197): with use_gravity and use_stratified, the
+// pairs whose two images have gravity are solved first as a 1-DoF problem on their largest component, unless there is
+// none or they are more than 95 % of the pairs; then the whole graph.  Not restated: the pre-pass that estimates unknown
+// cam_from_rig rotations with trivial rigs (.cc:65-182).  When it would run (a rig with an uncalibrated sensor and
+// !skip_initialization) the call says so on stderr and returns false.
+struct RotationAveragerOptions : public RotationEstimatorOptions {   // rotation_averager.h:7-12
+  RotationAveragerOptions() = default;
+  RotationAveragerOptions(const RotationEstimatorOptions& o) : RotationEstimatorOptions(o) {}
+  bool use_stratified = true;
+};
+
+inline bool SolveRotationAveraging(ViewGraph& view_graph, std::unordered_map<rig_t, Rig>& rigs,
+                                   std::unordered_map<frame_t, Frame>& frames, std::unordered_map<image_t, Image>& images,
+                                   const RotationAveragerOptions& options) {
+  KeepLargestConnectedComponents(view_graph, frames, images);                                 // .cc:13
+  auto image_has_gravity = [&](const Image& im) {
+    const auto f = frames.find(im.frame_id);
+    if (f == frames.end() || !f->second.HasGravity()) return false;
+    double q[4];
+    return im.HasTrivialFrame() || b200host_adapt::FrameCamFromRig(f->second, im.camera_id, q);
+  };
+  auto registered = [&](const Image& im) {
+    const auto f = frames.find(im.frame_id);
+    return f != frames.end() && f->second.is_registered;
+  };
+  bool solve_1dof = options.use_gravity && options.use_stratified;
+  ViewGraph view_graph_grav;
+  size_t total_pairs = 0;
+  if (solve_1dof) {
+    for (const auto& [pair_id, pr] : view_graph.image_pairs) {                                 // .cc:22-39
+      if (!pr.is_valid) continue;
+      const auto i1 = images.find(pr.image_id1), i2 = images.find(pr.image_id2);
+      if (i1 == images.end() || i2 == images.end() || !registered(i1->second) || !registered(i2->second)) continue;
+      ++total_pairs;
+      if (image_has_gravity(i1->second) && image_has_gravity(i2->second)) {
+        ImagePair p = pr;
+        p.is_valid = true;
+        view_graph_grav.image_pairs.emplace(pair_id, p);
+      }
+    }
+  }
+  const size_t grav_pairs = view_graph_grav.image_pairs.size();
+  std::fprintf(stderr, "Total image pairs: %zu, gravity image pairs: %zu\n", total_pairs, grav_pairs);
+  solve_1dof = solve_1dof && !(grav_pairs == 0 || grav_pairs > total_pairs * 0.95);          // .cc:49-50
+  if (solve_1dof) {
+    KeepLargestConnectedComponents(view_graph_grav, frames, images);                          // .cc:56
+    RotationEstimatorOptions o1 = options;
+    RotationEstimator est_grav(o1);
+    if (!est_grav.EstimateRotations(view_graph_grav, rigs, frames, images)) return false;
+    KeepLargestConnectedComponents(view_graph, frames, images);                               // .cc:62
+  }
+  bool unknown_cams = false;
+  for (auto& [rig_id, rig] : rigs) unknown_cams = unknown_cams || !b200host_adapt::AllSensorsCalibrated(rig);
+  if (unknown_cams && !options.skip_initialization) {
+    std::fprintf(stderr, "SolveRotationAveraging: cameras with an unknown cam_from_rig need the trivial-rig pre-pass "
+                         "(rotation_averager.cc:65-182), which is not supported here\n");
+    return false;
+  }
+  RotationEstimatorOptions o = options;
+  if (unknown_cams) o.skip_initialization = false;                                            // .cc:188-190
+  RotationEstimator est(o);
+  const bool ok = est.EstimateRotations(view_graph, rigs, frames, images);
+  KeepLargestConnectedComponents(view_graph, frames, images);                                 // .cc:195
+  return ok;
+}
+
 }  // namespace b200sfm_shim

@@ -33,6 +33,22 @@ inline void RAlignRowMajor(const glomap::Frame& f, double out[9]) {
   for (int r = 0; r < 3; ++r)
     for (int c = 0; c < 3; ++c) out[3 * r + c] = R(r, c);
 }
+// cam_from_rig rotation (quaternion xyzw) of a non-reference camera through the frame's rig pointer; false when unknown
+inline bool FrameCamFromRig(const glomap::Frame& f, glomap::camera_t camera_id, double q[4]) {
+  if (!f.RigPtr()) return false;
+  const auto& c = f.RigPtr()->MaybeSensorFromRig(glomap::sensor_t(glomap::SensorType::CAMERA, camera_id));
+  if (!c.has_value()) return false;
+  for (int k = 0; k < 4; ++k) q[k] = c->rotation.coeffs().data()[k];
+  return true;
+}
+// GravityInfo::SetGravity (scene/frame.h:46-50): gravity and R_align = GetAlignRot(g).  A template, so that it is
+// compiled only where a refiner writes gravity back.
+template <class FrameT>
+inline void SetFrameGravity(FrameT& f, const double g[3]) {
+  Eigen::Vector3d v;
+  for (int k = 0; k < 3; ++k) v[k] = g[k];
+  f.gravity_info.SetGravity(v);
+}
 }  // namespace b200host_adapt
 #else
 #include <map>
@@ -109,6 +125,8 @@ struct Frame {
   rig_t RigId() const { return rig_id; }
   bool is_registered = true;
   int cluster_id = -1;                 // set by PruneWeaklyConnectedImages
+  struct Rig* rig_ptr = nullptr;       // colmap::Frame::RigPtr()
+  struct Rig* RigPtr() const { return rig_ptr; }
   Rigid3d rig_from_world;
   Rigid3d& RigFromWorld() { return rig_from_world; }
   const Rigid3d& RigFromWorld() const { return rig_from_world; }
@@ -172,5 +190,12 @@ inline bool HasCamFromRig(const b200host::Rig& rig, b200host::camera_t camera_id
 inline void RAlignRowMajor(const b200host::Frame& f, double out[9]) {
   for (int k = 0; k < 9; ++k) out[k] = f.gravity_info.R_align[k];
 }
+inline bool FrameCamFromRig(const b200host::Frame& f, b200host::camera_t camera_id, double q[4]) {
+  if (!f.RigPtr() || !HasCamFromRig(*f.RigPtr(), camera_id)) return false;
+  const b200host::Rigid3d c = f.RigPtr()->SensorFromRig(camera_id);
+  for (int k = 0; k < 4; ++k) q[k] = c.rotation.c[k];
+  return true;
+}
+inline void SetFrameGravity(b200host::Frame& f, const double g[3]) { f.gravity_info.SetGravity({{g[0], g[1], g[2]}}); }
 }  // namespace b200host_adapt
 #endif

@@ -792,3 +792,62 @@ def make_cluster_tracks(group_sizes, tracks_per_window: int = 40, bridges=(), se
     obs_frame = np.concatenate([np.asarray(t, np.int64) for t in tracks]).astype(np.int32) if tracks else np.zeros(0, np.int32)
     return dict(track_begin=track_begin, obs_frame=obs_frame, num_frames=F, group=new_group,
                 threshold=max(float(tracks_per_window), 20.0))
+
+
+# ---------------------------------------------------------------------------
+# Gravity priors (`glomap rotation_averager --gravity_path`, docs/rotation_averager.md)
+# ---------------------------------------------------------------------------
+def _random_axis_rotations(rng, k: int, angle_sigma: float) -> np.ndarray:
+    """CreateRandomRotation (controllers/rotation_averager_test.cc:16-34): an axis uniform in (theta, phi) and a normal
+    angle of standard deviation ``angle_sigma`` radians; returns rotation vectors [k,3]."""
+    theta = rng.uniform(0, 2 * np.pi, size=k)
+    phi = rng.uniform(0, np.pi, size=k)
+    axis = np.stack([np.cos(theta) * np.sin(phi), np.sin(theta) * np.sin(phi), np.cos(phi)], 1)
+    return axis * rng.normal(0, angle_sigma, size=(k, 1))
+
+
+def make_gravity(R_gt: np.ndarray, noise_deg: float = 0.0, outlier_ratio: float = 0.0, seed: int = 1):
+    """PrepareGravity (controllers/rotation_averager_test.cc:36-63): the gravity of frame f is R_gt[f] (0, 1, 0)
+    (rig_from_world times the world's gravity), turned by a random rotation of ``noise_deg`` standard deviation; with
+    probability ``outlier_ratio`` it is replaced by the unit rotation axis of a random rotation (1 rad standard
+    deviation).  Returns (gravity [F,3], is_outlier [F])."""
+    rng = np.random.default_rng(seed)
+    R_gt = np.asarray(R_gt, dtype=np.float64)
+    F = len(R_gt)
+    g = R_gt[:, :, 1].copy()
+    if noise_deg > 0:
+        g = np.einsum("nij,nj->ni", geo.so3_exp(_random_axis_rotations(rng, F, np.radians(noise_deg))), g)
+    out = rng.uniform(size=F) < outlier_ratio if outlier_ratio > 0 else np.zeros(F, bool)
+    if out.any():
+        w = _random_axis_rotations(rng, int(out.sum()), 1.0)
+        g[out] = w / np.linalg.norm(w, axis=1, keepdims=True)
+    return g, out
+
+
+def write_gravity_file(path: str, names, gravity: np.ndarray) -> None:
+    """IMAGE_NAME GX GY GZ (glomap/io/pose_io.cc:139-180); rows of NaN (no prior) are not written."""
+    with open(path, "w") as f:
+        for nm, g in zip(names, np.asarray(gravity, dtype=np.float64)):
+            if np.isfinite(g).all():
+                f.write(f"{nm} {g[0]:.17g} {g[1]:.17g} {g[2]:.17g}\n")
+
+
+def read_gravity_file(path: str, names) -> np.ndarray:
+    """ReadGravity's parse: [len(names),3] with NaN rows for the images the file does not name; unknown names are
+    ignored."""
+    idx = {nm: i for i, nm in enumerate(names)}
+    g = np.full((len(names), 3), np.nan)
+    with open(path) as f:
+        for line in f:
+            tok = line.rstrip("\n").split(" ")
+            if len(tok) >= 4 and tok[0] in idx:
+                g[idx[tok[0]]] = [float(x) for x in tok[1:4]]
+    return g
+
+
+def write_weight_file(path: str, vg: ViewGraph, weight: np.ndarray, names=None) -> None:
+    """IMAGE_NAME_1 IMAGE_NAME_2 WEIGHT (ReadRelWeight, glomap/io/pose_io.cc:91-135)."""
+    names = names or [f"img{i:04d}" for i in range(vg.n_images)]
+    with open(path, "w") as f:
+        for e in range(vg.E):
+            f.write(f"{names[vg.ei[e]]} {names[vg.ej[e]]} {float(weight[e]):.17g}\n")

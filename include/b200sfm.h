@@ -540,6 +540,66 @@ int b200sfm_prune_weakly_connected(b200sfm_ctx* ctx, int32_t num_frames, int64_t
                                    int64_t max_pair_keys_per_pass, int32_t* cluster_id, uint8_t* is_registered,
                                    int32_t* num_clusters, b200sfm_prune_stats* stats);
 
+/* ---- gravity refinement -------------------------------------------------------------------------------------------
+ * GravityRefiner::RefineGravity (glomap/estimators/gravity_refinement.cc:9-181), run by `glomap rotation_averager
+ * --refine_gravity 1`, in frame space: frames 0..F-1, and per pair the frame-level relative rotation
+ * M = R_c2^T R_rel R_c1 (rig2_from_rig1; R_c is the image's cam_from_rig rotation, the identity for a trivial frame).
+ *   1. IdentifyErrorProneGravity (.cc:129-181): a pair is a mistake when CalcAngle(R, AngleToRotUp(RotUpToAngle(R))) >
+ *      max_gravity_error for R = Ra2^T M Ra1; it counts once toward the (mistakes, total) of each of its two frames (twice
+ *      for a pair inside one frame).  A frame is error-prone when total >= min_num_neighbors and
+ *      mistakes / total >= max_outlier_ratio
+ *   2. per error-prone frame (.cc:42-124): the observed gravities are M^T g2 for the frame of image 1 and M g1 for the
+ *      frame of image 2 (g = column 1 of R_align; a pair inside the frame is one term, of the first kind).  With fewer
+ *      than min_num_neighbors terms the frame is skipped (status 1); otherwise AverageGravity (math/gravity.cc:37-91) starts
+ *      an LM on SphereManifold<3> with residual g - g_obs under ArctanLoss(1 - cos(max_gravity_error)), and the result is
+ *      accepted (status 2) when fewer than max_outlier_ratio of the terms lie more than 2 max_gravity_error away, else
+ *      rejected (status 3)
+ * Rules where the reference depends on hash order or a library convention:
+ *   (i)   every error-prone frame is refined against the gravities as they were on entry (the reference refines in
+ *         unordered_set order and later frames see earlier results)
+ *   (ii)  when exactly half of the terms point against the principal direction, its sign is the one whose dot product
+ *         with the frame's prior gravity is >= 0 (the reference leaves it to the SVD)
+ *   (iii) the error test depends on the completion of R_align around its gravity column; the reference completes it with
+ *         Eigen's Householder QR (GetAlignRot, math/gravity.cc:11-24), and callers that want its decisions pass that one.
+ *   R_align [F][9]       row-major; column 1 = unit gravity.  Frames with gravity must have finite entries and a non-zero
+ *                        column 1 (B200SFM_ERR_INVALID_ARG otherwise)
+ *   has_gravity [F]      nonzero: the frame has a gravity prior; pairs with a frame without one are ignored
+ *   frame1, frame2 [E]   frames of image 1 / image 2 of the valid pairs whose two images have gravity (.cc:62-64,149);
+ *                        outside [0, F) gives B200SFM_ERR_INVALID_ARG (checked on the device, never dereferenced); E < 2^30
+ *   M [E][9]             row-major; a non-finite entry gives B200SFM_ERR_INVALID_ARG
+ *   gravity [F][3]       out: the refined gravity, written for the frames of status 2 only
+ *   status [F]           out: 0 = not error-prone, 1 = error-prone with too few terms, 2 = refined and accepted,
+ *                        3 = refined and rejected; written for every frame when a frame is error-prone
+ *   stats                may be NULL
+ * E == 0, or no error-prone frame, gives B200SFM_OK with nothing written.  A context with more than one rank gives
+ * B200SFM_ERR_UNSUPPORTED; a kernel launch that fails gives B200SFM_ERR_CUDA (checked before the call returns). */
+typedef struct {
+  double max_outlier_ratio;    /* 0.5 (gravity_refinement.h:14) */
+  double max_gravity_error;    /* degrees, 1 (gravity_refinement.h:16) */
+  int32_t min_num_neighbors;   /* 7 (gravity_refinement.h:18) */
+  int32_t max_num_iterations;  /* 100 (optimization_base.h:20) */
+  double function_tolerance;   /* 1e-5 (optimization_base.h:22) */
+  double gradient_tolerance;   /* Ceres default 1e-10 */
+  double parameter_tolerance;  /* Ceres default 1e-8 */
+  int32_t reserved[4];
+} b200sfm_gravity_opts;
+
+void b200sfm_gravity_default_opts(b200sfm_gravity_opts* opts);
+
+typedef struct {
+  int32_t error_prone_frames;
+  int32_t rectified_frames;    /* status 2 */
+  int32_t too_few_terms;       /* status 1 */
+  int32_t max_lm_iterations;
+  int64_t lm_iterations;       /* summed over the refined frames */
+  double ms_total;             /* host wall clock of the call */
+  double ms_h2d, ms_error_test, ms_csr, ms_refine;   /* device events */
+} b200sfm_gravity_stats;
+
+int b200sfm_gravity_refine(b200sfm_ctx* ctx, const b200sfm_gravity_opts* opts, int32_t F, const double* R_align,
+                           const uint8_t* has_gravity, int64_t E, const int32_t* frame1, const int32_t* frame2,
+                           const double* M, double* gravity, uint8_t* status, b200sfm_gravity_stats* stats);
+
 #ifdef __cplusplus
 }
 #endif
