@@ -153,6 +153,8 @@ PROTOTYPES = {
     "b200sfm_image_pairs_inlier_count": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
                                                    c_int64] + [c_void_p] * 9 + [c_double] * 3 + [c_void_p] * 3),
     "b200sfm_tracks_free": (None, [c_void_p]),
+    "b200sfm_tracks_select": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_void_p] + [c_int32] * 4
+                              + [c_void_p, P(c_int64)]),
     "b200sfm_gp_default_opts": (None, [P(GPOpts)]),
     "b200sfm_gp_solve": (c_int32, [c_void_p, P(GPOpts), c_int32, c_int32, c_int64] + [c_void_p] * 8 + [P(LMStats)]),
     "b200sfm_gp_problem_create": (c_int32, [c_void_p, c_int32, c_int32, c_int64] + [c_void_p] * 5 + [c_int32, P(c_void_p)]),

@@ -11,6 +11,7 @@
 #include "prune_kernels.cuh"
 #include "ra_solver.cuh"
 #include "track_kernels.cuh"
+#include "track_select_kernels.cuh"
 #include "vgc_solver.cuh"
 
 namespace {
@@ -856,6 +857,42 @@ void b200sfm_tracks_free(b200sfm_tracks* t) {
   guarded(t->ctx, [&]() {
     cudaSetDevice(t->ctx->device);
     delete t;
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_tracks_select(b200sfm_ctx* ctx, int64_t num_tracks, const uint64_t* track_ids, const int64_t* begin,
+                          const uint32_t* obs_image, int32_t num_registered, const uint32_t* registered_image_ids,
+                          int32_t min_num_tracks_per_view, int32_t min_num_view_per_track, int32_t max_num_view_per_track,
+                          int32_t max_num_tracks, uint8_t* keep, int64_t* num_selected) {
+  if (!ctx || !begin || !num_selected || num_tracks < 0 || num_registered < 0) return B200SFM_ERR_INVALID_ARG;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (num_tracks > 0 && (!track_ids || !keep)) return invalid("null track_ids or keep");
+  if (num_registered > 0 && !registered_image_ids) return invalid("null registered_image_ids");
+  if (num_tracks > 0x7ffffffeLL) return invalid("more than 2^31 - 2 tracks");
+  if (begin[0] != 0) return invalid("begin[0] must be 0");
+  for (int64_t t = 0; t < num_tracks; ++t)
+    if (begin[t + 1] < begin[t]) return invalid("begin must be non-decreasing");
+  const long long n = begin[num_tracks];
+  if (n > 0x7ffffffeLL) return invalid("more than 2^31 - 2 observations");
+  if (n > 0 && !obs_image) return invalid("null obs_image");
+  *num_selected = 0;
+  if (num_tracks == 0) return B200SFM_OK;
+  // the reference compares these int options with size_t / track_t values: a negative one converts to a huge unsigned
+  const long long quota = min_num_tracks_per_view < 0 ? -1 : (long long)min_num_tracks_per_view;
+  const unsigned long long min_views = (unsigned long long)(long long)min_num_view_per_track;
+  const unsigned long long max_views = (unsigned long long)(long long)max_num_view_per_track;
+  const long long cap = max_num_tracks < 0 ? -1 : (long long)max_num_tracks + 1;
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    b200::TrackSelectRunner r(ctx);
+    static_assert(sizeof(unsigned long long) == sizeof(uint64_t) && sizeof(long long) == sizeof(int64_t), "64-bit ids and offsets");
+    long long num = 0;
+    if (!r.run((int)num_tracks, reinterpret_cast<const unsigned long long*>(track_ids), reinterpret_cast<const long long*>(begin), n,
+               obs_image, num_registered, registered_image_ids, quota, min_views, max_views, cap, keep, &num))
+      throw b200::InvalidInput{"two tracks share a track id"};
+    B200_CUDA_OK(cudaGetLastError());   // a failed launch of this call is reported here, not left pending for the next caller
+    *num_selected = num;
     return (int)B200SFM_OK;
   });
 }

@@ -9,7 +9,7 @@
 //   4. stable sort of the nodes by root -> tracks in ascending track id, observations of a track in ascending global id
 //   5. a track is discarded (observations cleared, id kept, :118-131) when two of its features inside ONE image are
 //      further apart than thres_inconsistency pixels
-// The greedy, order-dependent selection FindTracksForProblem (:153-234) stays on the host (track_establishment.py).
+// The selection FindTracksForProblem (:153-227) is track_select_kernels.cuh.
 #pragma once
 #include <cub/cub.cuh>
 

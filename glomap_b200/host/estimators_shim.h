@@ -1103,6 +1103,133 @@ image_t PruneWeaklyConnectedImages(FrameMap& frames, ImageMap& images, TrackMap&
 }
 
 // ---------------------------------------------------------------------------
+struct TrackEstablishmentOptions {   // track_establishment.h:10-25 (field for field)
+  double thres_inconsistency = 10.;
+  int min_num_tracks_per_view = -1;
+  int min_num_view_per_track = 3;
+  int max_num_view_per_track = 100;
+  int max_num_tracks = 10000000;
+};
+
+// TrackEngine (controllers/track_establishment.{h,cc}), stage 4 of GlobalMapper::Solve, on the device.  The constructor
+// takes any options type with the reference's five fields (glomap's own TrackEstablishmentOptions inside a glomap
+// build) and copies them.
+//   EstablishFullTracks: the inlier matches of the valid pairs (sorted pair-id order) as image_id << 32 | feature_id with
+//     their pixels from Image::features -> b200sfm_tracks_establish; every track, the discarded ones with no observations,
+//     goes into `tracks` (cleared first, :7).  Returns the number of tracks.
+//   FindTracksForProblem: tracks in sorted track-id order, registered = the images whose frame is registered ->
+//     b200sfm_tracks_select; the selected tracks are copied with their observations restricted to the registered images.
+//     Returns the number selected.
+// Both return 0 and leave their output unchanged when the device call fails or a pair or observation names an unknown
+// image (message on stderr).
+// A class template (deduced from the constructor's arguments) so that it is compiled only where it is used.
+template <class ViewGraphT = ViewGraph, class ImageMap = std::unordered_map<image_t, Image>>
+class TrackEngine {
+ public:
+  template <class Options>
+  TrackEngine(const ViewGraphT& view_graph, const ImageMap& images, const Options& options)
+      : view_graph_(view_graph), images_(images) {
+    options_.thres_inconsistency = options.thres_inconsistency;
+    options_.min_num_tracks_per_view = options.min_num_tracks_per_view;
+    options_.min_num_view_per_track = options.min_num_view_per_track;
+    options_.max_num_view_per_track = options.max_num_view_per_track;
+    options_.max_num_tracks = options.max_num_tracks;
+  }
+
+  size_t EstablishFullTracks(std::unordered_map<track_t, Track>& tracks) {
+    using Pair = typename std::remove_reference<decltype(view_graph_.image_pairs.begin()->second)>::type;
+    std::map<image_pair_t, const Pair*> psorted;
+    for (const auto& [id, pr] : view_graph_.image_pairs) psorted[id] = &pr;
+    std::vector<uint64_t> g1, g2;
+    std::vector<double> xy1, xy2;
+    for (const auto& [id, pr] : psorted) {
+      if (!pr->is_valid) continue;
+      auto a = images_.find(pr->image_id1), b = images_.find(pr->image_id2);
+      if (a == images_.end() || b == images_.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return 0; }
+      for (const int k : pr->inliers) {
+        const long f1 = pr->matches(k, 0), f2 = pr->matches(k, 1);
+        if (f1 < 0 || f2 < 0 || f1 >= (long)a->second.features.size() || f2 >= (long)b->second.features.size()) {
+          std::fprintf(stderr, "b200sfm: inlier match with a feature outside its image\n");
+          return 0;
+        }
+        g1.push_back((uint64_t)pr->image_id1 << 32 | (uint64_t)f1);
+        g2.push_back((uint64_t)pr->image_id2 << 32 | (uint64_t)f2);
+        xy1.push_back(a->second.features[f1][0]); xy1.push_back(a->second.features[f1][1]);
+        xy2.push_back(b->second.features[f2][0]); xy2.push_back(b->second.features[f2][1]);
+      }
+    }
+    b200sfm_ctx* ctx = DefaultContext();
+    if (!ctx) return 0;
+    b200sfm_tracks* h = nullptr;
+    int64_t T = 0, n = 0, discarded = 0;
+    int rc = b200sfm_tracks_establish(ctx, (int64_t)g1.size(), g1.data(), g2.data(), xy1.data(), xy2.data(), options_.thres_inconsistency,
+                                      &h, &T, &n, &discarded);
+    std::vector<uint64_t> ids(T);
+    std::vector<int64_t> begin(T + 1, 0);
+    std::vector<uint32_t> img(n), feat(n);
+    if (rc == B200SFM_OK) rc = b200sfm_tracks_get(h, ids.data(), begin.data(), img.data(), feat.data());
+    b200sfm_tracks_free(h);
+    if (rc != B200SFM_OK) {
+      std::fprintf(stderr, "b200sfm: TrackEngine::EstablishFullTracks failed: %s\n", b200sfm_last_error(ctx));
+      return 0;
+    }
+    tracks.clear();
+    for (int64_t t = 0; t < T; ++t) {
+      Track& tr = tracks[(track_t)ids[t]];
+      tr.track_id = (track_t)ids[t];
+      for (int64_t k = begin[t]; k < begin[t + 1]; ++k) tr.observations.emplace_back((image_t)img[k], (feature_t)feat[k]);
+    }
+    return tracks.size();
+  }
+
+  size_t FindTracksForProblem(const std::unordered_map<track_t, Track>& tracks_full,
+                              std::unordered_map<track_t, Track>& tracks_selected) {
+    std::map<track_t, const Track*> tsorted;
+    for (const auto& [id, t] : tracks_full) tsorted[id] = &t;
+    std::vector<uint64_t> ids;
+    std::vector<int64_t> begin{0};
+    std::vector<uint32_t> obs_image;
+    for (const auto& [id, t] : tsorted) {
+      ids.push_back((uint64_t)id);
+      for (const auto& ob : t->observations) obs_image.push_back((uint32_t)ob.first);
+      begin.push_back((int64_t)obs_image.size());
+    }
+    std::set<image_t> registered;
+    for (const auto& [id, im] : images_)
+      if (im.IsRegistered()) registered.insert(id);
+    const std::vector<uint32_t> reg(registered.begin(), registered.end());
+    b200sfm_ctx* ctx = DefaultContext();
+    if (!ctx) return 0;
+    std::vector<uint8_t> keep(ids.size(), 0);
+    int64_t num = 0;
+    const int rc = b200sfm_tracks_select(ctx, (int64_t)ids.size(), ids.data(), begin.data(), obs_image.data(), (int32_t)reg.size(),
+                                         reg.data(), options_.min_num_tracks_per_view, options_.min_num_view_per_track,
+                                         options_.max_num_view_per_track, options_.max_num_tracks, keep.data(), &num);
+    if (rc != B200SFM_OK) {
+      std::fprintf(stderr, "b200sfm: TrackEngine::FindTracksForProblem failed: %s\n", b200sfm_last_error(ctx));
+      return 0;
+    }
+    std::unordered_map<track_t, Track> out;
+    size_t t = 0;
+    for (const auto& [id, tr] : tsorted) {
+      if (keep[t++]) {
+        Track& o = out[id];
+        o.track_id = id;
+        for (const auto& ob : tr->observations)
+          if (registered.count(ob.first)) o.observations.push_back(ob);
+      }
+    }
+    tracks_selected = out;
+    return tracks_selected.size();
+  }
+
+ private:
+  TrackEstablishmentOptions options_;
+  const ViewGraphT& view_graph_;
+  const ImageMap& images_;
+};
+
+// ---------------------------------------------------------------------------
 // GravityRefiner (estimators/gravity_refinement.{h,cc}), run by `rotation_averager --refine_gravity 1`, on the device
 // (b200sfm_gravity_refine): frames in sorted frame-id order, valid pairs in sorted pair-id order whose two images have
 // gravity (a frame prior and, off the rig's reference sensor, a known cam_from_rig), M = R_c2^T R_rel R_c1.  Accepted

@@ -8,8 +8,10 @@ rotations too; normalise; reprojection filters with the tightening threshold ``m
 
 It mirrors the reference's control flow so that the GPU solvers are exercised in the order, and with the option
 mutations, the real mapper uses; it is host glue (as in the reference) and owns no numerics: every solve and every
-filter goes through ``libb200sfm.so``.  Trivial frames only.  Not covered (they are COLMAP / PoseLib code in the
-reference): view-graph calibration, relative-pose estimation, track establishment, retriangulation."""
+filter goes through ``libb200sfm.so``.  Trivial frames only.  Stage 4, track establishment (``TrackEngine``:
+EstablishFullTracks, then FindTracksForProblem, both on the device), runs when ``Solve`` is given the image pairs and
+features.  Not covered here: view-graph calibration, relative-pose estimation, retriangulation (COLMAP code in the
+reference)."""
 from __future__ import annotations
 
 import dataclasses
@@ -17,6 +19,7 @@ import dataclasses
 import numpy as np
 
 from . import estimators as E, geometry as geo, processors as PR, reconstruction_pruning as RP, synthetic as S
+from . import track_establishment as TE
 
 
 @dataclasses.dataclass
@@ -46,6 +49,8 @@ class GlobalMapperOptions:
     skip_global_positioning: bool = False
     skip_bundle_adjustment: bool = False
     skip_pruning: bool = True                # global_mapper.h:41; --skip_pruning 0 turns stage 8 on
+    opt_track: TE.TrackEstablishmentOptions = dataclasses.field(default_factory=TE.TrackEstablishmentOptions)
+    skip_track_establishment: bool = False   # stage 4 runs only when Solve is given the image pairs and features
 
 
 def compact_observations(scene: S.Scene, keep: np.ndarray) -> S.Scene:
@@ -118,11 +123,15 @@ class GlobalMapper:
         return scene
 
     # -- controllers/global_mapper.cc:19-355 (stages 3, 5, 6) -----------------------------------------
-    def Solve(self, view_graph: S.ViewGraph, scene: S.Scene):
+    def Solve(self, view_graph: S.ViewGraph, scene: S.Scene, image_pairs=None, features: dict | None = None):
         """Returns (ok, scene): poses / points / intrinsics of ``scene`` estimated from the relative rotations of
-        ``view_graph`` and the tracks of ``scene`` (its poses and points are only used when a stage is skipped)."""
+        ``view_graph`` and the tracks of ``scene`` (its poses and points are only used when a stage is skipped).
+        Given ``image_pairs`` (``track_establishment.ImagePairMatches``) and ``features`` ({image_id: [n,2] pixels}; camera k
+        of ``scene`` is the k-th smallest image id), stage 4 builds the tracks on the device instead and the tracks of
+        ``scene`` are not used."""
         o, thr = self.options_, self.options_.inlier_thresholds
         scene = scene.copy()
+        track_stage = image_pairs is not None and features is not None and not o.skip_track_establishment
         # 3. rotation averaging: first run for filtering, second for the estimate (:84-116)
         if not o.skip_rotation_averaging:
             vg = view_graph
@@ -139,6 +148,17 @@ class GlobalMapper:
                     raise NotImplementedError("images outside the largest connected component must be removed by the caller")
                 self.log.append(f"rotation averaging run {run + 1}: {int((~valid).sum())} edges filtered")
             scene.quat = geo.rotmat_to_quat_xyzw_fast(R)
+        # 4. track establishment (:119-137): every image is left after stage 3 (it raises otherwise), so all are registered
+        if track_stage:
+            image_ids = sorted(int(i) for i in features)
+            if len(image_ids) != scene.C:
+                raise ValueError(f"features name {len(image_ids)} images, the scene has {scene.C} cameras")
+            full, discarded = TE.establish_full_tracks_device(image_pairs, features, o.opt_track, self.ctx)
+            sel = TE.find_tracks_for_problem_device(full, image_ids, o.opt_track, self.ctx)
+            flat = TE.tracks_to_scene(sel, features, image_ids, scene.cam_intr, scene.intr_model, scene.intr_params)
+            flat.quat, flat.trans = scene.quat, scene.trans
+            scene = flat
+            self.log.append(f"track establishment: {len(full)} tracks ({discarded} discarded), {len(sel)} selected")
         # 5. global positioning (:143-189)
         if not o.skip_global_positioning:
             bear = PR.undistort_images(scene)

@@ -10,6 +10,9 @@
   ``min_num_tracks_per_view`` -- compared as an UNSIGNED 64-bit value exactly like the reference (``track_t`` counters
   against an ``int``), so the default -1 means "no quota" -- and the ``max_num_tracks`` cut-off.
 
+Both run on the GPU as well, with the same result: ``establish_full_tracks_device`` (b200sfm_tracks_establish) and
+``find_tracks_for_problem_device`` (b200sfm_tracks_select, the greedy loop in its exact data-parallel form).
+
 Global feature id = image_id << 32 | feature_id (:48-53); a track is identified by the smallest global id of its
 component (the reference roots the union at the smaller id).  Observations inside a track are sorted by global id
 (the reference iterates an unordered_set; the order is immaterial to the solvers).
@@ -161,6 +164,10 @@ def establish_full_tracks_device(pairs, features: dict, options: TrackEstablishm
 
 
 def find_tracks_for_problem(tracks: Tracks, registered_images, options: TrackEstablishmentOptions | None = None) -> Tracks:
+    """FindTracksForProblem on the host, a loop over the tracks.  Only ``min_num_tracks_per_view`` is compared as an
+    unsigned value here; the reference also converts ``min_num_view_per_track``, ``max_num_view_per_track`` and
+    ``max_num_tracks`` to unsigned, so for a NEGATIVE value of one of those three this loop differs from the reference
+    (and from ``find_tracks_for_problem_device``, which follows the reference).  Non-negative values agree."""
     o = options or TrackEstablishmentOptions()
     reg = np.asarray(sorted(int(i) for i in registered_images), np.int64)
     lens = np.diff(tracks.begin)
@@ -195,6 +202,59 @@ def find_tracks_for_problem(tracks: Tracks, registered_images, options: TrackEst
         return Tracks(np.zeros(0, np.uint64), np.zeros(1, np.int64), np.zeros(0, np.uint32), np.zeros(0, np.uint32))
     return Tracks(np.asarray(out_ids, np.uint64), np.asarray(out_begin, np.int64), np.concatenate(out_img).astype(np.uint32),
                   np.concatenate(out_feat).astype(np.uint32))
+
+
+def restrict_to_images(tracks: Tracks, image_ids) -> Tracks:
+    """Observations restricted to ``image_ids`` (track_temp of FindTracksForProblem, :181-190); tracks keep their order."""
+    m = np.isin(tracks.obs_image, np.asarray([int(i) for i in image_ids], np.uint32))
+    t = np.repeat(np.arange(len(tracks)), np.diff(tracks.begin))
+    lens = np.bincount(t[m], minlength=len(tracks))
+    return Tracks(tracks.track_ids.copy(), np.concatenate([[0], np.cumsum(lens)]).astype(np.int64), tracks.obs_image[m],
+                  tracks.obs_feature[m])
+
+
+def _subset(tracks: Tracks, idx: np.ndarray) -> Tracks:
+    lens = np.diff(tracks.begin)[idx]
+    out_begin = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    pos = np.repeat(np.asarray(tracks.begin, np.int64)[idx] - out_begin[:-1], lens) + np.arange(out_begin[-1])
+    return Tracks(tracks.track_ids[idx], np.concatenate([[0], np.cumsum(lens)]).astype(np.int64), tracks.obs_image[pos],
+                  tracks.obs_feature[pos])
+
+
+def find_tracks_for_problem_device(tracks: Tracks, registered_images, options: TrackEstablishmentOptions | None = None,
+                                   ctx=None) -> Tracks:
+    """FindTracksForProblem on the GPU (b200sfm_tracks_select).  Same result and layout as ``find_tracks_for_problem``:
+    the selected tracks in descending (length, id) order, observations restricted to the registered images.  The four
+    options are compared as unsigned values, as in the reference (see ``find_tracks_for_problem``).  Two tracks with one
+    id raise ``_lib.B200Error`` (INVALID_ARG)."""
+    import ctypes as ct
+
+    from . import _lib, estimators as E
+    o = options or TrackEstablishmentOptions()
+    for f in ("min_num_tracks_per_view", "min_num_view_per_track", "max_num_view_per_track", "max_num_tracks"):
+        v = int(getattr(o, f))
+        if not -2**31 <= v < 2**31:
+            raise ValueError(f"{f} = {v} is outside the range of int")
+    ctx = ctx or E.default_context()
+    T = len(tracks)
+    ids = np.ascontiguousarray(tracks.track_ids, np.uint64)
+    begin = np.ascontiguousarray(tracks.begin, np.int64)
+    img = np.ascontiguousarray(tracks.obs_image, np.uint32)
+    if len(begin) != T + 1 or len(img) != int(begin[-1]):
+        raise ValueError("tracks.begin must have len(tracks) + 1 entries and end at len(tracks.obs_image)")
+    reg = np.ascontiguousarray([int(i) for i in registered_images], np.uint32)
+    keep = np.zeros(T, np.uint8)
+    num = ct.c_int64()
+    ptr = lambda a: a.ctypes.data_as(ct.c_void_p) if len(a) else None   # noqa: E731
+    _lib.check(ctx.handle, ctx.lib.b200sfm_tracks_select(ctx.handle, T, ptr(ids), begin.ctypes.data_as(ct.c_void_p), ptr(img),
+                                                         len(reg), ptr(reg), int(o.min_num_tracks_per_view),
+                                                         int(o.min_num_view_per_track), int(o.max_num_view_per_track),
+                                                         int(o.max_num_tracks), ptr(keep), ct.byref(num)))
+    sel = np.nonzero(keep)[0]
+    assert len(sel) == num.value
+    lens = np.diff(begin)[sel]
+    sel = sel[np.lexsort((ids[sel], lens))[::-1]]            # descending (length, id), the reference's processing order
+    return restrict_to_images(_subset(tracks, sel), reg)
 
 
 def tracks_to_scene(tracks: Tracks, features: dict, image_ids, cam_intr, intr_model, intr_params):

@@ -244,8 +244,8 @@ void b200sfm_ba_problem_free(b200sfm_ba_problem* p);
  * gid = image_id << 32 | feature_id (:48-53) with the pixel of both features (Image::features).  Result: tracks in
  * ascending track id (= smallest global id of the component, the reference's root rule :56-60), observations of a track
  * in ascending global id; a track with two features of ONE image further apart than thres_inconsistency pixels keeps its
- * id but loses its observations (:118-131) and is counted in num_discarded.  The order-dependent greedy selection
- * FindTracksForProblem (:153-234) stays on the host. */
+ * id but loses its observations (:118-131) and is counted in num_discarded.  The selection FindTracksForProblem is
+ * b200sfm_tracks_select below. */
 typedef struct b200sfm_tracks b200sfm_tracks;
 int b200sfm_tracks_establish(b200sfm_ctx* ctx, int64_t num_matches, const uint64_t* gid1, const uint64_t* gid2,
                              const double* xy1 /*[M][2]*/, const double* xy2 /*[M][2]*/, double thres_inconsistency,
@@ -253,6 +253,29 @@ int b200sfm_tracks_establish(b200sfm_ctx* ctx, int64_t num_matches, const uint64
 int b200sfm_tracks_get(b200sfm_tracks* t, uint64_t* track_ids /*[T]*/, int64_t* begin /*[T+1]*/, uint32_t* obs_image /*[n]*/,
                        uint32_t* obs_feature /*[n]*/);
 void b200sfm_tracks_free(b200sfm_tracks* t);
+/* TrackEngine::FindTracksForProblem (track_establishment.cc:153-227) on the device, through its exact data-parallel form
+ * (a per-image counter saturates, so an observation counts iff its rank among the registered observations of its image in
+ * processing order is <= the quota).  Input: T tracks as host arrays, a CSR over the image ids of their observations in any
+ * order, and the registered images (any order, repeats allowed).  The reference's rules:
+ *   - candidates: L >= min_num_view_per_track and L <= max_num_view_per_track, L = number of observations (registered or
+ *     not), processed in descending (L, track id) order;
+ *   - a candidate with fewer than min_num_view_per_track DISTINCT registered images is skipped;
+ *   - a registered observation increments its image's counter while the counter is <= min_num_tracks_per_view; a track
+ *     with an increment is selected;
+ *   - the walk stops once more than max_num_tracks tracks are selected (so at most max_num_tracks + 1 are).
+ * The four options are ints compared with unsigned values, as in the reference: min_num_tracks_per_view < 0 (the default
+ * -1) means no quota, min_num_view_per_track < 0 selects nothing, max_num_view_per_track < 0 removes the upper length
+ * bound, max_num_tracks < 0 removes the cap.
+ * Output: keep[t] = 1 for a selected track and num_selected; the caller restricts the selected tracks' observations to the
+ * registered images.  Two tracks with one id, begin[0] != 0, a decreasing begin, null arrays for T > 0 or n > 0, and more
+ * than 2^31 - 2 tracks or observations give B200SFM_ERR_INVALID_ARG (checked before the device is touched, except the
+ * duplicate ids).  T == 0 returns num_selected = 0.  Runs on the context's device without a collective: on a
+ * distributed context each rank selects from the tracks it is given. */
+int b200sfm_tracks_select(b200sfm_ctx* ctx, int64_t num_tracks, const uint64_t* track_ids /*[T]*/,
+                          const int64_t* begin /*[T+1] CSR over obs_image*/, const uint32_t* obs_image /*[n]*/,
+                          int32_t num_registered, const uint32_t* registered_image_ids /*[R]*/,
+                          int32_t min_num_tracks_per_view, int32_t min_num_view_per_track, int32_t max_num_view_per_track,
+                          int32_t max_num_tracks, uint8_t* keep /*[T] out, 1 = selected*/, int64_t* num_selected);
 
 /* ---- image pair inliers ------------------------------------------------------------------------------------------------
  * ImagePairsInlierCount (glomap/processors/image_pair_inliers.cc:200-213), the scorers ScoreErrorEssential / Fundamental /
