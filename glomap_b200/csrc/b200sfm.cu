@@ -7,6 +7,7 @@
 #include "context.cuh"
 #include "gp_solver.cuh"
 #include "gravity_kernels.cuh"
+#include "mst_kernels.cuh"
 #include "pair_kernels.cuh"
 #include "prune_kernels.cuh"
 #include "ra_solver.cuh"
@@ -1156,6 +1157,55 @@ int b200sfm_ra_solve_rig(b200sfm_ctx* ctx, const b200sfm_ra_opts* opts, int32_t 
   });
   if (stats) *stats = st;
   return finish(ctx, rc);
+}
+
+int b200sfm_ra_mst_init(b200sfm_ctx* ctx, int32_t n_nodes, int64_t n_edges, const int32_t* ei, const int32_t* ej,
+                        const double* R_rel, const double* weight, int32_t root, double* R, int32_t* parent,
+                        b200sfm_mst_stats* stats) {
+  const auto t0 = std::chrono::steady_clock::now();
+  if (!ctx || !R || n_nodes < 1 || n_edges < 0) return B200SFM_ERR_INVALID_ARG;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (n_edges > 0 && (!ei || !ej || !R_rel || !weight)) return invalid("null edge array");
+  if (n_edges > INT32_MAX) return invalid("more than 2^31 - 1 edges");
+  if (root < 0 || root >= n_nodes) return invalid("root out of range");
+  double wmax = -INFINITY;
+  for (int64_t e = 0; e < n_edges; ++e) {
+    if (ei[e] < 0 || ei[e] >= n_nodes || ej[e] < 0 || ej[e] >= n_nodes) return invalid("edge index out of range");
+    if (!std::isfinite(weight[e])) return invalid("non-finite edge weight");
+    wmax = std::max(wmax, weight[e]);
+  }
+  if (ctx->world > 1) {
+    ctx->err = "the spanning tree needs every edge: single-rank contexts only";
+    return B200SFM_ERR_UNSUPPORTED;
+  }
+  const long long launches0 = ctx->launches;
+  b200::MstStats st;
+  int rc = B200SFM_OK;
+  if (n_edges == 0) {   // the root alone
+    if (parent) {
+      std::fill(parent, parent + n_nodes, -1);
+      parent[root] = root;
+    }
+    st.num_reached = 1;
+  } else {
+    rc = guarded(ctx, [&]() {
+      B200_CUDA_OK(cudaSetDevice(ctx->device));
+      b200::MstRunner r(ctx);
+      r.run(n_nodes, (int)n_edges, ei, ej, R_rel, weight, wmax, root, R, parent, st);
+      B200_CUDA_OK(cudaGetLastError());   // a failed launch of this call is reported here, not left pending for the next caller
+      return (int)B200SFM_OK;
+    });
+  }
+  if (stats) {
+    *stats = b200sfm_mst_stats{};
+    stats->num_reached = st.num_reached;
+    stats->num_tree_edges = st.num_tree_edges;
+    stats->boruvka_rounds = st.boruvka_rounds;
+    stats->max_depth = st.max_depth;
+    stats->kernel_launches = ctx->launches - launches0;
+    stats->ms_total = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  }
+  return rc;
 }
 
 }  // extern "C"

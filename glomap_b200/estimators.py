@@ -549,7 +549,7 @@ def initialize_from_maximum_spanning_tree(vg, R_init: np.ndarray | None = None) 
     """Host-side InitializeFromMaximumSpanningTree
     (global_rotation_averaging.cc:87-138 + math/tree.cc:78-170): Kruskal on
     (max_weight - weight), BFS from index 0, compose R_child from the parent
-    along tree edges.  O(E log E), stays on the host (SURVEY.md 8(a) row a4)."""
+    along tree edges.  O(E log E); the reference that initialize_from_maximum_spanning_tree_device is tested against."""
     import scipy.sparse as sp
     from scipy.sparse.csgraph import breadth_first_order, minimum_spanning_tree
     n = vg.n_images
@@ -571,6 +571,33 @@ def initialize_from_maximum_spanning_tree(vg, R_init: np.ndarray | None = None) 
         else:                                # R_curr = R_rel R_parent                          (.cc:130-134)
             R[node] = vg.R_rel[lut[(par, int(node))]] @ R[par]
     return R
+
+
+# EstimateRotations initialises on the device from this many edges up (single-rank contexts).  On an H100 the device
+# call (about 0.6 ms of fixed cost: copies, launches, a few synchronisations) was faster than the host function at every
+# size measured, down to 45 edges, but by no more than about 0.2 ms below 200 edges (profiles/mst_init_bench.py, DESIGN.md 6.w);
+# the smallest graphs stay on the host, where the two cost the same to within that margin.
+MST_DEVICE_MIN_EDGES = 100
+
+
+def initialize_from_maximum_spanning_tree_device(vg, R_init: np.ndarray | None = None, ctx: Context | None = None,
+                                                 root: int = 0, stats: _lib.MSTStats | None = None):
+    """InitializeFromMaximumSpanningTree on the device (b200sfm_ra_mst_init): the same tree and composition as
+    initialize_from_maximum_spanning_tree, rooted at ``root``, which starts from R_init[root] (the identity without
+    R_init).  Unreached nodes keep R_init.  Returns (R [n,3,3], parent [n]: parent[root] = root, unreached -1);
+    ``stats``, when given, receives the call's b200sfm_mst_stats."""
+    ctx = ctx or default_context()
+    n = vg.n_images
+    R = np.tile(np.eye(3), (n, 1, 1)) if R_init is None else np.array(R_init, dtype=np.float64, order="C", copy=True)
+    if R.shape != (n, 3, 3):
+        raise ValueError(f"R_init must be [{n},3,3], got {R.shape}")
+    parent = np.empty(n, np.int32)
+    st = stats if stats is not None else _lib.MSTStats()
+    ei, ej = _c(vg.ei, np.int32), _c(vg.ej, np.int32)
+    Rr, w = _c(np.reshape(vg.R_rel, (-1, 9)), np.float64), _c(vg.weight, np.float64)
+    _lib.check(ctx.handle, ctx.lib.b200sfm_ra_mst_init(ctx.handle, n, len(ei), _ptr(ei), _ptr(ej), _ptr(Rr), _ptr(w), root,
+                                                       _ptr(R), _ptr(parent), ct.byref(st)))
+    return R, parent
 
 
 def rig_view_graph(vg, img_frame, img_sensor, sensor_quat, R_gt_frames=None):
@@ -637,11 +664,14 @@ class RotationEstimator:
         o = self.options_
         n = vg.n_images
         use_grav = o.use_gravity and gravity is not None
+        ctx = self.ctx or default_context()
         if not o.skip_initialization and not o.use_gravity:
-            R0 = initialize_from_maximum_spanning_tree(vg, R_init)
+            if ctx.world_size == 1 and vg.E >= MST_DEVICE_MIN_EDGES:
+                R0, _ = initialize_from_maximum_spanning_tree_device(vg, R_init, ctx)
+            else:
+                R0 = initialize_from_maximum_spanning_tree(vg, R_init)
         else:
             R0 = np.tile(np.eye(3), (n, 1, 1)) if R_init is None else np.asarray(R_init, dtype=np.float64)
-        ctx = self.ctx or default_context()
         co = o.to_c()
         st = _lib.RAStats()
         ei, ej = _c(vg.ei, np.int32), _c(vg.ej, np.int32)
