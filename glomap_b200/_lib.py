@@ -97,6 +97,17 @@ class MSTStats(ct.Structure):
         return {f: getattr(self, f) for f, _ in self._fields_}
 
 
+class RigInitStats(ct.Structure):
+    _fields_ = [
+        ("num_ref_frames", c_int32), ("num_cam_samples", c_int32), ("num_cams_averaged", c_int32),
+        ("num_frame_samples", c_int32), ("num_frames_averaged", c_int32), ("reserved0", c_int32),
+        ("kernel_launches", c_int64), ("ms_total", c_double),
+    ]
+
+    def as_dict(self):
+        return {f: getattr(self, f) for f, _ in self._fields_ if f != "reserved0"}
+
+
 class PruneStats(ct.Structure):
     _fields_ = [
         ("covisible_pairs", c_int64), ("pairs_min5", c_int64), ("visibility_edges", c_int64), ("strong_threshold", c_double),
@@ -181,6 +192,7 @@ PROTOTYPES = {
     "b200sfm_ra_solve": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int64] + [c_void_p] * 4 + [c_int32, c_void_p, P(RAStats)]),
     "b200sfm_ra_solve_rig": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int32, c_int64] + [c_void_p] * 8 + [c_int32, c_void_p, P(RAStats)]),
     "b200sfm_ra_mst_init": (c_int32, [c_void_p, c_int32, c_int64] + [c_void_p] * 4 + [c_int32, c_void_p, c_void_p, P(MSTStats)]),
+    "b200sfm_rig_rotations_from_images": (c_int32, [c_void_p, c_int64, c_int32, c_int32] + [c_void_p] * 10 + [P(RigInitStats)]),
     "b200sfm_vgc_default_opts": (None, [P(VGCOpts)]),
     "b200sfm_view_graph_calibrate": (c_int32, [c_void_p, P(VGCOpts), c_int32, c_void_p, c_void_p, c_void_p, c_int64]
                                      + [c_void_p] * 6 + [P(LMStats)]),

@@ -11,6 +11,7 @@
 #include "pair_kernels.cuh"
 #include "prune_kernels.cuh"
 #include "ra_solver.cuh"
+#include "rig_init_kernels.cuh"
 #include "track_kernels.cuh"
 #include "track_select_kernels.cuh"
 #include "vgc_solver.cuh"
@@ -1202,6 +1203,52 @@ int b200sfm_ra_mst_init(b200sfm_ctx* ctx, int32_t n_nodes, int64_t n_edges, cons
     stats->num_tree_edges = st.num_tree_edges;
     stats->boruvka_rounds = st.boruvka_rounds;
     stats->max_depth = st.max_depth;
+    stats->kernel_launches = ctx->launches - launches0;
+    stats->ms_total = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  }
+  return rc;
+}
+
+int b200sfm_rig_rotations_from_images(b200sfm_ctx* ctx, int64_t n_images, int32_t n_frames, int32_t n_cameras,
+                                      const int32_t* image_frame, const int32_t* image_camera,
+                                      const uint8_t* image_estimated, const double* cam_from_world,
+                                      const int32_t* frame_ref_camera, const uint8_t* camera_known, double* cam_from_rig,
+                                      int32_t* cam_samples, double* rig_from_world, int32_t* frame_samples,
+                                      b200sfm_rig_init_stats* stats) {
+  const auto t0 = std::chrono::steady_clock::now();
+  if (!ctx) return B200SFM_ERR_INVALID_ARG;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (!image_frame || !image_camera || !cam_from_world || !frame_ref_camera || !camera_known || !cam_from_rig || !rig_from_world)
+    return invalid("null array");
+  if (n_images < 1 || n_images > INT32_MAX) return invalid("n_images must be in [1, 2^31 - 1]");
+  if (n_frames < 1 || n_cameras < 1) return invalid("n_frames and n_cameras must be at least 1");
+  for (int64_t i = 0; i < n_images; ++i) {
+    if (image_frame[i] < -1 || image_frame[i] >= n_frames) return invalid("image frame index out of range");
+    if (image_camera[i] < 0 || image_camera[i] >= n_cameras) return invalid("image camera index out of range");
+  }
+  for (int32_t f = 0; f < n_frames; ++f)
+    if (frame_ref_camera[f] < 0 || frame_ref_camera[f] >= n_cameras) return invalid("frame reference camera out of range");
+  if (ctx->world > 1) {
+    ctx->err = "the frames' samples span every image: single-rank contexts only";
+    return B200SFM_ERR_UNSUPPORTED;
+  }
+  const long long launches0 = ctx->launches;
+  b200::RigInitStats st;
+  const int rc = guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    b200::RigInitRunner r(ctx);
+    r.run((int)n_images, n_frames, n_cameras, image_frame, image_camera, image_estimated, cam_from_world, frame_ref_camera,
+          camera_known, cam_from_rig, cam_samples, rig_from_world, frame_samples, st);
+    B200_CUDA_OK(cudaGetLastError());   // a failed launch of this call is reported here, not left pending for the next caller
+    return (int)B200SFM_OK;
+  });
+  if (stats) {
+    *stats = b200sfm_rig_init_stats{};
+    stats->num_ref_frames = st.num_ref_frames;
+    stats->num_cam_samples = st.num_cam_samples;
+    stats->num_cams_averaged = st.num_cams_averaged;
+    stats->num_frame_samples = st.num_frame_samples;
+    stats->num_frames_averaged = st.num_frames_averaged;
     stats->kernel_launches = ctx->launches - launches0;
     stats->ms_total = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   }

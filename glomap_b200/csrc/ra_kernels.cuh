@@ -765,6 +765,31 @@ __global__ void ra_update(int n, int n_frames, double* __restrict__ theta, const
   }
 }
 
+// colmap::AverageQuaternions with unit weights (UPSTREAM-UNVERIFIED restatement), in two halves shared by ra_update_cams
+// and rig_init_kernels.cuh: the packed symmetric 4x4 sum q q^T (10 entries, row by row) and its dominant eigenvector.
+__device__ __forceinline__ void quat_outer_acc(double M[10], const double q[4]) {
+  int idx = 0;
+#pragma unroll
+  for (int a = 0; a < 4; ++a)
+#pragma unroll
+    for (int b = a; b < 4; ++b) M[idx++] += q[a] * q[b];
+}
+// dominant eigenvector by power iteration from the first quaternion q0 (the averaged rotations are estimates of one
+// rotation: the gap to the second eigenvalue is large); the sign follows q0
+__device__ __forceinline__ void quat_avg_power(const double M[10], const double q0[4], double v[4]) {
+  const double S[4][4] = {{M[0], M[1], M[2], M[3]}, {M[1], M[4], M[5], M[6]}, {M[2], M[5], M[7], M[8]}, {M[3], M[6], M[8], M[9]}};
+  v[0] = q0[0]; v[1] = q0[1]; v[2] = q0[2]; v[3] = q0[3];
+  for (int it = 0; it < 200; ++it) {
+    double u[4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a) u[a] = S[a][0] * v[0] + S[a][1] * v[1] + S[a][2] * v[2] + S[a][3] * v[3];
+    const double nn = sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2] + u[3] * u[3]);
+    if (!(nn > 0.0)) break;
+#pragma unroll
+    for (int a = 0; a < 4; ++a) v[a] = u[a] / nn;
+  }
+}
+
 // Unknown cam_from_rig rotations (.cc:646-693): for every frame f that holds an image of camera c the updated rotation
 // is R_c R_f exp(-step_c) R_f^T (R_f = the frame's ALREADY UPDATED rotation); the new R_c is the quaternion average
 // (colmap::AverageQuaternions, unit weights: dominant eigenvector of sum q q^T) over those frames.  One warp per camera.
@@ -811,29 +836,14 @@ __global__ void __launch_bounds__(128) ra_update_cams(int n_frames, int n_cams, 
       tt = 0.5 / tt;
       q[3] = (P[3 * k + j] - P[3 * j + k]) * tt; q[j] = (P[3 * j + i] + P[3 * i + j]) * tt; q[k] = (P[3 * k + i] + P[3 * i + k]) * tt;
     }
-    int idx = 0;
-#pragma unroll
-    for (int a = 0; a < 4; ++a)
-#pragma unroll
-      for (int b = a; b < 4; ++b) M[idx++] += q[a] * q[b];
+    quat_outer_acc(M, q);
     if (!have0) { q0[0] = q[0]; q0[1] = q[1]; q0[2] = q[2]; q0[3] = q[3]; have0 = true; }
   }
 #pragma unroll
   for (int k = 0; k < 10; ++k) M[k] = warp_sum(M[k]);
   if (lane != 0 || cf_begin[c + 1] == cf_begin[c]) return;
-  // dominant eigenvector by power iteration from the first quaternion (the averaged rotations are estimates of one
-  // rotation: the gap to the second eigenvalue is large)
-  const double S[4][4] = {{M[0], M[1], M[2], M[3]}, {M[1], M[4], M[5], M[6]}, {M[2], M[5], M[7], M[8]}, {M[3], M[6], M[8], M[9]}};
-  double v[4] = {q0[0], q0[1], q0[2], q0[3]};
-  for (int it = 0; it < 200; ++it) {
-    double u[4];
-#pragma unroll
-    for (int a = 0; a < 4; ++a) u[a] = S[a][0] * v[0] + S[a][1] * v[1] + S[a][2] * v[2] + S[a][3] * v[3];
-    const double nn = sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2] + u[3] * u[3]);
-    if (!(nn > 0.0)) break;
-#pragma unroll
-    for (int a = 0; a < 4; ++a) v[a] = u[a] / nn;
-  }
+  double v[4];
+  quat_avg_power(M, q0, v);
   double R[9], out[3];
   quat_to_R(v, R);
   R_to_aa(R, out);

@@ -24,6 +24,7 @@ inline bool AllSensorsCalibrated(const glomap::Rig& rig) {
   return true;
 }
 inline bool IsRefSensor(const glomap::Rig& rig, glomap::camera_t camera_id) { return rig.RefSensorId().id == camera_id; }
+inline glomap::camera_t RefCameraId(const glomap::Rig& rig) { return rig.RefSensorId().id; }
 inline bool HasCamFromRig(const glomap::Rig& rig, glomap::camera_t camera_id) {
   return rig.MaybeSensorFromRig(glomap::sensor_t(glomap::SensorType::CAMERA, camera_id)).has_value();
 }
@@ -186,6 +187,7 @@ inline void SetCamFromRig(b200host::Rig& rig, b200host::camera_t camera_id, cons
 // every non-reference sensor of the rig has a cam_from_rig (global_rotation_averaging.cc:47-59)
 inline bool AllSensorsCalibrated(const b200host::Rig& rig) { return rig.uncalibrated.empty(); }
 inline bool IsRefSensor(const b200host::Rig& rig, b200host::camera_t camera_id) { return camera_id == rig.ref_camera_id; }
+inline b200host::camera_t RefCameraId(const b200host::Rig& rig) { return rig.ref_camera_id; }
 inline bool HasCamFromRig(const b200host::Rig& rig, b200host::camera_t camera_id) { return rig.cam_from_rig.count(camera_id) != 0; }
 inline void RAlignRowMajor(const b200host::Frame& f, double out[9]) {
   for (int k = 0; k < 9; ++k) out[k] = f.gravity_info.R_align[k];

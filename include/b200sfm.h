@@ -489,6 +489,59 @@ int b200sfm_ra_mst_init(b200sfm_ctx* ctx, int32_t n_nodes, int64_t n_edges, cons
                         const double* R_rel, const double* weight, int32_t root, double* R, int32_t* parent,
                         b200sfm_mst_stats* stats);
 
+typedef struct {
+  int32_t num_ref_frames;       /* frames with a registered reference image */
+  int32_t num_cam_samples;      /* samples over all cameras (rule 2) */
+  int32_t num_cams_averaged;    /* unknown cameras that got an average (rule 3) */
+  int32_t num_frame_samples;    /* samples over all frames (rule 4) */
+  int32_t num_frames_averaged;  /* frames that got an average */
+  int32_t reserved0;
+  int64_t kernel_launches;
+  double ms_total;              /* host wall clock of the call */
+} b200sfm_rig_init_stats;
+
+/* ConvertRotationsFromImageToRig (glomap/estimators/rotation_initializer.cc:7-125) on flat arrays in sorted-id order:
+ * per-image cam_from_world rotations -> the cam_from_rig rotations of the unknown cameras and the frames' rig_from_world
+ * rotations.  Quaternions are xyzw (Eigen's coeffs() order) and need not be normalised.
+ *   image_frame [I]        frame index of the image, -1 when it is not registered
+ *   image_camera [I]       camera index
+ *   image_estimated [I]    1 when cam_from_world holds an estimate for the image (the reference's cam_from_worlds map);
+ *                          NULL: every image
+ *   cam_from_world [I][4]
+ *   frame_ref_camera [F]   the reference camera of the frame's rig
+ *   camera_known [K]       1 when the camera's cam_from_rig is known (MaybeSensorFromRig has a value); pass the reference
+ *                          cameras as known, with the identity
+ *   cam_from_rig [K][4]    in: the known rotations; out: the averaged ones (rows of other cameras untouched)
+ *   cam_samples [K]        out, or NULL: the number of samples of each camera (0 for a known one)
+ *   rig_from_world [F][4]  in/out: a frame without a sample keeps its input
+ *   frame_samples [F]      out, or NULL
+ * Rules (images in ascending index; the reference's order is Frame::ImageIds()):
+ *   1. the reference image of frame f is its registered image of smallest index whose camera is frame_ref_camera[f]
+ *      (.cc:24-43, the first in ImageIds()); a frame without one gives no camera sample
+ *   2. every registered image i of a frame with reference image r whose camera is neither the frame's reference camera
+ *      nor known gives its camera the sample q_i conj(q_r) (.cc:45-73); the reference .at()-throws when i or r has no
+ *      estimate, here such a sample is skipped
+ *   3. an unknown camera with at least one sample gets their average (.cc:79-88; the caller sets its translation to NaN);
+ *      a camera without a sample stays unknown
+ *   4. every frame averages over its registered, estimated images (.cc:91-122): the reference image contributes q_i,
+ *      another image whose camera is known or was averaged in rule 3 contributes conj(q_cam_from_rig) q_i, any other
+ *      is skipped.  The reference re-averages inside the image loop; its final value is the average over all samples
+ *   5. the average is colmap::AverageQuaternions with unit weights (UPSTREAM-UNVERIFIED restatement): the dominant
+ *      eigenvector of sum q q^T over the normalised samples, by the power iteration ra_update_cams uses (200 steps from
+ *      the first sample: exact to rounding when the samples estimate one rotation, as they do here; samples spread
+ *      over very different rotations converge more slowly); a single sample is returned as it is (normalised).  The
+ *      sign is canonical: w >= 0
+ *   6. sums run in a fixed order without floating-point atomics: repeated calls give bit-identical outputs
+ * A null context or array (but image_estimated, cam_samples, frame_samples, stats), n_images < 1 or > INT32_MAX,
+ * n_frames < 1, n_cameras < 1, and a frame or camera index out of range give B200SFM_ERR_INVALID_ARG before the device is
+ * touched; a context with more than one rank gives B200SFM_ERR_UNSUPPORTED. */
+int b200sfm_rig_rotations_from_images(b200sfm_ctx* ctx, int64_t n_images, int32_t n_frames, int32_t n_cameras,
+                                      const int32_t* image_frame, const int32_t* image_camera,
+                                      const uint8_t* image_estimated, const double* cam_from_world,
+                                      const int32_t* frame_ref_camera, const uint8_t* camera_known, double* cam_from_rig,
+                                      int32_t* cam_samples, double* rig_from_world, int32_t* frame_samples,
+                                      b200sfm_rig_init_stats* stats);
+
 /* ---- view-graph calibration ---------------------------------------------------------------------------------------
  * ViewGraphCalibrator::Solve (glomap/estimators/view_graph_calibration.cc:11-185), stage 1 of GlobalMapper::Solve
  * (controllers/global_mapper.cc:41-50): one focal length per camera refined from the fundamental matrices of the image
