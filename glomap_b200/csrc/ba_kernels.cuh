@@ -13,8 +13,8 @@
 //              the default with constant intrinsics) stores 48-B A_o rows in the same buffer
 //   V[P][6], Vinv[P][6], gp[P][3]         per point (packed symmetric)
 //   U[C][21], gc[C][6], Sd[C][21], Minv[C][21]   per camera (packed symmetric)
-//   camera-order copies pt_c[Nv], xy_c[Nv], camord_obs[Nv] + segments (<= kSeg = 256 observations of ONE
-//   camera -- or of one (frame, sensor) with known rigs -- handled by one warp)
+//   camera-order copies pt_c[Nv], xy_c[Nv], camord_obs[Nv] + segments (about kSeg = 256, fewer than 1.5 kSeg,
+//   observations of ONE camera -- or of one (frame, sensor) with known rigs -- handled by one warp)
 // Point-order kernels run one CTA (kTile = 128 threads) per tile of whole points with
 // <= 128 observations (longer tracks: several chunks); one thread per observation, per-point
 // reductions through shared memory.
@@ -27,7 +27,12 @@ namespace b200 {
 constexpr int kCamRec = 8;    // q(4) t(3) packed{mask, intr idx}
 constexpr int kIntrRec = 8;   // fx fy cx cy k1 k2 model pad
 constexpr double kZEps = 1e-12;
-constexpr int kSeg = 256;     // observations per camera-order segment (one warp)
+constexpr int kSeg = 256;     // observations per camera-order segment (one warp), nominal: see seg_split
+// Number of camera-order segments of a bucket of n observations: n / kSeg rounded to the nearest (at least one), of
+// equal length (so all are shorter than 1.5 kSeg).  Every segment costs its warp the camera records, a shuffle
+// reduction and the atomics, and cutting at every kSeg would leave a warp only the few observations past a multiple of
+// kSeg (at config 4, where a (slice, camera) bucket holds 250 +- 16, a quarter of the segments would be such tails).
+__host__ __device__ constexpr int seg_split(int n) { return n <= 0 ? 0 : (n < kSeg + kSeg / 2 ? 1 : (n + kSeg / 2) / kSeg); }
 constexpr int kIntrSmem = 16; // intrinsics blocks cached in shared memory by the point-order kernels
 constexpr int kJpDoubles = 6;  // v2 point-order row: A_o = J_pt^T J_pt (packed symmetric 3x3) -> 48 B
 constexpr int kSensorRec = 16; // known rigs: R_cam_from_rig (9, row-major), t_cam_from_rig (3), intrinsics idx, pad
@@ -540,7 +545,7 @@ __global__ void __launch_bounds__(kTile, B200_K1_MIN_CTAS) ba_linearize_points(B
 
 // ---------------------------------------------------------------------------
 // K2a: camera blocks U = sum Jc^T Jc (packed 21), gc = sum Jc^T r, camera order.
-// One warp per segment (<= kSeg observations of ONE camera).
+// One warp per segment (one camera's observations, see seg_split).
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) ba_linearize_cams(BAView v, const double* __restrict__ cam_rec,
                                                         const double* __restrict__ intr_rec,

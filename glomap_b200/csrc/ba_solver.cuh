@@ -57,9 +57,9 @@ __global__ void k_cam_keys(long long N, int VC, int smul, int min_views, int sli
 }
 __global__ void k_seg_counts(int n_buckets, const int* __restrict__ bucket_count, int* __restrict__ seg_count) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
-  if (c < n_buckets) seg_count[c] = (bucket_count[c] + kSeg - 1) / kSeg;
+  if (c < n_buckets) seg_count[c] = seg_split(bucket_count[c]);
 }
-// segments of <= kSeg observations of one bucket (k_cam_keys): bucket c belongs to virtual camera c % VC
+// the seg_split(n) equal segments of one bucket (k_cam_keys): bucket c belongs to virtual camera c % VC
 __global__ void k_fill_segs(int n_buckets, int VC, int smul, const int* __restrict__ cam_begin, const int* __restrict__ seg_off,
                             const int* __restrict__ cam_intr, const int* __restrict__ sensor_intr,
                             int* __restrict__ seg_cam, int* __restrict__ seg_sensor, int* __restrict__ seg_intr,
@@ -70,13 +70,14 @@ __global__ void k_fill_segs(int n_buckets, int VC, int smul, const int* __restri
   const int vc = c % VC;
   const int frame = vc / smul, sensor = vc - frame * smul;
   const int blk = sensor_intr ? sensor_intr[sensor] : (cam_intr ? cam_intr[frame] : 0);
-  int s = seg_off[c];
-  for (int i = b; i < e; i += kSeg, ++s) {
+  const int n = e - b, ns = seg_split(n);
+  for (int j = 0; j < ns; ++j) {
+    const int s = seg_off[c] + j;
     seg_cam[s] = frame;
     if (seg_sensor) seg_sensor[s] = sensor;
     if (seg_intr) seg_intr[s] = blk;
-    seg_begin[s] = i;
-    seg_end[s] = min(i + kSeg, e);
+    seg_begin[s] = b + (int)((long long)n * j / ns);
+    seg_end[s] = b + (int)((long long)n * (j + 1) / ns);
   }
 }
 __global__ void k_gather_camorder(int Nv, const int* __restrict__ camord_obs, const int* __restrict__ obs_pt,
