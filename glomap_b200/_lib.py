@@ -173,6 +173,10 @@ PROTOTYPES = {
     "b200sfm_tracks_get": (c_int32, [c_void_p] * 5),
     "b200sfm_image_pairs_inlier_count": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
                                                    c_int64] + [c_void_p] * 9 + [c_double] * 3 + [c_void_p] * 3),
+    "b200sfm_view_graph_filter_rotations": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_int64] + [c_void_p] * 3
+                                            + [c_double, c_void_p, P(c_int64)]),
+    "b200sfm_view_graph_keep_largest_component": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_int64] + [c_void_p] * 4
+                                                  + [P(c_int32)]),
     "b200sfm_tracks_free": (None, [c_void_p]),
     "b200sfm_tracks_select": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_void_p] + [c_int32] * 4
                               + [c_void_p, P(c_int64)]),

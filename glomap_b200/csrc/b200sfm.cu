@@ -15,6 +15,7 @@
 #include "track_kernels.cuh"
 #include "track_select_kernels.cuh"
 #include "vgc_solver.cuh"
+#include "view_graph_kernels.cuh"
 
 namespace {
 
@@ -622,6 +623,52 @@ int b200sfm_image_pairs_inlier_count(b200sfm_ctx* ctx, int32_t num_images, const
                                         matches, max_epipolar_error_E, max_epipolar_error_F, max_epipolar_error_H, need.data(), is_inlier,
                                         num_inliers, score))
       throw b200::InvalidInput{"match feature index out of range of its image"};
+    return (int)B200SFM_OK;
+  });
+}
+
+// ---- view-graph passes of stage 3 -------------------------------------------------
+int b200sfm_view_graph_filter_rotations(b200sfm_ctx* ctx, int32_t num_images, const double* cam_from_world_quat_xyzw,
+                                        const uint8_t* image_registered, int64_t num_pairs, const int32_t* pair_image1,
+                                        const int32_t* pair_image2, const double* pair_quat_xyzw, double max_angle_deg,
+                                        uint8_t* pair_valid, int64_t* num_invalidated) {
+  if (!ctx || num_images < 0 || num_pairs < 0 || !num_invalidated) return B200SFM_ERR_INVALID_ARG;
+  *num_invalidated = 0;
+  if (num_pairs == 0) return B200SFM_OK;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if ((num_images > 0 && !cam_from_world_quat_xyzw) || !pair_image1 || !pair_image2 || !pair_quat_xyzw || !pair_valid)
+    return invalid("null argument");
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    b200::ViewGraphRunner r(ctx);
+    long long n = 0;
+    if (!r.filter_rotations(num_images, cam_from_world_quat_xyzw, image_registered, num_pairs, pair_image1, pair_image2,
+                            pair_quat_xyzw, max_angle_deg, pair_valid, &n))
+      throw b200::InvalidInput{"pair image index outside [0, num_images)"};
+    B200_CUDA_OK(cudaGetLastError());
+    *num_invalidated = n;
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_view_graph_keep_largest_component(b200sfm_ctx* ctx, int32_t num_frames, int32_t num_images, const int32_t* image_frame,
+                                              int64_t num_pairs, const int32_t* pair_image1, const int32_t* pair_image2,
+                                              uint8_t* pair_valid, uint8_t* frame_registered, int32_t* num_registered_images) {
+  if (!ctx || num_frames < 0 || num_images < 0 || num_pairs < 0 || !num_registered_images) return B200SFM_ERR_INVALID_ARG;
+  *num_registered_images = 0;
+  if (num_pairs == 0) return B200SFM_OK;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if ((num_images > 0 && !image_frame) || (num_frames > 0 && !frame_registered) || !pair_image1 || !pair_image2 || !pair_valid)
+    return invalid("null argument");
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    b200::ViewGraphRunner r(ctx);
+    int n = 0;
+    if (!r.keep_largest_component(num_frames, num_images, image_frame, num_pairs, pair_image1, pair_image2, pair_valid,
+                                  frame_registered, &n))
+      throw b200::InvalidInput{"pair image index outside [0, num_images) or image_frame outside [0, num_frames)"};
+    B200_CUDA_OK(cudaGetLastError());
+    *num_registered_images = n;
     return (int)B200SFM_OK;
   });
 }

@@ -903,7 +903,128 @@ struct RelPoseFilter {
     for (auto& [id, pr] : view_graph.image_pairs)   // 0 matches: NaN, not below the threshold -- the pair stays valid
       if (pr.is_valid && pr.inliers.size() / double(pr.matches.rows()) < min_inlier_ratio) pr.is_valid = false;
   }
+  // relpose_filter.cc:7-33 on the device (b200sfm_view_graph_filter_rotations): images are flattened in sorted-id order
+  // with their cam_from_world rotation (cam_from_rig * rig_from_world for a non-reference camera of a rig) and their
+  // registration, the valid pairs in sorted pair-id order.  A registered image whose frame has no pose, or whose
+  // cam_from_rig is unknown, gets a NaN rotation, so its pairs are kept.  Returns the number of pairs invalidated; -1 and
+  // nothing changed when a pair names an unknown image or the device call fails (message on stderr).
+  template <class ViewGraphT, class ImageMap>
+  static int64_t FilterRotations(ViewGraphT& view_graph, const ImageMap& images, double max_angle) {
+    using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
+    using Img = typename ImageMap::mapped_type;
+    std::map<image_t, const Img*> isorted;
+    for (auto& [id, im] : images) isorted[id] = &im;
+    std::map<image_t, int32_t> iidx;
+    std::vector<double> quat;
+    std::vector<uint8_t> reg;
+    const double nan = std::numeric_limits<double>::quiet_NaN();
+    for (auto& [id, im] : isorted) {
+      iidx[id] = (int32_t)reg.size();
+      reg.push_back(im->IsRegistered() ? 1 : 0);
+      double q[4] = {nan, nan, nan, nan};
+      if (reg.back() && im->frame_ptr->HasPose()) {
+        const double* r = im->frame_ptr->RigFromWorld().rotation.coeffs().data();
+        const auto* rig = im->frame_ptr->RigPtr();
+        double c[4];
+        if (im->HasTrivialFrame() || !rig || b200host_adapt::IsRefSensor(*rig, im->camera_id)) {
+          std::copy(r, r + 4, q);
+        } else if (b200host_adapt::FrameCamFromRig(*im->frame_ptr, im->camera_id, c)) {
+          QuatMul(c, r, q);
+        }
+      }
+      quat.insert(quat.end(), q, q + 4);
+    }
+    std::map<image_pair_t, Pair*> psorted;
+    for (auto& [id, pr] : view_graph.image_pairs)
+      if (pr.is_valid) psorted[id] = &pr;
+    std::vector<Pair*> pairs;
+    std::vector<int32_t> img1, img2;
+    std::vector<double> rel;
+    for (auto& [id, pr] : psorted) {
+      auto a = iidx.find(pr->image_id1), b = iidx.find(pr->image_id2);
+      if (a == iidx.end() || b == iidx.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return -1; }
+      pairs.push_back(pr);
+      img1.push_back(a->second);
+      img2.push_back(b->second);
+      const double* q = pr->cam2_from_cam1.rotation.coeffs().data();
+      rel.insert(rel.end(), q, q + 4);
+    }
+    if (pairs.empty()) return 0;
+    b200sfm_ctx* ctx = DefaultContext();
+    if (!ctx) return -1;
+    std::vector<uint8_t> valid(pairs.size(), 1);
+    int64_t n = 0;
+    const int rc = b200sfm_view_graph_filter_rotations(ctx, (int32_t)reg.size(), quat.data(), reg.data(), (int64_t)pairs.size(),
+                                                       img1.data(), img2.data(), rel.data(), max_angle, valid.data(), &n);
+    if (rc != B200SFM_OK) {
+      std::fprintf(stderr, "b200sfm: FilterRotations failed: %s\n", b200sfm_last_error(ctx));
+      return -1;
+    }
+    for (size_t e = 0; e < pairs.size(); ++e)
+      if (!valid[e]) pairs[e]->is_valid = false;
+    return n;
+  }
 };
+
+// ViewGraph::KeepLargestConnectedComponents (scene/view_graph.cc:56-97) on the device
+// (b200sfm_view_graph_keep_largest_component): frames, images and pairs are flattened in sorted-id order; is_registered of
+// every frame and is_valid of every pair are written back.  Equally large components: the one holding the smallest frame
+// id.  Returns the number of registered images; 0 and nothing changed without a valid pair, and also when a pair names an
+// unknown image, an image an unknown frame, or the device call fails (message on stderr).  The host version
+// KeepLargestConnectedComponents below computes the same and is what SolveRotationAveraging and the CLI call.
+template <class ViewGraphT, class FrameMap, class ImageMap>
+int KeepLargestConnectedComponentsDevice(ViewGraphT& view_graph, FrameMap& frames, ImageMap& images) {
+  using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
+  using Frm = typename FrameMap::mapped_type;
+  std::map<frame_t, Frm*> fsorted;
+  for (auto& [id, f] : frames) fsorted[id] = &f;
+  std::map<frame_t, int32_t> fidx;
+  std::vector<Frm*> fr;
+  std::vector<uint8_t> reg;
+  for (auto& [id, f] : fsorted) {
+    fidx[id] = (int32_t)fr.size();
+    fr.push_back(f);
+    reg.push_back(f->is_registered ? 1 : 0);
+  }
+  std::map<image_t, int32_t> iidx;
+  std::vector<image_t> ids;
+  for (auto& [id, im] : images) ids.push_back(id);
+  std::sort(ids.begin(), ids.end());
+  std::vector<int32_t> image_frame;
+  for (image_t id : ids) {
+    auto f = fidx.find(images.at(id).frame_id);
+    if (f == fidx.end()) { std::fprintf(stderr, "b200sfm: image of an unknown frame\n"); return 0; }
+    iidx[id] = (int32_t)image_frame.size();
+    image_frame.push_back(f->second);
+  }
+  std::map<image_pair_t, Pair*> psorted;
+  for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
+  std::vector<Pair*> pairs;
+  std::vector<int32_t> img1, img2;
+  std::vector<uint8_t> valid;
+  for (auto& [id, pr] : psorted) {
+    auto a = iidx.find(pr->image_id1), b = iidx.find(pr->image_id2);
+    if (a == iidx.end() || b == iidx.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return 0; }
+    pairs.push_back(pr);
+    img1.push_back(a->second);
+    img2.push_back(b->second);
+    valid.push_back(pr->is_valid ? 1 : 0);
+  }
+  if (pairs.empty()) return 0;
+  b200sfm_ctx* ctx = DefaultContext();
+  if (!ctx) return 0;
+  int32_t n = 0;
+  const int rc = b200sfm_view_graph_keep_largest_component(ctx, (int32_t)fr.size(), (int32_t)image_frame.size(), image_frame.data(),
+                                                           (int64_t)pairs.size(), img1.data(), img2.data(), valid.data(), reg.data(), &n);
+  if (rc != B200SFM_OK) {
+    std::fprintf(stderr, "b200sfm: KeepLargestConnectedComponents failed: %s\n", b200sfm_last_error(ctx));
+    return 0;
+  }
+  if (n == 0) return 0;
+  for (size_t f = 0; f < fr.size(); ++f) fr[f]->is_registered = reg[f] != 0;
+  for (size_t e = 0; e < pairs.size(); ++e) pairs[e]->is_valid = valid[e] != 0;
+  return n;
+}
 
 
 // ---------------------------------------------------------------------------

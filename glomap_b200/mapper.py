@@ -6,6 +6,13 @@ rotations too; normalise; reprojection filters with the tightening threshold ``m
 ``skip_pruning = False``, stage 8: ``PruneWeaklyConnectedImages`` over the final tracks (``frame_cluster_id`` /
 ``frame_registered`` of the mapper; ``colmap_io.write_clustered_model`` writes one model per cluster).
 
+After each rotation averaging run, ``RelPoseFilter::FilterRotations`` and ``ViewGraph::KeepLargestConnectedComponents``
+(view_graph.py; on the GPU from ``VIEW_GRAPH_DEVICE_MIN_PAIRS`` pairs up) invalidate pairs and may leave images outside
+the largest component.  Those images are unregistered (``image_registered`` of the mapper): the second run and the stages
+after it see only the registered images (track establishment is given their ids; global positioning and bundle
+adjustment run on the scene compacted to their cameras, and the results are scattered back), and an unregistered camera
+keeps its input pose, as in the reference, where its frame is simply not optimised.
+
 It mirrors the reference's control flow so that the GPU solvers are exercised in the order, and with the option
 mutations, the real mapper uses; it is host glue (as in the reference) and owns no numerics: every solve and every
 filter goes through ``libb200sfm.so``.  Trivial frames only.  Stage 4, track establishment (``TrackEngine``:
@@ -19,7 +26,7 @@ import dataclasses
 import numpy as np
 
 from . import estimators as E, geometry as geo, processors as PR, reconstruction_pruning as RP, synthetic as S
-from . import track_establishment as TE
+from . import track_establishment as TE, view_graph as VG
 
 
 @dataclasses.dataclass
@@ -90,6 +97,50 @@ def _sub_view_graph(vg: S.ViewGraph, edge_mask) -> S.ViewGraph:
                        vg.R_gt)
 
 
+# Below this many pairs the two view-graph passes of stage 3 run as the host restatements (view_graph.py), which give
+# the same masks: a device call costs a few allocations, copies and synchronisations, more than the host loops over a
+# handful of pairs (profiles/view_graph_filter_bench.py).
+VIEW_GRAPH_DEVICE_MIN_PAIRS = 100
+
+
+def registered_view_graph(vg: S.ViewGraph, pair_valid, image_registered):
+    """The valid pairs between registered images, the images renumbered in ascending order: (view graph, image ids)."""
+    idx = np.flatnonzero(image_registered)
+    if len(idx) == vg.n_images:
+        return _sub_view_graph(vg, np.asarray(pair_valid, bool)), idx
+    remap = np.full(vg.n_images, -1, np.int64)
+    remap[idx] = np.arange(len(idx))
+    ei, ej = np.asarray(vg.ei), np.asarray(vg.ej)
+    k = np.asarray(pair_valid, bool) & image_registered[ei] & image_registered[ej]
+    R_gt = None if vg.R_gt is None else np.asarray(vg.R_gt)[idx]
+    return S.ViewGraph(len(idx), remap[ei[k]].astype(np.int32), remap[ej[k]].astype(np.int32), np.asarray(vg.R_rel)[k],
+                       np.asarray(vg.weight)[k], R_gt), idx
+
+
+def compact_cameras(scene: S.Scene, idx: np.ndarray) -> S.Scene:
+    """The scene over the cameras ``idx`` (ascending), renumbered in that order; the observations of the other cameras
+    are dropped, every point is kept."""
+    keep = np.zeros(scene.C, bool)
+    keep[idx] = True
+    out = compact_observations(scene, keep[scene.obs_cam])
+    remap = np.full(scene.C, -1, np.int64)
+    remap[idx] = np.arange(len(idx))
+    out.obs_cam = remap[out.obs_cam].astype(np.int32)
+    out.quat, out.trans, out.cam_intr = scene.quat[idx].copy(), scene.trans[idx].copy(), scene.cam_intr[idx].copy()
+    return out
+
+
+def scatter_cameras(full: S.Scene, part: S.Scene, idx: np.ndarray) -> S.Scene:
+    """Inverse of ``compact_cameras``: ``full`` with the poses of the cameras ``idx``, the points, tracks and intrinsics of
+    ``part``; the other cameras keep their poses."""
+    out = full.copy()
+    out.quat[idx], out.trans[idx] = part.quat, part.trans
+    out.points, out.pt_obs_begin = part.points.copy(), part.pt_obs_begin.copy()
+    out.obs_cam, out.obs_xy = np.asarray(idx)[part.obs_cam].astype(np.int32), part.obs_xy.copy()
+    out.intr_model, out.intr_params = part.intr_model.copy(), part.intr_params.copy()
+    return out
+
+
 class GlobalMapper:
     def __init__(self, options: GlobalMapperOptions | None = None, ctx: E.Context | None = None):
         self.options_ = options or GlobalMapperOptions()
@@ -97,6 +148,7 @@ class GlobalMapper:
         self.log: list[str] = []
         self.frame_cluster_id: np.ndarray | None = None   # stage 8: cluster of every frame (-1: none)
         self.frame_registered: np.ndarray | None = None   # stage 8: frames of the largest visibility component
+        self.image_registered: np.ndarray | None = None   # stage 3: images of the view graph's largest component
 
     # -- helpers ------------------------------------------------------------------------------------
     def _filters(self, scene: S.Scene, what) -> S.Scene:
@@ -122,6 +174,22 @@ class GlobalMapper:
             self.last_filtered = n
         return scene
 
+    def _filter_rotations(self, vg: S.ViewGraph, q_rel, R, valid, registered, max_angle):
+        """RelPoseFilter::FilterRotations: (valid, pairs invalidated)."""
+        q_img = geo.rotmat_to_quat_xyzw_fast(R)
+        if vg.E >= VIEW_GRAPH_DEVICE_MIN_PAIRS:
+            return VG.filter_rotations_device(q_img, vg.ei, vg.ej, q_rel, max_angle, valid, registered,
+                                              self.ctx or E.default_context())
+        return VG.filter_rotations(q_img, vg.ei, vg.ej, q_rel, max_angle, valid, registered)
+
+    def _largest_component(self, vg: S.ViewGraph, valid, registered):
+        """ViewGraph::KeepLargestConnectedComponents, frames = images: (valid, registered, registered images)."""
+        frame = np.arange(vg.n_images, dtype=np.int32)
+        if vg.E >= VIEW_GRAPH_DEVICE_MIN_PAIRS:
+            return VG.keep_largest_connected_components_device(vg.n_images, frame, vg.ei, vg.ej, valid, registered,
+                                                               self.ctx or E.default_context())
+        return VG.keep_largest_connected_components(vg.n_images, frame, vg.ei, vg.ej, valid, registered)
+
     # -- controllers/global_mapper.cc:19-355 (stages 3, 5, 6) -----------------------------------------
     def Solve(self, view_graph: S.ViewGraph, scene: S.Scene, image_pairs=None, features: dict | None = None):
         """Returns (ok, scene): poses / points / intrinsics of ``scene`` estimated from the relative rotations of
@@ -132,33 +200,71 @@ class GlobalMapper:
         o, thr = self.options_, self.options_.inlier_thresholds
         scene = scene.copy()
         track_stage = image_pairs is not None and features is not None and not o.skip_track_establishment
-        # 3. rotation averaging: first run for filtering, second for the estimate (:84-116)
+        # 3. rotation averaging: first run for filtering, second for the estimate, each followed by FilterRotations and
+        # KeepLargestConnectedComponents (:84-116)
+        self.image_registered = reg = np.ones(scene.C, bool)
         if not o.skip_rotation_averaging:
             vg = view_graph
+            q_rel = geo.rotmat_to_quat_xyzw_fast(vg.R_rel)
+            valid, reg = np.ones(vg.E, bool), np.ones(vg.n_images, bool)
+            R_all = None
             for run in range(2):
+                # SolveRotationAveraging solves on the largest component (rotation_averager.cc:13)
+                valid, reg, num_img = self._largest_component(vg, valid, reg)
+                self.image_registered = reg
+                if num_img == 0:
+                    self.log.append(f"rotation averaging run {run + 1}: no pair is left")
+                    return False, scene
+                sub, idx = registered_view_graph(vg, valid, reg)
                 ra = E.RotationEstimator(o.opt_ra, self.ctx)
-                ok, R = ra.EstimateRotations(vg)
+                ok, R = ra.EstimateRotations(sub)
                 if not ok:
                     if run == 1:
                         return False, scene
                     continue
-                valid = filter_rotations(vg, R, thr.max_rotation_error)
-                vg = _sub_view_graph(vg, valid)
-                if not largest_connected_component(vg.n_images, vg.ei, vg.ej).all():
-                    raise NotImplementedError("images outside the largest connected component must be removed by the caller")
-                self.log.append(f"rotation averaging run {run + 1}: {int((~valid).sum())} edges filtered")
-            scene.quat = geo.rotmat_to_quat_xyzw_fast(R)
-        # 4. track establishment (:119-137): every image is left after stage 3 (it raises otherwise), so all are registered
+                R_all = np.tile(np.eye(3), (vg.n_images, 1, 1))
+                R_all[idx] = R
+                valid, cut = self._filter_rotations(vg, q_rel, R_all, valid, reg, thr.max_rotation_error)
+                valid, reg, num_img = self._largest_component(vg, valid, reg)
+                self.image_registered = reg
+                if num_img == 0:
+                    self.log.append(f"rotation averaging run {run + 1}: no connected component is left")
+                    return False, scene
+                self.log.append(f"rotation averaging run {run + 1}: {cut} edges filtered, {num_img} / {vg.n_images} images "
+                                "in the largest component")
+            scene.quat = np.where(reg[:, None], geo.rotmat_to_quat_xyzw_fast(R_all), scene.quat)
+        # cameras of the registered images: the problem of stages 4-6 (all of them unless stage 3 cut some off)
+        cams = np.flatnonzero(reg)
+        full = scene
+        if len(cams) < scene.C:
+            scene = compact_cameras(scene, cams)
+        # 4. track establishment (:119-137) over the registered images
         if track_stage:
             image_ids = sorted(int(i) for i in features)
-            if len(image_ids) != scene.C:
-                raise ValueError(f"features name {len(image_ids)} images, the scene has {scene.C} cameras")
-            full, discarded = TE.establish_full_tracks_device(image_pairs, features, o.opt_track, self.ctx)
-            sel = TE.find_tracks_for_problem_device(full, image_ids, o.opt_track, self.ctx)
-            flat = TE.tracks_to_scene(sel, features, image_ids, scene.cam_intr, scene.intr_model, scene.intr_params)
+            if len(image_ids) != full.C:
+                raise ValueError(f"features name {len(image_ids)} images, the scene has {full.C} cameras")
+            reg_ids = [image_ids[k] for k in cams]
+            full_tracks, discarded = TE.establish_full_tracks_device(image_pairs, features, o.opt_track, self.ctx)
+            sel = TE.find_tracks_for_problem_device(full_tracks, reg_ids, o.opt_track, self.ctx)
+            flat = TE.tracks_to_scene(sel, features, reg_ids, scene.cam_intr, scene.intr_model, scene.intr_params)
             flat.quat, flat.trans = scene.quat, scene.trans
             scene = flat
-            self.log.append(f"track establishment: {len(full)} tracks ({discarded} discarded), {len(sel)} selected")
+            self.log.append(f"track establishment: {len(full_tracks)} tracks ({discarded} discarded), {len(sel)} selected")
+        ok, scene = self._solve_positions(scene)
+        if len(cams) < full.C:
+            scene = scatter_cameras(full, scene, cams)
+        if not ok:
+            return False, scene
+        # 8. reconstruction pruning (:340-353): trivial frames, so the tracks' frames are their images
+        if not o.skip_pruning:
+            out = RP.prune_weakly_connected_images(scene.pt_obs_begin, scene.obs_cam, scene.C, ctx=self.ctx)
+            self.frame_cluster_id, self.frame_registered = out["cluster_id"], out["is_registered"]
+            self.log.append(f"pruning: {out['num_clusters']} clusters, threshold {out['stats']['strong_threshold']:g}")
+        return True, scene
+
+    def _solve_positions(self, scene: S.Scene):
+        """Stages 5 and 6 on the registered cameras: (ok, scene)."""
+        o, thr = self.options_, self.options_.inlier_thresholds
         # 5. global positioning (:143-189)
         if not o.skip_global_positioning:
             bear = PR.undistort_images(scene)
@@ -199,9 +305,4 @@ class GlobalMapper:
                 ite += 1
             scene = self._filters(scene, [("reprojection", thr.max_reprojection_error),
                                           ("triangulation", thr.min_triangulation_angle)])
-        # 8. reconstruction pruning (:340-353): trivial frames, so the tracks' frames are their images
-        if not o.skip_pruning:
-            out = RP.prune_weakly_connected_images(scene.pt_obs_begin, scene.obs_cam, scene.C, ctx=self.ctx)
-            self.frame_cluster_id, self.frame_registered = out["cluster_id"], out["is_registered"]
-            self.log.append(f"pruning: {out['num_clusters']} clusters, threshold {out['stats']['strong_threshold']:g}")
         return True, scene

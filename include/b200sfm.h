@@ -317,6 +317,37 @@ int b200sfm_image_pairs_inlier_count(b200sfm_ctx* ctx, int32_t num_images, const
                                      double max_epipolar_error_E, double max_epipolar_error_F, double max_epipolar_error_H,
                                      uint8_t* is_inlier, int32_t* num_inliers, double* score);
 
+/* ---- view-graph passes of stage 3 ---------------------------------------------------------------------------------------
+ * GlobalMapper::Solve runs both after each rotation averaging (controllers/global_mapper.cc:91-115), and
+ * SolveRotationAveraging takes the largest component before and between its solves (controllers/rotation_averager.cc).
+ *
+ * b200sfm_view_graph_filter_rotations: RelPoseFilter::FilterRotations (glomap/processors/relpose_filter.cc:7-33).  A pair
+ * with pair_valid[e] != 0 whose two images are registered (image_registered NULL: all are) is invalidated when the angle
+ * between q2 * q1^-1 (cam_from_world_quat_xyzw [I][4] of its images) and its cam2_from_cam1 rotation pair_quat_xyzw [E][4]
+ * is larger than max_angle_deg.  The angle is Eigen's angularDistance (math/rigid3d.cc:7-9, the Rigid3d overload of
+ * CalcAngle): d = q_calc * conj(q_rel), 2 atan2(|d.vec|, |d.w|), in degrees.  An angle equal to max_angle_deg keeps the
+ * pair, and so does a NaN angle.  num_invalidated counts the pairs this call invalidated.
+ *
+ * b200sfm_view_graph_keep_largest_component: ViewGraph::KeepLargestConnectedComponents (glomap/scene/view_graph.cc:56-97)
+ * in frame space.  image_frame [I] names each image's frame in [0, F).  The nodes are the frames of the valid pairs
+ * (CreateFrameAdjacencyList, :140-150; a valid pair inside one frame makes that frame a node).  Of the connected
+ * components the largest is kept; between equally large ones, the one holding the smallest frame index (the reference's
+ * choice depends on hash-map order).  Then frame_registered [F] is 1 exactly for the frames of that component, every pair
+ * with an image outside it gets pair_valid 0, and num_registered_images is the number of images whose frame is registered.
+ * Without a valid pair nothing is written and num_registered_images is 0 (:71).
+ *
+ * Both: host buffers.  A pair image index outside [0, num_images), or an image_frame outside [0, num_frames), gives
+ * B200SFM_ERR_INVALID_ARG; it is checked on the device, never dereferenced, and the outputs are then untouched.
+ * num_pairs == 0 returns B200SFM_OK with a zero count.  No collectives: on a distributed context each rank works on the
+ * graph it is given. */
+int b200sfm_view_graph_filter_rotations(b200sfm_ctx* ctx, int32_t num_images, const double* cam_from_world_quat_xyzw,
+                                        const uint8_t* image_registered, int64_t num_pairs, const int32_t* pair_image1,
+                                        const int32_t* pair_image2, const double* pair_quat_xyzw, double max_angle_deg,
+                                        uint8_t* pair_valid, int64_t* num_invalidated);
+int b200sfm_view_graph_keep_largest_component(b200sfm_ctx* ctx, int32_t num_frames, int32_t num_images, const int32_t* image_frame,
+                                              int64_t num_pairs, const int32_t* pair_image1, const int32_t* pair_image2,
+                                              uint8_t* pair_valid, uint8_t* frame_registered, int32_t* num_registered_images);
+
 /* ---- (ii) global positioning (BATA) ----------------------------------------- */
 /* Mirror of GlobalPositionerOptions (global_positioning.h:9-54) + inherited
  * solver options (optimization_base.h:18-23) + PCG knobs.  Only the
