@@ -219,10 +219,31 @@ class BAStepProbeOut(ct.Structure):
                                       "schur_jacobi", "nbk")]
 
 
+class RAProbeInfo(ct.Structure):
+    """b200sfm_test_ra_info (include/b200sfm_testing.h)."""
+    _fields_ = [(f, c_int32) for f in ("n", "n_frames", "n_cams", "has_grav", "use_csr", "use_2lvl", "fused", "nc")] + \
+              [("rows_total", c_int64), ("E_total", c_int64)]
+
+
+class RASystemProbeOut(ct.Structure):
+    """b200sfm_test_ra_system_out (include/b200sfm_testing.h)."""
+    _fields_ = [(f, c_void_p) for f in ("res", "w", "b", "rhs", "deg", "Minv", "Ac")] + [("b_norm2", c_double)]
+
+
 # name -> (restype, argtypes); the test-only probe of include/b200sfm_testing.h (not part of the drop-in ABI)
 TEST_PROTOTYPES = {
     "b200sfm_test_ba_step": (c_int32, [c_void_p, P(BAOpts), c_double, c_double, P(BAStepProbeOut)]),
     "b200sfm_test_ba_apply": (c_int32, [c_void_p, c_void_p, c_void_p]),
+    "b200sfm_test_ra_problem_create": (c_int32, [c_void_p, P(RAOpts), c_int32, c_int32, c_int64] + [c_void_p] * 9
+                                       + [c_int32, c_void_p, P(c_void_p)]),
+    "b200sfm_test_ra_problem_free": (None, [c_void_p]),
+    "b200sfm_test_ra_problem_info": (c_int32, [c_void_p, P(RAProbeInfo), c_void_p]),
+    "b200sfm_test_ra_system": (c_int32, [c_void_p, c_int32, c_double, c_int32, P(RASystemProbeOut)]),
+    "b200sfm_test_ra_apply": (c_int32, [c_void_p, c_void_p, c_void_p]),
+    "b200sfm_test_ra_precond": (c_int32, [c_void_p, c_void_p, c_void_p]),
+    "b200sfm_test_ra_pcg": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, P(c_int32)]),
+    "b200sfm_test_ra_admm_step": (c_int32, [c_void_p, c_double] + [c_void_p] * 6),
+    "b200sfm_test_ra_update": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -1207,6 +1207,141 @@ int b200sfm_ra_solve_rig(b200sfm_ctx* ctx, const b200sfm_ra_opts* opts, int32_t 
   return finish(ctx, rc);
 }
 
+// ---- RA test probe (include/b200sfm_testing.h) -------------------------------------------------------------------
+struct b200sfm_test_ra_problem {
+  b200sfm_ra_problem p;
+  int square = -1;   // the system b200sfm_test_ra_system prepared last (-1: none yet)
+};
+
+int b200sfm_test_ra_problem_create(b200sfm_ctx* ctx, const b200sfm_ra_opts* opts, int32_t n_frames, int32_t n_cams,
+                                   int64_t n_edges, const int32_t* ei, const int32_t* ej, const int32_t* eci,
+                                   const int32_t* ecj, const double* R_rel, const double* edge_w,
+                                   const uint8_t* frame_has_gravity, const int32_t* cam_frames_begin,
+                                   const int32_t* cam_frames, int32_t fixed_frame, const double* theta,
+                                   b200sfm_test_ra_problem** out) {
+  if (!ctx || !opts || !theta || !out) return B200SFM_ERR_INVALID_ARG;
+  *out = nullptr;
+  if (ctx->world > 1) { ctx->err = "the test probe is single-rank only"; return B200SFM_ERR_INVALID_ARG; }
+  if (n_frames <= 0 || n_cams < 0) { ctx->err = "no frames"; return B200SFM_ERR_INVALID_ARG; }
+  if (n_cams > 0 && (!eci || !ecj || !cam_frames_begin || !cam_frames)) { ctx->err = "null camera array"; return B200SFM_ERR_INVALID_ARG; }
+  if (n_edges < 0 || (n_edges > 0 && (!ei || !ej || !R_rel))) { ctx->err = "null edge array"; return B200SFM_ERR_INVALID_ARG; }
+  if (fixed_frame < 0 || fixed_frame >= n_frames) { ctx->err = "fixed_frame out of range"; return B200SFM_ERR_INVALID_ARG; }
+  const int n = n_frames + n_cams;
+  for (int64_t e = 0; e < n_edges; ++e) {
+    if (ei[e] < 0 || ei[e] >= n_frames || ej[e] < 0 || ej[e] >= n_frames) { ctx->err = "edge index out of range"; return B200SFM_ERR_INVALID_ARG; }
+    if (n_cams > 0 && ((eci[e] != -1 && (eci[e] < n_frames || eci[e] >= n)) || (ecj[e] != -1 && (ecj[e] < n_frames || ecj[e] >= n)))) {
+      ctx->err = "camera node out of range (must be -1 or in [n_frames, n_frames + n_cams))";
+      return B200SFM_ERR_INVALID_ARG;
+    }
+  }
+  if (n_cams > 0) {
+    if (cam_frames_begin[0] != 0) { ctx->err = "cam_frames_begin must start at 0"; return B200SFM_ERR_INVALID_ARG; }
+    for (int c = 0; c < n_cams; ++c)
+      if (cam_frames_begin[c + 1] < cam_frames_begin[c]) { ctx->err = "cam_frames_begin must be non-decreasing"; return B200SFM_ERR_INVALID_ARG; }
+    for (int k = 0; k < cam_frames_begin[n_cams]; ++k)
+      if (cam_frames[k] < 0 || cam_frames[k] >= n_frames) { ctx->err = "cam_frames out of range"; return B200SFM_ERR_INVALID_ARG; }
+  }
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    auto* h = new b200sfm_test_ra_problem;
+    try {
+      h->p.create(ctx, n, n_edges, ei, ej, R_rel, edge_w, opts->use_weight, fixed_frame, theta, frame_has_gravity, n_cams,
+                  eci, ecj, cam_frames_begin, cam_frames);
+    } catch (...) {
+      delete h;
+      throw;
+    }
+    *out = h;
+    return (int)B200SFM_OK;
+  });
+}
+
+void b200sfm_test_ra_problem_free(b200sfm_test_ra_problem* h) {
+  if (!h) return;
+  cudaSetDevice(h->p.ctx->device);
+  cudaStreamSynchronize(h->p.ctx->stream);
+  b200::AllocScope alloc_scope(pool_stream(h->p.ctx));   // back to the stream-ordered pool
+  delete h;
+}
+
+int b200sfm_test_ra_problem_info(b200sfm_test_ra_problem* h, b200sfm_test_ra_info* info, int32_t* agg_of) {
+  if (!h || !info) return B200SFM_ERR_INVALID_ARG;
+  return guarded(h->p.ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(h->p.ctx->device));
+    h->p.test_info(info, agg_of);
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_ra_system(b200sfm_test_ra_problem* h, int32_t mode, double sigma2, int32_t square,
+                           b200sfm_test_ra_system_out* out) {
+  if (!h || !out || mode < 0 || mode > 2 || (square != 0 && square != 1) || (mode == 1 && !(sigma2 > 0.0)))
+    return B200SFM_ERR_INVALID_ARG;
+  return guarded(h->p.ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(h->p.ctx->device));
+    h->p.test_system(mode, sigma2, square, out);
+    h->square = square;
+    return (int)B200SFM_OK;
+  });
+}
+
+static int ra_probe_ready(b200sfm_test_ra_problem* h) {
+  if (h->square >= 0) return B200SFM_OK;
+  h->p.ctx->err = "the RA probe needs a preceding b200sfm_test_ra_system";
+  return B200SFM_ERR_INVALID_ARG;
+}
+
+int b200sfm_test_ra_apply(b200sfm_test_ra_problem* h, const double* x, double* y) {
+  if (!h || !x || !y) return B200SFM_ERR_INVALID_ARG;
+  if (ra_probe_ready(h) != B200SFM_OK) return B200SFM_ERR_INVALID_ARG;
+  return guarded(h->p.ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(h->p.ctx->device));
+    h->p.test_apply(h->square, x, y);
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_ra_precond(b200sfm_test_ra_problem* h, const double* r, double* z) {
+  if (!h || !r || !z) return B200SFM_ERR_INVALID_ARG;
+  if (ra_probe_ready(h) != B200SFM_OK) return B200SFM_ERR_INVALID_ARG;
+  return guarded(h->p.ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(h->p.ctx->device));
+    h->p.test_precond(r, z);
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_ra_pcg(b200sfm_test_ra_problem* h, int32_t k, const double* warm_x, double* x_out, int32_t* iterations) {
+  if (!h || !x_out || k < 1) return B200SFM_ERR_INVALID_ARG;
+  if (ra_probe_ready(h) != B200SFM_OK) return B200SFM_ERR_INVALID_ARG;
+  return guarded(h->p.ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(h->p.ctx->device));
+    const int it = h->p.test_pcg(h->square, k, warm_x, x_out);
+    if (iterations) *iterations = it;
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_ra_admm_step(b200sfm_test_ra_problem* h, double rho, const double* x, const double* b, double* z,
+                              double* u, double* rsu, double* norms) {
+  if (!h || !x || !b || !z || !u || !rsu || !norms || !(rho > 0.0)) return B200SFM_ERR_INVALID_ARG;
+  if (ra_probe_ready(h) != B200SFM_OK) return B200SFM_ERR_INVALID_ARG;
+  return guarded(h->p.ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(h->p.ctx->device));
+    h->p.test_admm_step(rho, x, b, z, u, rsu, norms);
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_ra_update(b200sfm_test_ra_problem* h, const double* step, double* theta_out, double* sums) {
+  if (!h || !step || !theta_out || !sums) return B200SFM_ERR_INVALID_ARG;
+  return guarded(h->p.ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(h->p.ctx->device));
+    h->p.test_update(step, theta_out, sums);
+    return (int)B200SFM_OK;
+  });
+}
+
 int b200sfm_ra_mst_init(b200sfm_ctx* ctx, int32_t n_nodes, int64_t n_edges, const int32_t* ei, const int32_t* ej,
                         const double* R_rel, const double* weight, int32_t root, double* R, int32_t* parent,
                         b200sfm_mst_stats* stats) {

@@ -228,6 +228,7 @@ __global__ void ra_scatter(RAView v, const double* __restrict__ w, int square, c
   const EdgeRows er = edge_rows(v, i, j);
   const int nci = (v.eci && i >= 0) ? v.eci[e] : -1, ncj = (v.ecj && i >= 0) ? v.ecj[e] : -1;
   const bool same_frame = i == j;   // only with unknown cameras: the -I and +I on the frame cancel (.cc:300-304 keeps the pair)
+  const bool same_cam = nci == ncj;   // one unknown sensor in both images: its -I and +I cancel too (.cc:425-440 sums them)
 #pragma unroll
   for (int k = 0; k < 3; ++k) {
     if (er.y_only && k != 1) continue;
@@ -241,11 +242,11 @@ __global__ void ra_scatter(RAView v, const double* __restrict__ w, int square, c
       atomicAdd(&out[3 * (size_t)i + k], -a);
       if (deg) atomicAdd(&deg[3 * (size_t)i + k], we);
     }
-    if (ncj >= 0) {
+    if (ncj >= 0 && !same_cam) {
       atomicAdd(&out[3 * (size_t)ncj + k], a);
       if (deg) atomicAdd(&deg[3 * (size_t)ncj + k], we);
     }
-    if (nci >= 0) {
+    if (nci >= 0 && !same_cam) {
       atomicAdd(&out[3 * (size_t)nci + k], -a);
       if (deg) atomicAdd(&deg[3 * (size_t)nci + k], we);
     }
@@ -885,6 +886,8 @@ __global__ void ra_norm2_final(int nblk, const double* __restrict__ part_a, cons
 
 // Warm-started PCG initialisation: x is kept, Ax holds L x (all-reduced):
 //   r = b - Ax; z = Minv r; p = z; Ax <- 0; partial r.z, r.r, b.b
+// Minv is the packed 3x3 diagonal of ra_build_precond: a gravity frame's slots differ (1, 1/d_y, 1), so each slot
+// takes its own entry, as pcg_init / pcg_update apply it
 __global__ void __launch_bounds__(128) ra_pcg_init_warm(int nb, const double* __restrict__ Minv,
                                                         const double* __restrict__ b, double* __restrict__ Ax,
                                                         double* __restrict__ r, double* __restrict__ z,
@@ -894,14 +897,14 @@ __global__ void __launch_bounds__(128) ra_pcg_init_warm(int nb, const double* __
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   double rz = 0, rr = 0, bb = 0;
   if (c < nb) {
-    const double minv = Minv[6 * (size_t)c];   // diagonal preconditioner
+    const double minv[3] = {Minv[6 * (size_t)c], Minv[6 * (size_t)c + 3], Minv[6 * (size_t)c + 5]};
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       const size_t i = 3 * (size_t)c + k;
       const double bv = b[i];
       const double rv = bv - Ax[i];
       Ax[i] = 0.0;
-      const double zv = minv * rv;
+      const double zv = minv[k] * rv;
       r[i] = rv;
       z[i] = zv;
       p[i] = zv;

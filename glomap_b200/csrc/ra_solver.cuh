@@ -5,6 +5,7 @@
 #pragma once
 #include <cub/cub.cuh>
 
+#include "../../include/b200sfm_testing.h"
 #include "context.cuh"
 #include "pcg.cuh"
 #include "ra_kernels.cuh"
@@ -260,6 +261,19 @@ struct b200sfm_ra_problem {
     }
   }
 
+  // fused iteration (ra_kernels.cuh: ra2_*): four kernels, the prolongation folded into the direction update.  Opt-in
+  // (B200SFM_RA_FUSED=1): at config 5 on one H100 (700 W) it is within 2 % of the seven-kernel iteration (614 vs 624 ms
+  // per solve) with 24 k instead of 37 k launches -- the launch count is not what bounds the iteration.  It reorders the
+  // PCG arithmetic (the iteration count differs by one or two), so the default keeps the seven-kernel results.
+  bool fused_iteration() const {
+    return use_2lvl && use_csr && ctx->world == 1 && (getenv("B200SFM_RA_FUSED") && atoi(getenv("B200SFM_RA_FUSED")) == 1);
+  }
+
+  void fused_buffers() {
+    if (p4.n < (size_t)n * 4) p4.alloc((size_t)n * 4);
+    if (gbar.n < 2) { gbar.alloc(2); gbar.zero(ctx->stream); }
+  }
+
   // x = L(w^p)^-1 rhs_vec by PCG (result in px); returns iterations.  Loop control on the device (pcg.cuh).
   int pcg_solve(const b200sfm_ra_opts& o, int square, const double* rhs_vec, bool& finite, bool warm = false) {
     using namespace b200;
@@ -277,14 +291,8 @@ struct b200sfm_ra_problem {
     double *part_pq = ctx->pcgh.d_part, *part_rz = ctx->pcgh.d_part + nblk_t, *part_rr = ctx->pcgh.d_part + 2 * (size_t)nblk_t;
     if (use_2lvl) B200_CUDA_OK(cudaMemsetAsync(ctx->pcgh.d_part, 0, (size_t)nblk_t * 3 * sizeof(double), s));
     PcgCtl* ctl = ctx->pcgh.d_ctl;
-    // fused iteration (ra_kernels.cuh: ra2_*): four kernels, the prolongation folded into the direction update.  Opt-in
-    // (B200SFM_RA_FUSED=1): at config 5 on one H100 (700 W) it is within 2 % of the seven-kernel iteration (614 vs 624 ms
-    // per solve) with 24 k instead of 37 k launches -- the launch count is not what bounds the iteration.  It reorders the
-    // PCG arithmetic (the iteration count differs by one or two), so the default keeps the seven-kernel results.
-    const bool fused = use_2lvl && use_csr && ctx->world == 1 && (getenv("B200SFM_RA_FUSED") && atoi(getenv("B200SFM_RA_FUSED")) == 1);
-    if (fused) {
-      if (p4.n < (size_t)n * 4) p4.alloc((size_t)n * 4);
-      if (gbar.n < 2) { gbar.alloc(2); gbar.zero(s); }
+    if (fused_iteration()) {
+      fused_buffers();
       PcgResult rf = ctx->pcgh.run(
           s, max_it,
           [&]() {
@@ -376,6 +384,43 @@ struct b200sfm_ra_problem {
     B200_LAUNCH(ctx, ra_coarse_prolong, cdiv(n, 256), 256, 0, n, coarse(), z, ctl);
   }
 
+  // residuals at theta and the weights of the next system (ra_residuals: mode 0 L1 rows, 1 Geman-McClure, 2 half-norm)
+  void residuals(int mode, double sigma2) {
+    using namespace b200;
+    if (E > 0) B200_LAUNCH(ctx, ra_residuals, cdiv(E, 256), 256, 0, view(), theta.p, mode, sigma2, res.p, w.p, flags.p);
+  }
+
+  // the L1 stage's linear system (.cc:479-541): b = W r, |b|^2 in scal[0], z = u = 0; ADMM on |A_w x - b|_1 with
+  // A_w^T A_w = L(w^2): rhs = A^T W^2 r = A_w^T b, deg = sum w^2
+  void l1_system() {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    B200_CUDA_OK(cudaMemsetAsync(scal.p, 0, 8 * sizeof(double), s));
+    if (E > 0) B200_LAUNCH(ctx, ra_weighted_rhs, cdiv(E, 256), 256, 0, view(), w.p, res.p, b.p, scal.p);
+    ctx->allreduce_sum(scal.p, 1);   // |b|^2 over all ranks
+    z.zero(s);
+    u.zero(s);
+    prepare_system(1, res.p);
+  }
+
+  // one ADMM iteration after the x-update in px: z, u; rhs | svec | uvec (ra_admm_step); scal[1..3] = |A_w x - z - b|^2,
+  // |A_w x|^2, |z|^2; scal[4..5] = |svec|^2, |uvec|^2
+  void admm_step(double rho) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    B200_CUDA_OK(cudaMemsetAsync(rhs.p, 0, (size_t)n * 9 * sizeof(double), s));
+    B200_CUDA_OK(cudaMemsetAsync(scal.p + 1, 0, 3 * sizeof(double), s));
+    if (E > 0)
+      B200_LAUNCH(ctx, ra_admm_step, cdiv(E, 256), 256, 0, view(), w.p, px.p, b.p, z.p, u.p, rho, rhs.p, rhs.p + (size_t)n * 3,
+                  rhs.p + (size_t)n * 6, scal.p);
+    ctx->allreduce_sum(rhs.p, (size_t)n * 9);
+    ctx->allreduce_sum(scal.p + 1, 3);
+    const int nb2 = cdiv((long long)n * 3, 256);
+    if (part.n < (size_t)nb2 * 2) part.alloc((size_t)nb2 * 2 + 3 * (size_t)cdiv(n, kPcgThreads));
+    B200_LAUNCH(ctx, ra_norm2_partial, nb2, 256, 0, n * 3, rhs.p + (size_t)n * 3, rhs.p + (size_t)n * 6, part.p, part.p + nb2);
+    B200_LAUNCH(ctx, ra_norm2_final, 1, 256, 0, nb2, part.p, part.p + nb2, scal.p + 4);
+  }
+
   // theta <- theta (+) step(px); returns (avg step, |step|, nan?)
   void apply_step(double& avg, double& norm, bool& bad) {
     using namespace b200;
@@ -391,6 +436,134 @@ struct b200sfm_ra_problem {
     bad = ctx->h_scal[10] > 0 || !std::isfinite(ctx->h_scal[9]);
   }
 
+  // ---- test probe (include/b200sfm_testing.h) ----------------------------------------------------------------------
+  void test_info(b200sfm_test_ra_info* info, int32_t* h_agg_of) {
+    info->n = n; info->n_frames = n_frames; info->n_cams = n_cams; info->has_grav = has_grav;
+    info->use_csr = use_csr; info->use_2lvl = use_2lvl; info->fused = fused_iteration(); info->nc = use_2lvl ? nc : 0;
+    info->rows_total = rows_total; info->E_total = E_total;
+    if (h_agg_of && use_2lvl) {
+      agg_of.download(h_agg_of, n, ctx->stream);
+      B200_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+    }
+  }
+
+  // the system of an L1 outer iteration (square = 1) or of an IRLS iteration (square = 0) at the current theta
+  void test_system(int mode, double sigma2, int square, b200sfm_test_ra_system_out* out) {
+    cudaStream_t s = ctx->stream;
+    residuals(mode, sigma2);
+    if (square) l1_system();
+    else prepare_system(0, res.p);
+    if (out->res) res.download(out->res, (size_t)E * 3, s);
+    if (out->w) w.download(out->w, E, s);
+    if (out->b && square) b.download(out->b, (size_t)E * 3, s);
+    if (out->rhs) rhs.download(out->rhs, (size_t)n * 3, s);
+    if (out->deg) deg.download(out->deg, (size_t)n * 3, s);
+    if (out->Minv) Minv.download(out->Minv, (size_t)n * 6, s);
+    if (out->Ac && use_2lvl) Ac.download(out->Ac, (size_t)nc * nc, s);
+    double bn = 0;
+    if (square) B200_CUDA_OK(cudaMemcpyAsync(&bn, scal.p, sizeof(double), cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    out->b_norm2 = bn;
+  }
+
+  // the PCG partials and control record as pcg_solve lays them out, reset
+  double* test_pcg_parts(int& nblk, int& nblk_t) {
+    nblk = b200::cdiv(n, b200::kPcgThreads);
+    nblk_t = nblk + (use_2lvl ? nblk_c : 0);
+    ctx->pcgh.ensure(1, (size_t)nblk_t * 3, ctx->world);
+    B200_CUDA_OK(cudaMemsetAsync(ctx->pcgh.d_part, 0, (size_t)nblk_t * 3 * sizeof(double), ctx->stream));
+    B200_CUDA_OK(cudaMemsetAsync(ctx->pcgh.d_ctl, 0, sizeof(b200::PcgCtl), ctx->stream));
+    return ctx->pcgh.d_part;
+  }
+
+  // y = L x: the mat-vec of a PCG iteration (fused: ra2_laplacian_dot on the padded copy ra2_direction writes)
+  void test_apply(int square, const double* h_x, double* h_y) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    int nblk, nblk_t;
+    double* part_pq = test_pcg_parts(nblk, nblk_t);
+    PcgCtl* ctl = ctx->pcgh.d_ctl;
+    if (fused_iteration()) {
+      fused_buffers();
+      std::vector<double> x4((size_t)n * 4, 0.0);
+      for (int i = 0; i < n; ++i) std::copy(h_x + 3 * (size_t)i, h_x + 3 * (size_t)i + 3, &x4[4 * (size_t)i]);
+      p4.upload(x4.data(), (size_t)n * 4, s);
+      B200_LAUNCH(ctx, ra2_laplacian_dot, nblk, kLapThreads, 0, csr(), p4.p, pq.p, part_pq, ctl);
+      pq.download(h_y, (size_t)n * 3, s);
+      B200_CUDA_OK(cudaStreamSynchronize(s));
+      return;
+    }
+    pp.upload(h_x, (size_t)n * 3, s);
+    yw.zero(s);
+    laplacian(view(), square, pp.p, yw.p, ctl);
+    ctx->allreduce_sum(yw.p, (size_t)n * 3);
+    B200_LAUNCH(ctx, pcg_apply_diag<3>, nblk, kPcgThreads, 0, n, Azero.p, Dzero.p, pp.p, yw.p, pq.p, part_pq, ctl);
+    pq.download(h_y, (size_t)n * 3, s);
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+  }
+
+  // z = M^-1 r as the first iteration of a cold solve applies it: pcg_init's Jacobi blocks, then the coarse correction
+  // (fused: ra2_coarse, and the fold of P zc into the first direction by ra2_direction)
+  void test_precond(const double* h_r, double* h_z) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    int nblk, nblk_t;
+    double* part = test_pcg_parts(nblk, nblk_t);
+    double *part_rz = part + nblk_t, *part_rr = part + 2 * (size_t)nblk_t;
+    yw.upload(h_r, (size_t)n * 3, s);
+    B200_LAUNCH(ctx, pcg_init<3>, nblk, kPcgThreads, 0, n, Minv.p, yw.p, px.p, pr.p, pz.p, part_rz, part_rr);
+    if (fused_iteration()) {
+      fused_buffers();
+      B200_LAUNCH(ctx, ra2_coarse, nblk_c, 128, 0, coarse(), pr.p, part_rz + nblk, gbar.p, nullptr);
+      B200_LAUNCH(ctx, ra2_direction, nblk, kPcgThreads, 0, n, nblk_t, 1, 0.0, pz.p, pp.p, p4.p, zc.p, agg_of.p,
+                  ctx->pcgh.dots(-1), part_rz, part_rr, nullptr, ctx->pcgh.dots(0), ctx->pcgh.d_ctl);
+      pp.download(h_z, (size_t)n * 3, s);
+    } else {
+      if (use_2lvl) coarse_correct(pr.p, pz.p, part_rz + nblk, nullptr);
+      pz.download(h_z, (size_t)n * 3, s);
+    }
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+  }
+
+  // exactly k iterations of pcg_solve on rhs (tolerance 0), cold or warm-started from h_warm
+  int test_pcg(int square, int k, const double* h_warm, double* h_x) {
+    cudaStream_t s = ctx->stream;
+    b200sfm_ra_opts o{};
+    o.pcg_max_iterations = k;
+    o.pcg_rel_tolerance = 0.0;
+    if (h_warm) px.upload(h_warm, (size_t)n * 3, s);
+    bool finite = true;
+    const int it = pcg_solve(o, square, rhs.p, finite, h_warm != nullptr);
+    px.download(h_x, (size_t)n * 3, s);
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    return it;
+  }
+
+  void test_admm_step(double rho, const double* h_x, const double* h_b, double* h_z, double* h_u, double* h_rsu,
+                      double* h_norms) {
+    cudaStream_t s = ctx->stream;
+    px.upload(h_x, (size_t)n * 3, s);
+    b.upload(h_b, (size_t)E * 3, s);
+    z.upload(h_z, (size_t)E * 3, s);
+    u.upload(h_u, (size_t)E * 3, s);
+    admm_step(rho);
+    z.download(h_z, (size_t)E * 3, s);
+    u.download(h_u, (size_t)E * 3, s);
+    rhs.download(h_rsu, (size_t)n * 9, s);
+    B200_CUDA_OK(cudaMemcpyAsync(h_norms, scal.p + 1, 5 * sizeof(double), cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+  }
+
+  void test_update(const double* h_step, double* h_theta, double* sums) {
+    px.upload(h_step, (size_t)n * 3, ctx->stream);
+    double avg, norm;
+    bool bad;
+    apply_step(avg, norm, bad);
+    theta.download(h_theta, (size_t)n * 3, ctx->stream);
+    B200_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+    sums[0] = avg; sums[1] = norm; sums[2] = bad ? 1.0 : 0.0;
+  }
+
   int solve(const b200sfm_ra_opts& o, b200sfm_ra_stats* st) {
     using namespace b200;
     cudaStream_t s = ctx->stream;
@@ -399,8 +572,6 @@ struct b200sfm_ra_problem {
     B200_CUDA_OK(cudaEventCreate(&ev0));
     B200_CUDA_OK(cudaEventCreate(&ev1));
     B200_CUDA_OK(cudaEventRecord(ev0, s));
-    RAView v = view();
-    const int egrid = cdiv(std::max<long long>(E, 1), 256);
     b200sfm_ra_stats local{};
     local.usable = 1;
     local.num_edges = E_real;
@@ -408,17 +579,11 @@ struct b200sfm_ra_problem {
     bool failed = false;
     // ---- L1 (.cc:479-541) ----------------------------------------------------------
     if (o.max_num_l1_iterations > 0) {
-      if (E > 0) B200_LAUNCH(ctx, ra_residuals, egrid, 256, 0, v, theta.p, 0, 0.0, res.p, w.p, flags.p);
+      residuals(0, 0.0);
       double last_norm = 0, curr_norm = 0;
       for (int it = 0; it < o.max_num_l1_iterations && !failed; ++it) {
         last_norm = curr_norm;
-        // b = W r ; ADMM on |A_w x - b|_1, A_w^T A_w = L(w^2)
-        B200_CUDA_OK(cudaMemsetAsync(scal.p, 0, 8 * sizeof(double), s));
-        if (E > 0) B200_LAUNCH(ctx, ra_weighted_rhs, egrid, 256, 0, v, w.p, res.p, b.p, scal.p);
-        ctx->allreduce_sum(scal.p, 1);   // |b|^2 over all ranks
-        z.zero(s);
-        u.zero(s);
-        prepare_system(1, res.p);   // rhs = A^T W^2 r = A_w^T b ; deg = sum w^2
+        l1_system();
         double b_norm2 = 0;
         const double eps_pri_thr = std::sqrt((double)rows_total) * o.l1_absolute_tolerance;   // sqrt(A.rows())
         const double eps_dual_thr = std::sqrt(3.0 * n) * o.l1_absolute_tolerance;
@@ -427,19 +592,7 @@ struct b200sfm_ra_problem {
           local.pcg_iterations += pcg_solve(o, 1, rhs.p, finite, /*warm=*/k > 0);
           ++local.admm_iterations;
           if (!finite) { failed = true; break; }
-          B200_CUDA_OK(cudaMemsetAsync(rhs.p, 0, (size_t)n * 9 * sizeof(double), s));
-          B200_CUDA_OK(cudaMemsetAsync(scal.p + 1, 0, 3 * sizeof(double), s));
-          if (E > 0)
-            B200_LAUNCH(ctx, ra_admm_step, egrid, 256, 0, v, w.p, px.p, b.p, z.p, u.p, o.l1_rho, rhs.p, rhs.p + (size_t)n * 3,
-                        rhs.p + (size_t)n * 6, scal.p);
-          ctx->allreduce_sum(rhs.p, (size_t)n * 9);
-          ctx->allreduce_sum(scal.p + 1, 3);
-          {
-            const int nb2 = cdiv((long long)n * 3, 256);
-            if (part.n < (size_t)nb2 * 2) part.alloc((size_t)nb2 * 2 + 3 * (size_t)cdiv(n, kPcgThreads));
-            B200_LAUNCH(ctx, ra_norm2_partial, nb2, 256, 0, n * 3, rhs.p + (size_t)n * 3, rhs.p + (size_t)n * 6, part.p, part.p + nb2);
-            B200_LAUNCH(ctx, ra_norm2_final, 1, 256, 0, nb2, part.p, part.p + nb2, scal.p + 4);
-          }
+          admm_step(o.l1_rho);
           B200_CUDA_OK(cudaMemcpyAsync(ctx->h_scal, scal.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, s));
           B200_CUDA_OK(cudaStreamSynchronize(s));
           const double* h = ctx->h_scal;
@@ -455,7 +608,7 @@ struct b200sfm_ra_problem {
         apply_step(avg, norm, bad);                                    // UpdateGlobalRotations (.cc:523)
         if (bad) { failed = true; break; }                             // .cc:508-512
         curr_norm = norm;
-        if (E > 0) B200_LAUNCH(ctx, ra_residuals, egrid, 256, 0, v, theta.p, 0, 0.0, res.p, w.p, flags.p);   // .cc:524
+        residuals(0, 0.0);                                             // .cc:524
         ++local.l1_iterations;
         if (avg < o.l1_step_convergence_threshold || std::fabs(last_norm - curr_norm) < kRaEps) break;   // .cc:528-535
       }
@@ -465,7 +618,7 @@ struct b200sfm_ra_problem {
       const double sigma = o.irls_loss_parameter_sigma * M_PI / 180.0;
       const int mode = (o.weight_type == 1) ? 2 : 1;
       for (int it = 0; it < o.max_num_irls_iterations; ++it) {
-        if (E > 0) B200_LAUNCH(ctx, ra_residuals, egrid, 256, 0, v, theta.p, mode, sigma * sigma, res.p, w.p, flags.p);
+        residuals(mode, sigma * sigma);
         {
           int hflag = 0;
           B200_CUDA_OK(cudaMemcpyAsync(&hflag, flags.p, sizeof(int), cudaMemcpyDeviceToHost, s));

@@ -1,4 +1,4 @@
-/* b200sfm_testing.h -- test-only probe into a resident bundle-adjustment problem.
+/* b200sfm_testing.h -- test-only probes into resident bundle-adjustment and rotation-averaging problems.
  *
  * NOT part of the drop-in ABI of b200sfm.h: these entry points exist so that the
  * test suite can compare every quantity one Levenberg-Marquardt step forms on the
@@ -67,6 +67,78 @@ int b200sfm_test_ba_step(b200sfm_ba_problem* problem, const b200sfm_ba_opts* opt
 /* y = (S + D) x over the nbk*6 camera-side dofs, with the linearisation and damping of the last
  * b200sfm_test_ba_step, through the mat-vec kernels of the selected path.  x, y: host arrays [nbk*6]. */
 int b200sfm_test_ba_apply(b200sfm_ba_problem* problem, const double* x, double* y);
+
+/* ---- rotation averaging ----------------------------------------------------------------------------------------
+ * A resident rotation-averaging problem, built by the constructor b200sfm_ra_solve_gravity / b200sfm_ra_solve_rig use
+ * (path selection, environment included, is the production one), and probes that run the solver's own stages on it.
+ *
+ * Node vectors hold n = n_frames + n_cams nodes of 3 doubles: the frames' angle-axis rotations, then the unknown
+ * cam_from_rig rotations.  A gravity frame's unknown is its y slot.  Edge vectors hold E = n_edges + 1 edges: the
+ * n_edges pairs, then the gauge pseudo-edge (identity -> fixed frame).  Jacobi blocks are packed 3x3 upper triangles
+ * (6 doubles per node). */
+typedef struct b200sfm_test_ra_problem b200sfm_test_ra_problem;
+
+/* The paths the problem selected.  fused: the fused two-level PCG iteration, read as a solve reads it. */
+typedef struct {
+  int32_t n, n_frames, n_cams, has_grav;
+  int32_t use_csr, use_2lvl, fused, nc;
+  int64_t rows_total, E_total;
+} b200sfm_test_ra_info;
+
+/* Outputs of b200sfm_test_ra_system.  Caller-owned, each may be NULL.  Sizes: res, b [3E]; w [E]; rhs, deg [3n];
+ * Minv [6n]; Ac [nc*nc] (two-level paths only). */
+typedef struct {
+  double* res;      /* residuals at theta */
+  double* w;        /* edge weights of the system (before squaring) */
+  double* b;        /* square = 1 only: the L1 stage's W r */
+  double* rhs;      /* A^T W^p r, p = 1 + square */
+  double* deg;      /* the Laplacian diagonal as the preconditioner sees it */
+  double* Minv;     /* Jacobi blocks */
+  double* Ac;       /* the inverted coarse matrix (P^T L P)^-1 */
+  double b_norm2;   /* square = 1 only: |W r|^2 */
+} b200sfm_test_ra_system_out;
+
+/* Arguments as b200sfm_ra_solve_rig (eci, ecj, cam_frames_begin, cam_frames: NULL when n_cams == 0) plus the gravity
+ * mask of b200sfm_ra_solve_gravity (NULL: none); theta [n*3] is the initial state.  Only opts->use_weight is read. */
+int b200sfm_test_ra_problem_create(b200sfm_ctx* ctx, const b200sfm_ra_opts* opts, int32_t n_frames, int32_t n_cams,
+                                   int64_t n_edges, const int32_t* ei, const int32_t* ej, const int32_t* eci,
+                                   const int32_t* ecj, const double* R_rel, const double* edge_w,
+                                   const uint8_t* frame_has_gravity, const int32_t* cam_frames_begin,
+                                   const int32_t* cam_frames, int32_t fixed_frame, const double* theta,
+                                   b200sfm_test_ra_problem** out);
+void b200sfm_test_ra_problem_free(b200sfm_test_ra_problem* problem);
+
+/* The selected paths; agg_of [n] (may be NULL) receives each node's aggregate on two-level paths. */
+int b200sfm_test_ra_problem_info(b200sfm_test_ra_problem* problem, b200sfm_test_ra_info* info, int32_t* agg_of);
+
+/* Residuals and weights at the current theta (mode 0: the L1 rows' weights, 1: Geman-McClure, 2: half-norm, with
+ * sigma2 = sigma^2 in radians^2), then the linear system as a solve prepares it: square = 1 as the L1 stage does (b = W r,
+ * z = u = 0, the coarse inverse kept while it holds the L1 weights), square = 0 as an IRLS iteration does. */
+int b200sfm_test_ra_system(b200sfm_test_ra_problem* problem, int32_t mode, double sigma2, int32_t square,
+                           b200sfm_test_ra_system_out* out);
+
+/* y = L x through the mat-vec of a PCG iteration on the selected path, with the weights of the last system.
+ * x, y [3n]. */
+int b200sfm_test_ra_apply(b200sfm_test_ra_problem* problem, const double* x, double* y);
+
+/* z = M^-1 r: the Jacobi blocks and, on two-level paths, the coarse correction, as a PCG iteration applies them.
+ * r, z [3n]. */
+int b200sfm_test_ra_precond(b200sfm_test_ra_problem* problem, const double* r, double* z);
+
+/* Exactly k PCG iterations (tolerance 0) on the last system's rhs: cold from x = 0, or warm-started from warm_x [3n]
+ * as the L1 stage's ADMM solves after the first.  x_out [3n]; iterations (may be NULL) receives the count. */
+int b200sfm_test_ra_pcg(b200sfm_test_ra_problem* problem, int32_t k, const double* warm_x, double* x_out,
+                        int32_t* iterations);
+
+/* One ADMM iteration of the L1 stage with the last system's weights after the x-update x [3n]: b [3E], z and u [3E]
+ * (updated in place), rsu [9n] receives rhs | svec | uvec, norms [5] |A_w x - z - b|^2, |A_w x|^2, |z|^2, |svec|^2,
+ * |uvec|^2. */
+int b200sfm_test_ra_admm_step(b200sfm_test_ra_problem* problem, double rho, const double* x, const double* b, double* z,
+                              double* u, double* rsu, double* norms);
+
+/* theta <- theta (+) step, the frames' update and the unknown cameras' quaternion average, as a solve applies a step.
+ * step, theta_out [3n]; sums [3] = average frame step, |step|, NaN flag. */
+int b200sfm_test_ra_update(b200sfm_test_ra_problem* problem, const double* step, double* theta_out, double* sums);
 
 #ifdef __cplusplus
 }

@@ -129,10 +129,12 @@ def test_testing_header_symbols_are_exported_and_mirrored():
 
 def test_testing_header_is_plain_c99_and_its_struct_matches_ctypes(tmp_path):
     import subprocess
-    fields = [f for f, _ in _lib.BAStepProbeOut._fields_]
-    lines = ["#include <stdio.h>", "#include <stddef.h>", '#include "b200sfm_testing.h"', "int main(void) {",
-             '  printf("size %zu\\n", sizeof(b200sfm_test_ba_step_out));']
-    lines += [f'  printf("{f} %zu\\n", offsetof(b200sfm_test_ba_step_out, {f}));' for f in fields]
+    structs = {"b200sfm_test_ba_step_out": _lib.BAStepProbeOut, "b200sfm_test_ra_info": _lib.RAProbeInfo,
+               "b200sfm_test_ra_system_out": _lib.RASystemProbeOut}
+    lines = ["#include <stdio.h>", "#include <stddef.h>", '#include "b200sfm_testing.h"', "int main(void) {"]
+    for cname, cls in structs.items():
+        lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
+        lines += [f'  printf("{cname}.{f} %zu\\n", offsetof({cname}, {f}));' for f, _ in cls._fields_]
     lines += ["  return 0;", "}"]
     src = tmp_path / "probe.c"
     src.write_text("\n".join(lines))
@@ -140,9 +142,10 @@ def test_testing_header_is_plain_c99_and_its_struct_matches_ctypes(tmp_path):
     subprocess.check_call(["/usr/bin/gcc", "-std=c99", "-Wall", "-Wextra", "-pedantic", "-Werror",
                            "-I" + os.path.join(ROOT, "include"), "-o", str(exe), str(src)])
     out = dict(l.split() for l in subprocess.check_output([str(exe)], text=True).splitlines())
-    assert int(out["size"]) == ct.sizeof(_lib.BAStepProbeOut)
-    for f in fields:
-        assert int(out[f]) == getattr(_lib.BAStepProbeOut, f).offset, f
+    for cname, cls in structs.items():
+        assert int(out[cname]) == ct.sizeof(cls), cname
+        for f, _ in cls._fields_:
+            assert int(out[f"{cname}.{f}"]) == getattr(cls, f).offset, f"{cname}.{f}"
 
 
 def test_probe_rejects_a_null_problem_without_touching_the_device():
@@ -152,3 +155,20 @@ def test_probe_rejects_a_null_problem_without_touching_the_device():
     x = (ct.c_double * 6)()
     assert lib.b200sfm_test_ba_step(None, ct.byref(o), 0.0, 1e4, ct.byref(out)) == INVALID
     assert lib.b200sfm_test_ba_apply(None, x, x) == INVALID
+    # rotation averaging (out-of-range indices with a live context: tests/test_ra_system_gpu.py)
+    o_ra, info, sysout = _lib.RAOpts(), _lib.RAProbeInfo(), _lib.RASystemProbeOut()
+    h = ct.c_void_p()
+    ei = (ct.c_int32 * 1)(0)
+    R = (ct.c_double * 9)(1, 0, 0, 0, 1, 0, 0, 0, 1)
+    th = (ct.c_double * 6)()
+    assert lib.b200sfm_test_ra_problem_create(None, ct.byref(o_ra), 2, 0, 1, ei, ei, None, None, R, None, None, None,
+                                              None, 0, th, ct.byref(h)) == INVALID
+    assert not h.value
+    lib.b200sfm_test_ra_problem_free(None)   # no-op
+    assert lib.b200sfm_test_ra_problem_info(None, ct.byref(info), None) == INVALID
+    assert lib.b200sfm_test_ra_system(None, 0, 0.0, 1, ct.byref(sysout)) == INVALID
+    assert lib.b200sfm_test_ra_apply(None, x, x) == INVALID
+    assert lib.b200sfm_test_ra_precond(None, x, x) == INVALID
+    assert lib.b200sfm_test_ra_pcg(None, 1, None, x, None) == INVALID
+    assert lib.b200sfm_test_ra_admm_step(None, 1.0, x, x, x, x, x, x) == INVALID
+    assert lib.b200sfm_test_ra_update(None, x, x, x) == INVALID
