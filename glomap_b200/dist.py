@@ -32,11 +32,12 @@ def shard_scene(scene, rank: int, world: int, chunk: int = 1):
     from .synthetic import RigScene, Scene
     a, b = shard_range(scene.P, chunk, rank, world)
     o0, o1 = int(scene.pt_obs_begin[a]), int(scene.pt_obs_begin[b])
-    if isinstance(scene, RigScene):   # known rigs: frames, sensors and intrinsics are replicated
+    if isinstance(scene, RigScene):   # known rigs: frames, sensors, intrinsics and the rig layout are replicated
         return RigScene(scene.quat.copy(), scene.trans.copy(), scene.points[a:b].copy(),
                         (scene.pt_obs_begin[a:b + 1] - o0).astype(np.int64), scene.obs_frame[o0:o1], scene.obs_sensor[o0:o1],
                         scene.obs_xy[o0:o1], scene.sensor_quat.copy(), scene.sensor_trans.copy(), scene.sensor_intr,
-                        scene.intr_model, scene.intr_params.copy()), (a, b)
+                        scene.intr_model, scene.intr_params.copy(), scene.image_frame, scene.image_sensor, scene.frame_rig,
+                        scene.sensor_rig, scene.rig_ref_sensor, scene.sensor_known), (a, b)
     return Scene(scene.quat.copy(), scene.trans.copy(), scene.points[a:b].copy(), (scene.pt_obs_begin[a:b + 1] - o0).astype(np.int64),
                  scene.obs_cam[o0:o1], scene.obs_xy[o0:o1], scene.cam_intr, scene.intr_model, scene.intr_params.copy()), (a, b)
 

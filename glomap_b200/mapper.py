@@ -15,10 +15,20 @@ keeps its input pose, as in the reference, where its frame is simply not optimis
 
 It mirrors the reference's control flow so that the GPU solvers are exercised in the order, and with the option
 mutations, the real mapper uses; it is host glue (as in the reference) and owns no numerics: every solve and every
-filter goes through ``libb200sfm.so``.  Trivial frames only.  Stage 4, track establishment (``TrackEngine``:
-EstablishFullTracks, then FindTracksForProblem, both on the device), runs when ``Solve`` is given the image pairs and
-features.  Not covered here: view-graph calibration, relative-pose estimation, retriangulation (COLMAP code in the
-reference)."""
+filter goes through ``libb200sfm.so``.  Stage 4, track establishment (``TrackEngine``: EstablishFullTracks, then
+FindTracksForProblem, both on the device), runs when ``Solve`` is given the image pairs and features.  Not covered here:
+view-graph calibration, relative-pose estimation, retriangulation (COLMAP code in the reference).
+
+``Solve`` takes trivial frames (``synthetic.Scene``, one camera = one frame) or camera rigs (``synthetic.RigScene``: several
+rigs, each frame seen through the sensors of its rig, cam_from_rig known or not).  On rigs, stage 3 runs
+``rotation_averager.solve_rotation_averaging_rig`` (which estimates the unknown cam_from_rig rotations; they get a NaN
+translation) and filters the image rotations cam_from_rig * rig_from_world; the largest component is taken in frame
+space, and an image is registered when its frame is (``frame_in_component`` / ``image_registered``).  Stages 4-6 run on
+the problem compacted to the registered frames and the sensors they use: the selected tracks become (frame, sensor)
+observations (``track_establishment.tracks_to_rig_scene``), global positioning uses the known cam_from_rig as offsets
+and solves the NaN translations as RigUnknownBATA centres, then the filters, the normalisation and the staged bundle
+adjustment run on the rig problem (with ``opt_ba.optimize_rig_poses`` every non-reference cam_from_rig is refined).
+An unregistered frame keeps its input pose, a sensor without a registered image its input cam_from_rig."""
 from __future__ import annotations
 
 import dataclasses
@@ -61,12 +71,17 @@ class GlobalMapperOptions:
 
 
 def compact_observations(scene: S.Scene, keep: np.ndarray) -> S.Scene:
-    """Drop the observations with keep == False (what the filters do to ``Track::observations``)."""
+    """Drop the observations with keep == False (what the filters do to ``Track::observations``); ``scene`` may be a
+    ``Scene`` or a ``RigScene``."""
     keep = np.asarray(keep, bool)
     pt = np.repeat(np.arange(scene.P), np.diff(scene.pt_obs_begin))
     lens = np.bincount(pt[keep], minlength=scene.P)
     out = scene.copy()
-    out.obs_cam, out.obs_xy = scene.obs_cam[keep], scene.obs_xy[keep]
+    if isinstance(scene, S.RigScene):
+        out.obs_frame, out.obs_sensor = scene.obs_frame[keep], scene.obs_sensor[keep]
+    else:
+        out.obs_cam = scene.obs_cam[keep]
+    out.obs_xy = scene.obs_xy[keep]
     out.pt_obs_begin = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
     return out
 
@@ -141,6 +156,52 @@ def scatter_cameras(full: S.Scene, part: S.Scene, idx: np.ndarray) -> S.Scene:
     return out
 
 
+def compact_frames(scene: S.RigScene, frames: np.ndarray):
+    """The rig problem over the frames ``frames`` (ascending), renumbered in that order: their images (in table order),
+    the sensors those images use (ascending, renumbered; a rig whose reference sensor is dropped gets -1), the
+    observations of those images; every point and intrinsics block is kept.  Returns (scene, sensor ids)."""
+    frames = np.asarray(frames, np.int64)
+    fmap = np.full(scene.F, -1, np.int64)
+    fmap[frames] = np.arange(len(frames))
+    img = fmap[scene.image_frame] >= 0
+    sensors = np.unique(scene.image_sensor[img]).astype(np.int64)
+    smap = np.full(scene.S, -1, np.int64)
+    smap[sensors] = np.arange(len(sensors))
+    out = compact_observations(scene, fmap[scene.obs_frame] >= 0)
+    out.obs_frame = fmap[out.obs_frame].astype(np.int32)
+    out.obs_sensor = smap[out.obs_sensor].astype(np.uint16)
+    out.quat, out.trans = scene.quat[frames].copy(), scene.trans[frames].copy()
+    out.sensor_quat, out.sensor_trans = scene.sensor_quat[sensors].copy(), scene.sensor_trans[sensors].copy()
+    out.sensor_intr, out.sensor_known = scene.sensor_intr[sensors].copy(), scene.sensor_known[sensors].copy()
+    out.sensor_rig, out.frame_rig = scene.sensor_rig[sensors].copy(), scene.frame_rig[frames].copy()
+    out.rig_ref_sensor = smap[scene.rig_ref_sensor].astype(np.int32)
+    out.image_frame = fmap[scene.image_frame[img]].astype(np.int32)
+    out.image_sensor = smap[scene.image_sensor[img]].astype(np.int32)
+    return out, sensors
+
+
+def scatter_frames(full: S.RigScene, part: S.RigScene, frames: np.ndarray, sensors: np.ndarray) -> S.RigScene:
+    """Inverse of ``compact_frames``: ``full`` with the poses of the frames ``frames`` and the cam_from_rig (and known
+    flag) of the sensors ``sensors`` from ``part``, and its points, tracks and intrinsics; the other frames and sensors
+    keep theirs."""
+    frames, sensors = np.asarray(frames, np.int64), np.asarray(sensors, np.int64)
+    out = full.copy()
+    out.quat[frames], out.trans[frames] = part.quat, part.trans
+    out.sensor_quat[sensors], out.sensor_trans[sensors] = part.sensor_quat, part.sensor_trans
+    out.sensor_known[sensors] = part.sensor_known
+    out.points, out.pt_obs_begin = part.points.copy(), part.pt_obs_begin.copy()
+    out.obs_frame = frames[part.obs_frame].astype(np.int32)
+    out.obs_sensor = sensors[part.obs_sensor.astype(np.int64)].astype(np.uint16)
+    out.obs_xy = part.obs_xy.copy()
+    out.intr_model, out.intr_params = part.intr_model.copy(), part.intr_params.copy()
+    return out
+
+
+def _ra_options(o: E.RotationEstimatorOptions):
+    from . import rotation_averager as RA
+    return RA.RotationAveragerOptions(**dataclasses.asdict(o))
+
+
 class GlobalMapper:
     def __init__(self, options: GlobalMapperOptions | None = None, ctx: E.Context | None = None):
         self.options_ = options or GlobalMapperOptions()
@@ -149,6 +210,7 @@ class GlobalMapper:
         self.frame_cluster_id: np.ndarray | None = None   # stage 8: cluster of every frame (-1: none)
         self.frame_registered: np.ndarray | None = None   # stage 8: frames of the largest visibility component
         self.image_registered: np.ndarray | None = None   # stage 3: images of the view graph's largest component
+        self.frame_in_component: np.ndarray | None = None  # stage 3, rigs: frames of the view graph's largest component
 
     # -- helpers ------------------------------------------------------------------------------------
     def _filters(self, scene: S.Scene, what) -> S.Scene:
@@ -176,19 +238,25 @@ class GlobalMapper:
 
     def _filter_rotations(self, vg: S.ViewGraph, q_rel, R, valid, registered, max_angle):
         """RelPoseFilter::FilterRotations: (valid, pairs invalidated)."""
-        q_img = geo.rotmat_to_quat_xyzw_fast(R)
+        return self._filter_rotations_q(vg, q_rel, geo.rotmat_to_quat_xyzw_fast(R), valid, registered, max_angle)
+
+    def _filter_rotations_q(self, vg: S.ViewGraph, q_rel, q_img, valid, registered, max_angle):
         if vg.E >= VIEW_GRAPH_DEVICE_MIN_PAIRS:
             return VG.filter_rotations_device(q_img, vg.ei, vg.ej, q_rel, max_angle, valid, registered,
                                               self.ctx or E.default_context())
         return VG.filter_rotations(q_img, vg.ei, vg.ej, q_rel, max_angle, valid, registered)
 
-    def _largest_component(self, vg: S.ViewGraph, valid, registered):
-        """ViewGraph::KeepLargestConnectedComponents, frames = images: (valid, registered, registered images)."""
-        frame = np.arange(vg.n_images, dtype=np.int32)
+    def _largest_component(self, vg: S.ViewGraph, valid, registered, image_frame=None):
+        """ViewGraph::KeepLargestConnectedComponents in frame space (frames = images unless ``image_frame`` [I] is
+        given, with ``registered`` then one flag per frame): (valid, registered, registered images)."""
+        if image_frame is None:
+            frame, F = np.arange(vg.n_images, dtype=np.int32), vg.n_images
+        else:
+            frame, F = image_frame, len(registered)
         if vg.E >= VIEW_GRAPH_DEVICE_MIN_PAIRS:
-            return VG.keep_largest_connected_components_device(vg.n_images, frame, vg.ei, vg.ej, valid, registered,
+            return VG.keep_largest_connected_components_device(F, frame, vg.ei, vg.ej, valid, registered,
                                                                self.ctx or E.default_context())
-        return VG.keep_largest_connected_components(vg.n_images, frame, vg.ei, vg.ej, valid, registered)
+        return VG.keep_largest_connected_components(F, frame, vg.ei, vg.ej, valid, registered)
 
     # -- controllers/global_mapper.cc:19-355 (stages 3, 5, 6) -----------------------------------------
     def Solve(self, view_graph: S.ViewGraph, scene: S.Scene, image_pairs=None, features: dict | None = None):
@@ -196,7 +264,13 @@ class GlobalMapper:
         ``view_graph`` and the tracks of ``scene`` (its poses and points are only used when a stage is skipped).
         Given ``image_pairs`` (``track_establishment.ImagePairMatches``) and ``features`` ({image_id: [n,2] pixels}; camera k
         of ``scene`` is the k-th smallest image id), stage 4 builds the tracks on the device instead and the tracks of
-        ``scene`` are not used."""
+        ``scene`` are not used.
+
+        ``scene`` may be a ``synthetic.RigScene`` instead: ``view_graph`` is then over its images (image k = row k of the
+        image table, and the k-th smallest id of ``features``), the poses are the frames' rig_from_world, and the
+        sensors whose cam_from_rig is not known are estimated (see ``_solve_rig``)."""
+        if isinstance(scene, S.RigScene):
+            return self._solve_rig(view_graph, scene, image_pairs, features)
         o, thr = self.options_, self.options_.inlier_thresholds
         scene = scene.copy()
         track_stage = image_pairs is not None and features is not None and not o.skip_track_establishment
@@ -262,17 +336,123 @@ class GlobalMapper:
             self.log.append(f"pruning: {out['num_clusters']} clusters, threshold {out['stats']['strong_threshold']:g}")
         return True, scene
 
+    def _rotation_averaging_rig(self, vg: S.ViewGraph, scene: S.RigScene) -> bool:
+        """Stage 3 on rigs (:84-116): SolveRotationAveraging twice, each run followed by FilterRotations on the image
+        rotations cam_from_rig * rig_from_world and KeepLargestConnectedComponents in frame space.  Sets
+        ``frame_in_component`` / ``image_registered`` and, in ``scene``, the rotations of the frames in the component
+        and those of the sensors it estimated (with a NaN translation, global_rotation_averaging.cc:800-813)."""
+        from . import rotation_averager as RA
+        o, thr = self.options_, self.options_.inlier_thresholds
+        fr, sen = scene.image_frame.astype(np.int64), scene.image_sensor.astype(np.int64)
+        ref_sensor = scene.rig_ref_sensor[scene.frame_rig]
+        known = scene.sensor_known.copy()
+        known[scene.rig_ref_sensor] = True
+        q_cam = scene.sensor_quat.copy()
+        q_rel = geo.rotmat_to_quat_xyzw_fast(vg.R_rel)
+        valid, freg = np.ones(vg.E, bool), np.ones(scene.F, bool)
+        R = geo.quat_xyzw_to_rotmat(scene.quat)
+        estimated = np.zeros(scene.S, bool)
+        ra_opts = _ra_options(o.opt_ra)
+        for run in range(2):
+            valid, freg, num_img = self._largest_component(vg, valid, freg, fr)
+            self.frame_in_component, self.image_registered = freg, freg[fr]
+            if num_img == 0:
+                self.log.append(f"rotation averaging run {run + 1}: no pair is left")
+                return False
+            ok, R_run, R_cam, solved = RA.solve_rotation_averaging_rig(_sub_view_graph(vg, valid), fr, sen, known, q_cam,
+                                                                       ref_sensor, ra_opts, R_init=R, ctx=self.ctx)
+            if not ok:
+                if run == 1:
+                    return False
+                continue
+            R = R_run
+            seen = np.zeros(scene.S, bool)
+            seen[sen[solved[fr]]] = True
+            new = seen & ~known                        # these cam_from_rig have a value from now on (.cc:800-813)
+            q_cam[new] = geo.rotmat_to_quat_xyzw_fast(R_cam[new])
+            known |= new
+            estimated |= new
+            # the image rotations; an image whose sensor has no rotation yet is NaN and keeps its pairs
+            q_img = geo.rotmat_to_quat_xyzw_fast(np.einsum("nij,njk->nik", geo.quat_xyzw_to_rotmat(q_cam)[sen], R[fr]))
+            q_img[~known[sen]] = np.nan
+            valid, cut = self._filter_rotations_q(vg, q_rel, q_img, valid, freg[fr], thr.max_rotation_error)
+            valid, freg, num_img = self._largest_component(vg, valid, freg, fr)
+            self.frame_in_component, self.image_registered = freg, freg[fr]
+            if num_img == 0:
+                self.log.append(f"rotation averaging run {run + 1}: no connected component is left")
+                return False
+            self.log.append(f"rotation averaging run {run + 1}: {cut} edges filtered, {num_img} / {scene.I} images in "
+                            f"the largest component ({int(freg.sum())} / {scene.F} frames)")
+        scene.quat = np.where(freg[:, None], geo.rotmat_to_quat_xyzw_fast(R), scene.quat)
+        has_image = np.zeros(scene.S, bool)
+        has_image[sen[freg[fr]]] = True
+        estimated &= has_image                         # a sensor without a registered image keeps its input
+        scene.sensor_quat[estimated] = q_cam[estimated]
+        scene.sensor_trans[estimated] = np.nan
+        return True
+
+    def _solve_rig(self, view_graph: S.ViewGraph, scene: S.RigScene, image_pairs=None, features: dict | None = None):
+        """``Solve`` on rigs (global_mapper.cc:82-353).  Stage 3 (``_rotation_averaging_rig``) registers the images of
+        the frames in the view graph's largest component.  Stages 4-6 run on the problem compacted to those frames and
+        the sensors their images use: tracks over the registered images, global positioning with the known
+        cam_from_rig as offsets and the sensors with a NaN translation as RigUnknownBATA centres (ConvertResults turns
+        them into translations), the filters and normalisation on the rig problem, then the staged bundle adjustment
+        (with ``opt_ba.optimize_rig_poses`` every non-reference sensor is a variable).  The results are scattered back:
+        an unregistered frame keeps its input pose, a sensor without a registered image its input cam_from_rig.
+        Stage 8 prunes in frame space."""
+        o = self.options_
+        full = scene.copy()
+        track_stage = image_pairs is not None and features is not None and not o.skip_track_establishment
+        self.frame_in_component = np.ones(full.F, bool)
+        self.image_registered = np.ones(full.I, bool)
+        if not o.skip_rotation_averaging and not self._rotation_averaging_rig(view_graph, full):
+            return False, scene
+        frames = np.flatnonzero(self.frame_in_component)
+        part, sensors = compact_frames(full, frames)
+        # 4. track establishment (:119-137) over the registered images
+        if track_stage:
+            image_ids = sorted(int(i) for i in features)
+            if len(image_ids) != full.I:
+                raise ValueError(f"features name {len(image_ids)} images, the scene has {full.I}")
+            reg_ids = [image_ids[k] for k in np.flatnonzero(self.image_registered)]
+            full_tracks, discarded = TE.establish_full_tracks_device(image_pairs, features, o.opt_track, self.ctx)
+            sel = TE.find_tracks_for_problem_device(full_tracks, reg_ids, o.opt_track, self.ctx)
+            part = TE.tracks_to_rig_scene(sel, features, reg_ids, part)
+            self.log.append(f"track establishment: {len(full_tracks)} tracks ({discarded} discarded), {len(sel)} selected")
+        ok, part = self._solve_positions(part)
+        out = scatter_frames(full, part, frames, sensors)
+        if not ok:
+            return False, out
+        # 8. reconstruction pruning (:340-353) over the frames of the observations
+        if not o.skip_pruning:
+            images = np.bincount(out.image_frame[self.image_registered], minlength=out.F)
+            res = RP.prune_weakly_connected_images(out.pt_obs_begin, out.obs_frame, out.F, frame_self_loop=images >= 2,
+                                                   ctx=self.ctx)
+            self.frame_cluster_id, self.frame_registered = res["cluster_id"], res["is_registered"]
+            self.log.append(f"pruning: {res['num_clusters']} clusters, threshold {res['stats']['strong_threshold']:g}")
+        return True, out
+
     def _solve_positions(self, scene: S.Scene):
-        """Stages 5 and 6 on the registered cameras: (ok, scene)."""
+        """Stages 5 and 6 on the registered cameras (or frames, for a ``RigScene``): (ok, scene)."""
         o, thr = self.options_, self.options_.inlier_thresholds
         # 5. global positioning (:143-189)
         if not o.skip_global_positioning:
             bear = PR.undistort_images(scene)
             gp = E.GlobalPositioner(o.opt_gp, self.ctx)
-            prob = E.PositioningProblem(scene.quat, scene.pt_obs_begin, scene.obs_cam, bear, centers=None, points=None)
+            if isinstance(scene, S.RigScene):
+                # RigBATA with the known cam_from_rig; a NaN translation (rotation averaging's estimate) is unknown
+                unk = np.isnan(scene.sensor_trans).any(axis=1)
+                prob = E.PositioningProblem(scene.quat, scene.pt_obs_begin, scene.obs_frame, bear, obs_sensor=scene.obs_sensor,
+                                            sensor_quat=scene.sensor_quat, sensor_trans=scene.sensor_trans,
+                                            sensor_unknown=unk if unk.any() else None)
+            else:
+                prob = E.PositioningProblem(scene.quat, scene.pt_obs_begin, scene.obs_cam, bear, centers=None, points=None)
             if not gp.Solve(prob):
                 return False, scene
             scene.trans, scene.points = prob.trans, prob.points
+            if isinstance(scene, S.RigScene) and prob.sensor_unknown is not None:
+                scene.sensor_trans = prob.sensor_trans                   # ConvertResults (.cc:578-582)
+                scene.sensor_known = scene.sensor_known | prob.sensor_unknown
             scene = self._filters(scene, [("angle", thr.max_angle_error), ("triangulation", thr.min_triangulation_angle),
                                           ("reprojection", 10 * thr.max_reprojection_error)])
             PR.normalize_reconstruction(scene)

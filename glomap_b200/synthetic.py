@@ -233,9 +233,14 @@ def perturb_scene(scene: Scene, rot_deg: float = 0.5, center_frac: float = 0.01,
 
 @dataclasses.dataclass
 class RigScene:
-    """Flat BA/GP problem with KNOWN camera rigs (b200sfm_ba_problem_create_rig): the pose unknowns are
-    the F frames (rig_from_world); image (f, s) = frame f seen through sensor s, whose cam_from_rig and
-    intrinsics block are constants of the sensor (glomap/scene/frame.h, colmap::Rig)."""
+    """Flat BA/GP problem with camera rigs (b200sfm_ba_problem_create_rig): the pose unknowns are
+    the F frames (rig_from_world); an image is a frame seen through one sensor, whose cam_from_rig and
+    intrinsics block are constants of the sensor (glomap/scene/frame.h, colmap::Rig).
+
+    The image table (``image_frame`` / ``image_sensor``, image k = row k) and the rigs (``frame_rig``, ``sensor_rig``,
+    ``rig_ref_sensor``) describe which sensors a frame uses; ``sensor_known`` marks the sensors whose cam_from_rig is
+    known (a rig's reference sensor is, with the identity).  Left as None they default to the dense layout: one rig of
+    all S sensors, sensor 0 its reference, every sensor known and image f * S + s = (frame f, sensor s)."""
     quat: np.ndarray          # [F,4] xyzw rig_from_world
     trans: np.ndarray         # [F,3]
     points: np.ndarray        # [P,3]
@@ -244,10 +249,53 @@ class RigScene:
     obs_sensor: np.ndarray    # [N] uint16
     obs_xy: np.ndarray        # [N,2] pixels
     sensor_quat: np.ndarray   # [S,4] xyzw cam_from_rig
-    sensor_trans: np.ndarray  # [S,3]
+    sensor_trans: np.ndarray  # [S,3] (NaN rows: translation not estimated yet)
     sensor_intr: np.ndarray   # [S] int32 -> intrinsics block
     intr_model: np.ndarray    # [K] int32
     intr_params: np.ndarray   # [K, INTR_STRIDE]
+    image_frame: np.ndarray | None = None     # [I] int32 frame of every image
+    image_sensor: np.ndarray | None = None    # [I] int32 sensor of every image
+    frame_rig: np.ndarray | None = None       # [F] int32
+    sensor_rig: np.ndarray | None = None      # [S] int32
+    rig_ref_sensor: np.ndarray | None = None  # [R] int32 reference sensor of every rig
+    sensor_known: np.ndarray | None = None    # [S] bool cam_from_rig known
+
+    def __post_init__(self):
+        F, S = len(self.quat), len(self.sensor_quat)
+        if self.image_frame is None:
+            self.image_frame = np.repeat(np.arange(F), S).astype(np.int32)
+        if self.image_sensor is None:
+            self.image_sensor = np.tile(np.arange(S), F).astype(np.int32)
+        if self.frame_rig is None:
+            self.frame_rig = np.zeros(F, np.int32)
+        if self.sensor_rig is None:
+            self.sensor_rig = np.zeros(S, np.int32)
+        if self.rig_ref_sensor is None:
+            self.rig_ref_sensor = np.zeros(1, np.int32)
+        if self.sensor_known is None:
+            self.sensor_known = np.ones(S, bool)
+
+    @property
+    def I(self):  # noqa: E743
+        return len(self.image_frame)
+
+    @property
+    def sensor_is_ref(self):
+        """[S] bool: the reference sensor of its rig (the sensors optimize_rig_poses keeps constant)."""
+        ref = np.zeros(self.S, bool)
+        r = np.asarray(self.rig_ref_sensor, np.int64)
+        ref[r[r >= 0]] = True
+        return ref
+
+    def image_index(self):
+        """[F, S] image of (frame, sensor), -1 where the table has none."""
+        idx = np.full((self.F, self.S), -1, np.int64)
+        idx[self.image_frame, self.image_sensor] = np.arange(self.I)
+        return idx
+
+    def obs_image(self):
+        """[N] image of every observation."""
+        return self.image_index()[self.obs_frame, self.obs_sensor]
 
     @property
     def C(self):
@@ -273,28 +321,26 @@ class RigScene:
         return RigScene(*[np.array(getattr(self, f.name), copy=True) for f in dataclasses.fields(self)])
 
     def image_poses(self):
-        """cam_from_world of all F*S images, image id = f * S + s."""
-        Rf = geo.quat_xyzw_to_rotmat(self.quat)
-        Rs = geo.quat_xyzw_to_rotmat(self.sensor_quat)
-        R = np.einsum("sij,fjk->fsik", Rs, Rf).reshape(-1, 3, 3)
-        t = (np.einsum("sij,fj->fsi", Rs, self.trans) + self.sensor_trans[None]).reshape(-1, 3)
+        """cam_from_world of the images of the table (dense layout: image id = f * S + s)."""
+        Rf = geo.quat_xyzw_to_rotmat(self.quat)[self.image_frame]
+        Rs = geo.quat_xyzw_to_rotmat(self.sensor_quat)[self.image_sensor]
+        R = np.einsum("nij,njk->nik", Rs, Rf)
+        t = np.einsum("nij,nj->ni", Rs, self.trans[self.image_frame]) + self.sensor_trans[self.image_sensor]
         return R, t
 
     def images_scene(self) -> Scene:
-        """The same observations as a trivial-frame Scene over the F*S images (poses composed)."""
+        """The same observations as a trivial-frame Scene over the images of the table (poses composed)."""
         R, t = self.image_poses()
-        obs_cam = (self.obs_frame.astype(np.int64) * self.S + self.obs_sensor).astype(np.int32)
-        cam_intr = np.tile(self.sensor_intr, self.F).astype(np.int32)
-        return Scene(geo.rotmat_to_quat_xyzw_fast(R), t, self.points.copy(), self.pt_obs_begin.copy(), obs_cam,
-                     self.obs_xy.copy(), cam_intr, self.intr_model.copy(), self.intr_params.copy())
+        return Scene(geo.rotmat_to_quat_xyzw_fast(R), t, self.points.copy(), self.pt_obs_begin.copy(),
+                     self.obs_image().astype(np.int32), self.obs_xy.copy(), self.sensor_intr[self.image_sensor].astype(np.int32),
+                     self.intr_model.copy(), self.intr_params.copy())
 
     def rig_dict(self):
-        """The ``rig`` argument of oracle.ba_oracle (per-image arrays, image id = f * S + s)."""
-        # img_sensor / sensor_q / sensor_t are read only with optimize_rig_poses (sensor 0 = reference sensor: constant)
-        img_sensor = np.tile(np.where(np.arange(self.S) == 0, -1, np.arange(self.S)), self.F)
-        return dict(obs_img=self.obs_frame.astype(np.int64) * self.S + self.obs_sensor,
-                    img_q=np.tile(self.sensor_quat, (self.F, 1)), img_t=np.tile(self.sensor_trans, (self.F, 1)),
-                    img_intr=np.tile(self.sensor_intr, self.F), img_sensor=img_sensor,
+        """The ``rig`` argument of oracle.ba_oracle (per-image arrays over the image table)."""
+        # img_sensor / sensor_q / sensor_t are read only with optimize_rig_poses (reference sensors: constant)
+        sen = self.image_sensor
+        return dict(obs_img=self.obs_image(), img_q=self.sensor_quat[sen].copy(), img_t=self.sensor_trans[sen].copy(),
+                    img_intr=self.sensor_intr[sen].copy(), img_sensor=np.where(self.sensor_is_ref[sen], -1, sen),
                     sensor_q=self.sensor_quat.copy(), sensor_t=self.sensor_trans.copy())
 
 
@@ -362,6 +408,77 @@ def perturb_rig_scene(scene: RigScene, rot_deg: float = 0.5, center_frac: float 
     out.trans = -np.einsum("nij,nj->ni", Rn, cn)
     out.points = scene.points + rng.normal(size=scene.points.shape) * point_frac * 3.0 / np.sqrt(3)
     return out
+
+
+@dataclasses.dataclass
+class RigDataset:
+    """A rig problem with everything the mapper takes (``mapper.GlobalMapper.Solve``)."""
+    scene: RigScene           # ground truth: poses, cam_from_rig, points and their observations
+    view_graph: ViewGraph     # image level (image k = row k of the scene's image table)
+    matches: dict             # make_pair_matches of scene.images_scene()
+    features: dict            # {image id: [n,2] pixels}, image id k = image k
+    image_pairs: list         # track_establishment.ImagePairMatches, every match an inlier
+
+
+def make_rig_dataset(num_rigs: int, cameras_per_rig: int, frames_per_rig: int, num_points: int,
+                     sensor_from_rig_translation_stddev: float = 0.1, sensor_from_rig_rotation_stddev: float = 5.0,
+                     pixel_sigma: float = 0.0, seed: int = 1, rotation_noise_deg: float = 0.0, min_shared: int = 10,
+                     model: int = SIMPLE_PINHOLE, focal: float = 1000.0, image_size: int = 1000,
+                     world_scale: float = 0.1) -> RigDataset:
+    """Rigs in the shape of ``colmap::SynthesizeDataset``: ``num_rigs`` rigs of ``cameras_per_rig`` cameras, each with
+    ``frames_per_rig`` frames (frame f belongs to rig f // frames_per_rig; rig r owns sensors r * cameras_per_rig ...,
+    the first its reference sensor with the identity cam_from_rig).  The other sensors are turned by a normal rotation
+    vector of ``sensor_from_rig_rotation_stddev`` degrees per axis and shifted by a normal translation of
+    ``sensor_from_rig_translation_stddev`` per axis.  Every sensor has its own intrinsics block and is known.  Frames sit on
+    a shell r in [8, 12] * ``world_scale`` looking at a ball of radius 3 * ``world_scale``; every image that sees a point
+    observes it, with ``pixel_sigma`` pixels of noise.  The default ``world_scale`` puts the points about one unit from
+    the frames: global positioning fixes its gauge by holding one observation's scale and the rig scale at 1
+    (global_positioning.cc:484-497), so known cam_from_rig translations agree with its solution only in a world of
+    about that size.  The view graph is ``view_graph_from_scene`` of ``images_scene()`` (pairs sharing >= ``min_shared``
+    points, ``rotation_noise_deg`` of rotation noise), the matches ``make_pair_matches`` without outliers."""
+    rng = np.random.default_rng([seed, 101])
+    R_, C_, F_ = int(num_rigs), int(cameras_per_rig), int(frames_per_rig)
+    F, S = R_ * F_, R_ * C_
+    Rf, tf = make_cameras(F, seed=seed, jitter_deg=5.0)
+    tf = tf * world_scale
+    w = rng.normal(size=(S, 3)) * np.radians(sensor_from_rig_rotation_stddev)
+    ts = rng.normal(size=(S, 3)) * sensor_from_rig_translation_stddev
+    ref = np.arange(R_) * C_
+    w[ref], ts[ref] = 0.0, 0.0
+    _, intr_model, intr_params = make_intrinsics(S, model, focal, image_size, S)
+    frame_rig = (np.arange(F) // F_).astype(np.int32)
+    image_frame = np.repeat(np.arange(F), C_).astype(np.int32)
+    image_sensor = (frame_rig[image_frame] * C_ + np.tile(np.arange(C_), F)).astype(np.int32)
+    scene = RigScene(geo.rotmat_to_quat_xyzw_fast(Rf), tf, np.zeros((0, 3)), np.zeros(1, np.int64), np.zeros(0, np.int32),
+                     np.zeros(0, np.uint16), np.zeros((0, 2)), geo.rotmat_to_quat_xyzw_fast(geo.so3_exp(w)), ts,
+                     np.arange(S, dtype=np.int32), intr_model, intr_params, image_frame, image_sensor, frame_rig,
+                     (np.arange(S) // C_).astype(np.int32), ref.astype(np.int32), np.ones(S, bool))
+    Ri, ti = scene.image_poses()
+    d = rng.normal(size=(num_points, 3))
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    points = d * 3.0 * world_scale * rng.uniform(0, 1, size=(num_points, 1)) ** (1 / 3)
+    Xc = np.einsum("nij,pj->pni", Ri, points) + ti[None]                   # [P, I, 3]
+    lim = 0.5 * image_size / focal * 1.2
+    with np.errstate(divide="ignore", invalid="ignore"):
+        vis = (Xc[..., 2] > 0.5 * world_scale) & (np.abs(Xc[..., 0] / Xc[..., 2]) < lim) & (np.abs(Xc[..., 1] / Xc[..., 2]) < lim)
+    p_idx, img = np.nonzero(vis)                                            # by point, then by image
+    xy = np.empty((len(img), 2))
+    for s in range(S):
+        m = image_sensor[img] == s
+        xy[m] = project(int(intr_model[s]), intr_params[s], Xc[p_idx[m], img[m]])
+    if pixel_sigma > 0:
+        xy += rng.normal(size=xy.shape) * pixel_sigma
+    scene.points = points
+    scene.pt_obs_begin = np.concatenate([[0], np.cumsum(vis.sum(1))]).astype(np.int64)
+    scene.obs_frame, scene.obs_sensor = image_frame[img], image_sensor[img].astype(np.uint16)
+    scene.obs_xy = xy
+    images = scene.images_scene()
+    vg = view_graph_from_scene(images, min_shared=min_shared, seed=seed, noise_deg=rotation_noise_deg)
+    matches = make_pair_matches(images, seed=seed, outlier_frac=0.0)
+    features, _, pairs = pairs_from_match_arrays(matches)
+    for p in pairs:
+        p.inliers = np.arange(len(p.matches))
+    return RigDataset(scene, vg, matches, features, pairs)
 
 
 def bearings_from_scene(scene: Scene) -> np.ndarray:

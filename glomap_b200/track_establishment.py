@@ -16,7 +16,7 @@ Both run on the GPU as well, with the same result: ``establish_full_tracks_devic
 Global feature id = image_id << 32 | feature_id (:48-53); a track is identified by the smallest global id of its
 component (the reference roots the union at the smaller id).  Observations inside a track are sorted by global id
 (the reference iterates an unordered_set; the order is immaterial to the solvers).
-The GPU solvers consume the result through ``tracks_to_scene``."""
+The GPU solvers consume the result through ``tracks_to_scene`` (``tracks_to_rig_scene`` for rigs)."""
 from __future__ import annotations
 
 import dataclasses
@@ -255,6 +255,34 @@ def find_tracks_for_problem_device(tracks: Tracks, registered_images, options: T
     lens = np.diff(begin)[sel]
     sel = sel[np.lexsort((ids[sel], lens))[::-1]]            # descending (length, id), the reference's processing order
     return restrict_to_images(_subset(tracks, sel), reg)
+
+
+def tracks_to_rig_scene(tracks: Tracks, features: dict, image_ids, rig_scene):
+    """The rig counterpart of ``tracks_to_scene``: ``rig_scene`` (a ``synthetic.RigScene``) with its tracks replaced by
+    ``tracks`` -- in ascending track id, each observation as (frame, sensor, pixel), points zero.  The image of the k-th
+    smallest of ``image_ids`` is image k of the scene's table.  Frames, sensors and intrinsics are shared with
+    ``rig_scene``."""
+    import dataclasses as dc
+    begin, fr, se, xy = _rig_observations(tracks, features, image_ids, rig_scene.image_frame, rig_scene.image_sensor)
+    return dc.replace(rig_scene, points=np.zeros((len(begin) - 1, 3)), pt_obs_begin=begin, obs_frame=fr, obs_sensor=se,
+                      obs_xy=xy)
+
+
+def _rig_observations(tracks: Tracks, features: dict, image_ids, image_frame, image_sensor):
+    """(pt_obs_begin, obs_frame, obs_sensor, obs_xy) of ``tracks_to_rig_scene``, without a loop over observations."""
+    image_ids = np.asarray(sorted(int(i) for i in image_ids), np.int64)
+    order = np.argsort(tracks.track_ids, kind="stable")
+    lens = np.diff(tracks.begin)[order]
+    begin = np.concatenate([[0], np.cumsum(lens)]).astype(np.int64)
+    src = np.repeat(np.asarray(tracks.begin, np.int64)[order] - begin[:-1], lens) + np.arange(begin[-1])
+    img = np.searchsorted(image_ids, tracks.obs_image[src].astype(np.int64))
+    if len(img) and (img.max() >= len(image_ids) or (image_ids[img] != tracks.obs_image[src]).any()):
+        raise ValueError("a track observes an image that image_ids does not name")
+    feats = [np.asarray(features[int(i)], np.float64).reshape(-1, 2) for i in image_ids]
+    feat_begin = np.concatenate([[0], np.cumsum([len(f) for f in feats])]).astype(np.int64)
+    all_xy = np.concatenate(feats) if feats else np.zeros((0, 2))
+    xy = all_xy[feat_begin[img] + tracks.obs_feature[src].astype(np.int64)]
+    return (begin, np.asarray(image_frame, np.int32)[img], np.asarray(image_sensor)[img].astype(np.uint16), xy)
 
 
 def tracks_to_scene(tracks: Tracks, features: dict, image_ids, cam_intr, intr_model, intr_params):
