@@ -230,6 +230,16 @@ class RASystemProbeOut(ct.Structure):
     _fields_ = [(f, c_void_p) for f in ("res", "w", "b", "rhs", "deg", "Minv", "Ac")] + [("b_norm2", c_double)]
 
 
+class GPStepProbeOut(ct.Structure):
+    """b200sfm_test_gp_step_out (include/b200sfm_testing.h)."""
+    _fields_ = [(f, c_void_p) for f in ("M", "bw", "jscale_s", "ds", "Vinv", "gX", "Dp", "jscale_p", "dX", "U", "gc", "Dc",
+                                        "Minv", "jscale_c", "b", "px", "resid", "cand_centers", "cand_points",
+                                        "cand_scales", "cand_ucen")] + \
+              [(f, c_double) for f in ("cost", "gmax", "g_dot_delta", "model_cost_change", "cand_cost", "step_norm",
+                                       "x_norm")] + \
+              [(f, c_int32) for f in ("pcg_iterations", "schur_jacobi", "CB", "n_us", "pcg_depth")]
+
+
 # name -> (restype, argtypes); the test-only probe of include/b200sfm_testing.h (not part of the drop-in ABI)
 TEST_PROTOTYPES = {
     "b200sfm_test_ba_step": (c_int32, [c_void_p, P(BAOpts), c_double, c_double, P(BAStepProbeOut)]),
@@ -244,6 +254,8 @@ TEST_PROTOTYPES = {
     "b200sfm_test_ra_pcg": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, P(c_int32)]),
     "b200sfm_test_ra_admm_step": (c_int32, [c_void_p, c_double] + [c_void_p] * 6),
     "b200sfm_test_ra_update": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "b200sfm_test_gp_step": (c_int32, [c_void_p, P(GPOpts), c_double, c_double, c_double, P(GPStepProbeOut)]),
+    "b200sfm_test_gp_apply": (c_int32, [c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -1082,6 +1082,33 @@ int b200sfm_gp_problem_solve(b200sfm_gp_problem* p, const b200sfm_gp_opts* opts,
   }));
 }
 
+// ---- GP test probe (include/b200sfm_testing.h) -------------------------------------------------------------------
+int b200sfm_test_gp_step(b200sfm_gp_problem* p, const b200sfm_gp_opts* opts, double first_radius, double radius,
+                         double alpha, b200sfm_test_gp_step_out* out) {
+  if (!p || !opts || !out || !(radius > 0.0) || first_radius < 0.0 || !(alpha > 0.0)) return B200SFM_ERR_INVALID_ARG;
+  if (p->ctx->world > 1) { p->ctx->err = "the test probe is single-rank only"; return B200SFM_ERR_INVALID_ARG; }
+  return guarded(p->ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(p->ctx->device));
+    if (opts->min_num_view_per_track != p->min_views) {
+      p->ctx->err = "min_num_view_per_track differs from the value the problem was created with";
+      return (int)B200SFM_ERR_INVALID_ARG;
+    }
+    p->test_step(*opts, first_radius, radius, alpha, out);
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_gp_apply(b200sfm_gp_problem* p, const double* x, double* y) {
+  if (!p || !x || !y) return B200SFM_ERR_INVALID_ARG;
+  if (p->ctx->world > 1) { p->ctx->err = "the test probe is single-rank only"; return B200SFM_ERR_INVALID_ARG; }
+  if (!p->probe_ready) { p->ctx->err = "b200sfm_test_gp_apply needs a preceding b200sfm_test_gp_step"; return B200SFM_ERR_INVALID_ARG; }
+  return guarded(p->ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(p->ctx->device));
+    p->test_apply(x, y);
+    return (int)B200SFM_OK;
+  });
+}
+
 void b200sfm_gp_problem_free(b200sfm_gp_problem* p) {
   if (!p) return;
   cudaSetDevice(p->ctx->device);

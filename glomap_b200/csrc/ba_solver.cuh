@@ -123,10 +123,11 @@ __global__ void k_normalize_quat(int C, double* __restrict__ q) {
     for (int k = 0; k < 4; ++k) q[4 * c + k] *= inv;
   }
 }
-// b = -(gc + y)
-__global__ void k_rhs(int n, const double* __restrict__ gc, const double* __restrict__ y, double* __restrict__ b) {
+// b = -(gc + y); fixed (optional, one entry per block of bs): b = 0 on the blocks with fixed < 0
+__global__ void k_rhs(int n, const double* __restrict__ gc, const double* __restrict__ y, double* __restrict__ b,
+                      const double* __restrict__ fixed = nullptr, int bs = 1) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) b[i] = -(gc[i] + (y ? y[i] : 0.0));
+  if (i < n) b[i] = (fixed && fixed[i / bs] < 0.0) ? 0.0 : -(gc[i] + (y ? y[i] : 0.0));
 }
 
 }  // namespace b200

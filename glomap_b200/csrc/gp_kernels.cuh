@@ -22,6 +22,8 @@
 namespace b200 {
 
 constexpr int kMDoubles = 6;
+// per-block record summed by the linearisation: U (6) | gc (3) | sum w s^2 (1) | Schur-Jacobi term (6) | raw gradient (3)
+constexpr int kOutW = 19;
 constexpr int kMBytes = 48;
 constexpr double kScaleLowerBound = 1e-5;   // global_positioning.cc:373
 
@@ -57,6 +59,7 @@ struct GPView {
   double* gX;                     // [P][3]
   double* Dp;                     // [P]
   double* jscale_p;               // [P]
+  double* graw;                   // [N][3] raw camera-side gradient w s r, before the scale is eliminated
 };
 
 __device__ __forceinline__ double lm_damp(double diag, double js, double radius) {
@@ -131,12 +134,13 @@ __global__ void gp_dyn_offsets(long long N, const int* __restrict__ obs_cam, con
 }
 
 // Blocks of the unknown sensors (dr/du_s = s R_rw^T = (dr/dc) R_rw^T):
-//   out16[C + su][0..5] += R M_o R^T, [6..8] += R b_o, [9] += w s^2      (one thread per observation, CTA-level sums)
+//   out[C + su][0..5] += R M_o R^T, [6..8] += R b_o, [9] += w s^2, [16..18] += R g_raw  (one thread per observation,
+//   CTA-level sums)
 __global__ void __launch_bounds__(256) gp_linearize_sensors(GPView v, double* __restrict__ out16) {
   __shared__ double scratch[32];
   const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   int su = -1;
-  double val[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  double val[13] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   if (o < v.N) {
     su = v.obs_us[o];
     const int pt = v.obs_pt[o];
@@ -159,13 +163,16 @@ __global__ void __launch_bounds__(256) gp_linearize_sensors(GPView v, double* __
 #pragma unroll
       for (int r = 0; r < 3; ++r) val[6 + r] = R[3 * r] * bw.x + R[3 * r + 1] * bw.y + R[3 * r + 2] * bw.z;
       val[9] = bw.w;
+      const double* g = v.graw + 3 * (size_t)o;
+#pragma unroll
+      for (int r = 0; r < 3; ++r) val[10 + r] = R[3 * r] * g[0] + R[3 * r + 1] * g[1] + R[3 * r + 2] * g[2];
     }
   }
   for (int s2 = 0; s2 < v.n_us; ++s2) {
 #pragma unroll
-    for (int k = 0; k < 10; ++k) {
+    for (int k = 0; k < 13; ++k) {
       const double t = block_sum(su == s2 ? val[k] : 0.0, scratch);
-      if (threadIdx.x == 0 && t != 0.0) atomicAdd(&out16[(size_t)(v.C + s2) * 16 + k], t);
+      if (threadIdx.x == 0 && t != 0.0) atomicAdd(&out16[(size_t)(v.C + s2) * kOutW + (k < 10 ? k : k + 6)], t);
     }
   }
 }
@@ -183,12 +190,13 @@ __global__ void gp_build_records(int C, const double* __restrict__ centers, cons
 
 // ---------------------------------------------------------------------------
 // G1: per-observation linearisation with the scale eliminated, per-point
-// blocks (damped, inverted).  scal[0] += cost, scal[1] = max|gX|
+// blocks (damped, inverted).  scal[0] += cost, scal[1] = max of the raw gradient over the variable points and the
+// projected raw gradient over the variable scales (the camera blocks add theirs in gp_finalize_cams)
 // ---------------------------------------------------------------------------
 struct G1Smem {
   alignas(128) double Mt[kTile * kMDoubles];
-  double red[10][kTile + 1];
-  double acc[10][kTilePts + 1];
+  double red[13][kTile + 1];
+  double acc[13][kTilePts + 1];
   unsigned pb[kTilePts + 1];
   double X[3][kTilePts + 1];
   double scratch[32];
@@ -213,10 +221,10 @@ __global__ void __launch_bounds__(kTile) gp_linearize_points(GPView v, const dou
 #pragma unroll
     for (int k = 0; k < 3; ++k) sm.X[k][tid] = points[3 * (size_t)(p0 + tid) + k];
 #pragma unroll
-    for (int k = 0; k < 10; ++k) sm.acc[k][tid] = 0.0;
+    for (int k = 0; k < 13; ++k) sm.acc[k][tid] = 0.0;
   }
   __syncthreads();
-  double cost = 0.0;
+  double cost = 0.0, gmax = 0.0;
   for (int c0 = 0; c0 < n; c0 += kTile) {
     const int nc = min(kTile, n - c0);
     GPObs o;
@@ -243,14 +251,28 @@ __global__ void __launch_bounds__(kTile) gp_linearize_points(GPView v, const dou
         cost += 0.5 * o.rho0;
         double4* bwp = reinterpret_cast<double4*>(v.bw + 4 * oi);
         *bwp = make_double4(o.b[0], o.b[1], o.b[2], o.ws2);
+        // raw gradient (Ceres' g = J^T r of the unreduced program): w s r for the centre, -w s r for the point and
+        // -w d.r for the scale, whose bound the norm projects on: |Project(s - g_s) - s|
+        const double ws = o.w * s;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          o.r[k] *= ws;
+          v.graw[3 * oi + k] = o.r[k];
+        }
+        if (svar) gmax = fmax(gmax, fabs(fmax(s + o.w * o.dr, kScaleLowerBound) - s));
       }
     }
     if (!use) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) o.M[k] = 0.0;
       o.b[0] = o.b[1] = o.b[2] = 0.0;
+      o.r[0] = o.r[1] = o.r[2] = 0.0;
       o.ws2 = 0.0;
-      if (tid < nc) *reinterpret_cast<double4*>(v.bw + 4 * ((size_t)o0 + c0 + tid)) = make_double4(0, 0, 0, 0);
+      if (tid < nc) {
+        const size_t oi = (size_t)o0 + c0 + tid;
+        *reinterpret_cast<double4*>(v.bw + 4 * oi) = make_double4(0, 0, 0, 0);
+        v.graw[3 * oi] = v.graw[3 * oi + 1] = v.graw[3 * oi + 2] = 0.0;
+      }
     }
     double* mrow = sm.Mt + tid * kMDoubles;
 #pragma unroll
@@ -262,14 +284,17 @@ __global__ void __launch_bounds__(kTile) gp_linearize_points(GPView v, const dou
     sm.red[7][tid] = -o.b[1];
     sm.red[8][tid] = -o.b[2];
     sm.red[9][tid] = o.ws2;
+    sm.red[10][tid] = -o.r[0];
+    sm.red[11][tid] = -o.r[1];
+    sm.red[12][tid] = -o.r[2];
     fence_proxy_async_smem();
     __syncthreads();
     if (tid == 0) {
       tma_store_1d(v.M + ((size_t)o0 + c0) * kMDoubles, sm.Mt, (uint32_t)nc * kMBytes);
       tma_store_commit();
     }
-    for (int item = tid; item < npts * 10; item += kTile) {
-      const int j = item / 10, k = item - 10 * j;
+    for (int item = tid; item < npts * 13; item += kTile) {
+      const int j = item / 13, k = item - 13 * j;
       const int lo = max((int)sm.pb[j] - (int)(o0 + c0), 0), hi = min((int)sm.pb[j + 1] - (int)(o0 + c0), nc);
       double a = 0.0;
       for (int i = lo; i < hi; ++i) a += sm.red[k][i];
@@ -278,7 +303,6 @@ __global__ void __launch_bounds__(kTile) gp_linearize_points(GPView v, const dou
     if (tid == 0) tma_store_wait_read();
     __syncthreads();
   }
-  double gmax = 0.0;
   if (tid < npts) {
     const size_t p = (size_t)(p0 + tid);
     const bool pvalid = (int)(sm.pb[tid + 1] - sm.pb[tid]) >= v.min_views;
@@ -298,7 +322,7 @@ __global__ void __launch_bounds__(kTile) gp_linearize_points(GPView v, const dou
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
         g[k] = sm.acc[6 + k][tid];
-        gmax = fmax(gmax, fabs(g[k]));
+        gmax = fmax(gmax, fabs(sm.acc[10 + k][tid]));
       }
     }
 #pragma unroll
@@ -316,7 +340,7 @@ __global__ void __launch_bounds__(kTile) gp_linearize_points(GPView v, const dou
 // ---------------------------------------------------------------------------
 // G2: camera blocks (camera order, one warp per segment):
 //   out[cam][0..5] += U = sum M_o, [6..8] += gc = sum b_o, [9] += sum w s^2,
-//   [10..15] += Sd = sum M_o Vinv_p M_o
+//   [10..15] += Sd = sum M_o Vinv_p M_o, [16..18] += the raw gradient sum w s r
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(128) gp_linearize_cams(GPView v, int with_schur, double* __restrict__ out16) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -324,9 +348,9 @@ __global__ void __launch_bounds__(128) gp_linearize_cams(GPView v, int with_schu
   if (warp >= v.n_segs) return;
   const int cam = v.seg_cam[warp];
   const int b = v.seg_begin[warp], e = v.seg_end[warp];
-  double acc[16];
+  double acc[kOutW];
 #pragma unroll
-  for (int k = 0; k < 16; ++k) acc[k] = 0.0;
+  for (int k = 0; k < kOutW; ++k) acc[k] = 0.0;
   for (int i = b + lane; i < e; i += 32) {
     const size_t o = (size_t)v.camord_obs[i];
     const double2* mp = reinterpret_cast<const double2*>(v.M + o * kMDoubles);
@@ -339,6 +363,9 @@ __global__ void __launch_bounds__(128) gp_linearize_cams(GPView v, int with_schu
     acc[7] += bw.y;
     acc[8] += bw.z;
     acc[9] += bw.w;
+    acc[16] += v.graw[3 * o];
+    acc[17] += v.graw[3 * o + 1];
+    acc[18] += v.graw[3 * o + 2];
     if (with_schur) {
       const int pt = v.pt_c[i];
       const double2* vp = reinterpret_cast<const double2*>(v.Vinv + (size_t)pt * 6);
@@ -357,9 +384,9 @@ __global__ void __launch_bounds__(128) gp_linearize_cams(GPView v, int with_schu
     }
   }
 #pragma unroll
-  for (int k = 0; k < 16; ++k) {
+  for (int k = 0; k < kOutW; ++k) {
     const double s = warp_sum(acc[k]);
-    if (lane == k && s != 0.0) atomicAdd(&out16[(size_t)cam * 16 + k], s);
+    if (lane == k && s != 0.0) atomicAdd(&out16[(size_t)cam * kOutW + k], s);
   }
 }
 
@@ -373,7 +400,7 @@ __global__ void gp_finalize_cams(int C, const double* __restrict__ out16, const 
   double gmax = 0.0;
   if (blockIdx.x == 0 && threadIdx.x < nslots) gmax = gslots[threadIdx.x];   // per-rank max|g_X| slots (sum all-reduced)
   if (c < C) {
-    const double* o = out16 + (size_t)c * 16;
+    const double* o = out16 + (size_t)c * kOutW;
     const double diag = o[9];
     const bool fixed = (cam_const && cam_const[c]) || !(diag > 0.0);
     double u[6], g[3], D = 0.0;
@@ -388,7 +415,7 @@ __global__ void gp_finalize_cams(int C, const double* __restrict__ out16, const 
 #pragma unroll
       for (int k = 0; k < 3; ++k) {
         g[k] = o[6 + k];
-        gmax = fmax(gmax, fabs(g[k]));
+        gmax = fmax(gmax, fabs(o[16 + k]));
       }
       double js = set_js ? 1.0 / (1.0 + sqrt(diag)) : jscale_c[c];
       if (set_js) jscale_c[c] = js;
@@ -659,13 +686,14 @@ __global__ void __launch_bounds__(kTile) gp_schur_pass(GPView v, const double* _
 // ---------------------------------------------------------------------------
 // candidate = Project(x + alpha delta)  (Ceres ParameterBlock::Plus projects on
 // the bounds); norms for the parameter tolerance.
-//   nscal[0] += |x_new - x|^2, nscal[1] += |x|^2  over variable blocks
+//   nscal[0] += |x_new - x|^2, nscal[1] += |x|^2  over variable blocks (Ceres' reduced program: constant points and
+//   scales, and centres with jscale_c < 0, are not in it)
 // ---------------------------------------------------------------------------
 __global__ void gp_apply_step(GPView v, double alpha, const double* __restrict__ centers,
                               const double* __restrict__ points, const double* __restrict__ scales,
                               const double* __restrict__ dc, const double* __restrict__ dX,
                               const double* __restrict__ ds, const double* __restrict__ jscale_c, int count_cams,
-                              double* __restrict__ centers_new, double* __restrict__ points_new,
+                              int points_var, double* __restrict__ centers_new, double* __restrict__ points_new,
                               double* __restrict__ scales_new, double* __restrict__ nscal,
                               const double* __restrict__ ucen, double* __restrict__ ucen_new) {
   __shared__ double scratch[32];
@@ -688,7 +716,7 @@ __global__ void gp_apply_step(GPView v, double alpha, const double* __restrict__
     const double d = alpha * dX[i];
     points_new[i] = xo + d;
     const int pt = (int)(i / 3);
-    if ((int)(v.pt_begin[pt + 1] - v.pt_begin[pt]) >= v.min_views) {
+    if (points_var && (int)(v.pt_begin[pt + 1] - v.pt_begin[pt]) >= v.min_views) {
       a0 += d * d;
       a1 += xo * xo;
     }

@@ -31,7 +31,7 @@ struct b200sfm_gp_problem {
   int cur = 0;
   DevBuf<double> cen4;
   // linear system
-  DevBuf<double> M, bw, jscale_s, Vinv, gX, Dp, jscale_p, out16, U, gc, Dc, Minv, jscale_c;
+  DevBuf<double> M, bw, graw, jscale_s, Vinv, gX, Dp, jscale_p, out16, U, gc, Dc, Minv, jscale_c;
   DevBuf<double> px, pr, pz, pp, pq, yw, bvec, dX, ds, scal;
   b200::EventTimer timer_lin, timer_mv;
   size_t smem_g1 = 0, smem_g3 = 0;
@@ -47,6 +47,7 @@ struct b200sfm_gp_problem {
     v.tile_pt_begin = tile_pt_begin.p; v.camord_obs = camord_obs.p; v.pt_c = pt_c.p;
     v.seg_cam = seg_cam.p; v.seg_begin = seg_begin.p; v.seg_end = seg_end.p;
     v.M = M.p; v.bw = bw.p; v.jscale_s = jscale_s.p; v.Vinv = Vinv.p; v.gX = gX.p; v.Dp = Dp.p; v.jscale_p = jscale_p.p;
+    v.graw = graw.p;
     return v;
   }
 
@@ -89,7 +90,7 @@ struct b200sfm_gp_problem {
   // per-block arrays of the reduced system (CB blocks of 3)
   void alloc_blocks() {
     cudaStream_t s = ctx->stream;
-    out16.alloc((size_t)CB * 16 + 1 + (size_t)ctx->world);   // per block 16 | cost | one max|g_X| slot per rank
+    out16.alloc((size_t)CB * b200::kOutW + 1 + (size_t)ctx->world);   // per block kOutW | cost | one max|g| slot per rank
     U.alloc((size_t)CB * 6); gc.alloc((size_t)CB * 3); Dc.alloc((size_t)CB * 3);
     Minv.alloc((size_t)CB * 6); jscale_c.alloc(CB);
     px.alloc((size_t)CB * 3); pr.alloc((size_t)CB * 3); pz.alloc((size_t)CB * 3); pp.alloc((size_t)CB * 3);
@@ -181,7 +182,7 @@ struct b200sfm_gp_problem {
       centers[i].alloc((size_t)C * 3); points[i].alloc((size_t)P * 3); scales[i].alloc(N);
     }
     cen4.alloc((size_t)C * 4);
-    M.alloc((size_t)N * kMDoubles); bw.alloc((size_t)N * 4); jscale_s.alloc(N);
+    M.alloc((size_t)N * kMDoubles); bw.alloc((size_t)N * 4); graw.alloc((size_t)N * 3); jscale_s.alloc(N);
     Vinv.alloc((size_t)P * 6); gX.alloc((size_t)P * 3); Dp.alloc(P); jscale_p.alloc(P);
     CB = C;
     alloc_blocks();
@@ -279,12 +280,12 @@ struct b200sfm_gp_problem {
       B200_LAUNCH(ctx, gp_linearize_cams, cdiv((long long)n_segs * 32, 128), 128, 0, v, schur_jacobi ? 1 : 0, out16.p);
     if (n_us > 0) B200_LAUNCH(ctx, gp_linearize_sensors, cdiv(N, 256), 256, 0, v, out16.p);
     // cost and this rank's max|g_X| (own slot) travel with the camera blocks through ONE sum all-reduce
-    B200_CUDA_OK(cudaMemcpyAsync(out16.p + (size_t)CB * 16, scal.p, sizeof(double), cudaMemcpyDeviceToDevice, s));
-    B200_CUDA_OK(cudaMemcpyAsync(out16.p + (size_t)CB * 16 + 1 + ctx->rank, scal.p + 1, sizeof(double), cudaMemcpyDeviceToDevice, s));
-    ctx->allreduce_sum(out16.p, (size_t)CB * 16 + 1 + (size_t)ctx->world);
+    B200_CUDA_OK(cudaMemcpyAsync(out16.p + (size_t)CB * b200::kOutW, scal.p, sizeof(double), cudaMemcpyDeviceToDevice, s));
+    B200_CUDA_OK(cudaMemcpyAsync(out16.p + (size_t)CB * b200::kOutW + 1 + ctx->rank, scal.p + 1, sizeof(double), cudaMemcpyDeviceToDevice, s));
+    ctx->allreduce_sum(out16.p, (size_t)CB * b200::kOutW + 1 + (size_t)ctx->world);
     B200_CUDA_OK(cudaMemsetAsync(scal.p + 1, 0, sizeof(double), s));
     B200_LAUNCH(ctx, gp_finalize_cams, cdiv(CB, 128), 128, 0, CB, out16.p, cam_const.p, jscale_c.p, first ? 1 : 0, radius,
-                schur_jacobi ? 1 : 0, U.p, gc.p, Dc.p, Minv.p, scal.p, out16.p + (size_t)CB * 16 + 1, ctx->world);
+                schur_jacobi ? 1 : 0, U.p, gc.p, Dc.p, Minv.p, scal.p, out16.p + (size_t)CB * b200::kOutW + 1, ctx->world);
     // rhs  (constant points have Vinv = 0 from G1, so the same passes apply)
     {
       yw.zero(s);
@@ -292,7 +293,9 @@ struct b200sfm_gp_problem {
                   nullptr, nullptr, nullptr);
       ctx->allreduce_sum(yw.p, nC3);
     }
-    B200_LAUNCH(ctx, k_rhs, cdiv(nC3, 256), 256, 0, nC3, gc.p, yw.p, bvec.p);
+    // constant blocks (jscale_c < 0) are identity rows with b = 0, here and in pcg_apply_diag: PCG leaves their dc at 0,
+    // so the back-substitution and the step scalars see the reduced program without them
+    B200_LAUNCH(ctx, k_rhs, cdiv(nC3, 256), 256, 0, nC3, gc.p, yw.p, bvec.p, jscale_c.p, 3);
     // PCG (3x3 blocks; loop control on the device, pcg.cuh)
     const int max_it = std::max(1, o.pcg_max_iterations);
     const int nblk = cdiv(CB, kPcgThreads);
@@ -308,27 +311,13 @@ struct b200sfm_gp_problem {
           double* d_pub = ctx->pcgh.dots(it - 1);
           B200_LAUNCH(ctx, pcg_direction<3>, nblk, kPcgThreads, 0, CB, nblk, it, o.pcg_min_iterations, o.pcg_rel_tolerance, pz.p,
                       pp.p, yw.p, ctx->pcgh.dots(it - 2), part_rz, part_rr, nullptr, d_pub, ctl);
-          cudaEvent_t m0 = nullptr, m1 = nullptr;
-          if (profile) {
-            m0 = timer_mv.next(); m1 = timer_mv.next();
-            B200_CUDA_OK(cudaEventRecord(m0, s));
-          }
-          if (ctx->pcgh.depth > 1)   // iterations are queued ahead of the read-back: the pass tests the stopping flag
-            B200_LAUNCH(ctx, (gp_schur_pass<0, true>), n_tiles, kTile, smem_g3, v, pp.p, yw.p, nullptr, nullptr, nullptr, 0.0, radius,
-                        nullptr, nullptr, nullptr, ctl);
-          else
-            B200_LAUNCH(ctx, gp_schur_pass<0>, n_tiles, kTile, smem_g3, v, pp.p, yw.p, nullptr, nullptr, nullptr, 0.0, radius,
-                        nullptr, nullptr, nullptr, nullptr);
-          if (profile) B200_CUDA_OK(cudaEventRecord(m1, s));
-          ctx->allreduce_sum(yw.p, nC3);
-          // unknown sensors: the pass already applied the direct term per observation (A = nullptr)
-          B200_LAUNCH(ctx, pcg_apply_diag<3>, nblk, kPcgThreads, 0, CB, n_us > 0 ? nullptr : U.p, Dc.p, pp.p, yw.p, pq.p, part_pq, ctl);
+          matvec(v, pp.p, yw.p, part_pq, ctl, profile);
           B200_LAUNCH(ctx, pcg_update<3>, nblk, kPcgThreads, 0, CB, nblk, Minv.p, pp.p, pq.p, px.p, pr.p, pz.p, d_pub, part_pq,
                       part_rz, part_rr, ctx->pcgh.dots(it), ctl);
         },
         [&](int launched) { B200_LAUNCH(ctx, pcg_finalize, 1, kPcgThreads, 0, nblk, launched, part_rr, ctl); });
     if (profile) timer_mv.used = mv_ev0 + 2 * (size_t)std::min(pr_.iters, pr_.launched);
-    B200_CUDA_OK(cudaMemcpyAsync(ctx->h_scal + 8, out16.p + (size_t)CB * 16, sizeof(double), cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaMemcpyAsync(ctx->h_scal + 8, out16.p + (size_t)CB * b200::kOutW, sizeof(double), cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaMemcpyAsync(ctx->h_scal + 9, scal.p + 1, sizeof(double), cudaMemcpyDeviceToHost, s));
     B200_CUDA_OK(cudaStreamSynchronize(s));
     res.cost = ctx->h_scal[8];
@@ -354,15 +343,40 @@ struct b200sfm_gp_problem {
     return res;
   }
 
+  // q = (S + D) p through the kernels of one PCG iteration: the implicit Schur pass (the SPEC variant when iterations
+  // are queued ahead of the read-back), the all-reduce, then the block diagonal.  y must be zero on entry; the pass
+  // accumulates into it.  Constant blocks (jscale_c < 0) are identity rows.
+  void matvec(const GPView& v, const double* p, double* y, double* part_pq, const b200::PcgCtl* ctl, bool profile) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    cudaEvent_t m0 = nullptr, m1 = nullptr;
+    if (profile) {
+      m0 = timer_mv.next(); m1 = timer_mv.next();
+      B200_CUDA_OK(cudaEventRecord(m0, s));
+    }
+    if (ctx->pcgh.depth > 1)   // iterations are queued ahead of the read-back: the pass tests the stopping flag
+      B200_LAUNCH(ctx, (gp_schur_pass<0, true>), n_tiles, kTile, smem_g3, v, p, y, nullptr, nullptr, nullptr, 0.0, 0.0,
+                  nullptr, nullptr, nullptr, ctl);
+    else
+      B200_LAUNCH(ctx, gp_schur_pass<0>, n_tiles, kTile, smem_g3, v, p, y, nullptr, nullptr, nullptr, 0.0, 0.0,
+                  nullptr, nullptr, nullptr, nullptr);
+    if (profile) B200_CUDA_OK(cudaEventRecord(m1, s));
+    ctx->allreduce_sum(y, (size_t)CB * 3);
+    // unknown sensors: the pass already applied the direct term per observation (A = nullptr)
+    B200_LAUNCH(ctx, pcg_apply_diag<3>, cdiv(CB, kPcgThreads), kPcgThreads, 0, CB, n_us > 0 ? nullptr : U.p, Dc.p, p, y, pq.p,
+                part_pq, ctl, jscale_c.p);
+  }
+
   // candidate = Project(x + alpha delta) into the other buffer; returns (cost, step_norm, x_norm)
-  void make_candidate(const GPView& v, double alpha, double huber_a, double& cand_cost, double& step_norm, double& x_norm) {
+  void make_candidate(const GPView& v, double alpha, double huber_a, bool points_var, double& cand_cost, double& step_norm,
+                      double& x_norm) {
     using namespace b200;
     cudaStream_t s = ctx->stream;
     const int nxt = cur ^ 1;
     B200_CUDA_OK(cudaMemsetAsync(scal.p + 12, 0, 2 * sizeof(double), s));
     const long long nthreads = std::max<long long>(N, std::max<long long>((long long)P * 3, (long long)CB * 3));
     B200_LAUNCH(ctx, gp_apply_step, cdiv(nthreads, 256), 256, 0, v, alpha, centers[cur].p, points[cur].p, scales[cur].p, px.p,
-                dX.p, ds.p, jscale_c.p, ctx->rank == 0 ? 1 : 0, centers[nxt].p, points[nxt].p, scales[nxt].p, scal.p + 12,
+                dX.p, ds.p, jscale_c.p, ctx->rank == 0 ? 1 : 0, points_var ? 1 : 0, centers[nxt].p, points[nxt].p, scales[nxt].p, scal.p + 12,
                 n_us > 0 ? ucen[cur].p : nullptr, n_us > 0 ? ucen[nxt].p : nullptr);
     cand_cost = eval_cost(nxt, v, huber_a);
     // points/scales norms are per-shard, camera norms replicated: reduce the former only approximately matters
@@ -415,7 +429,7 @@ struct b200sfm_gp_problem {
       }
       invalid = 0;
       double alpha = 1.0, cand = 0, step_norm = 0, x_norm = 0;
-      make_candidate(v, alpha, o.thres_loss_function, cand, step_norm, x_norm);
+      make_candidate(v, alpha, o.thres_loss_function, points_var, cand, step_norm, x_norm);
       if (scales_var && o.max_num_line_search_step_size_iterations > 0) {
         // projected Armijo line search (trust_region_minimizer.cc DoLineSearch; oracle/ceres_lm.py)
         const double g0 = r.g_dot_delta;
@@ -461,10 +475,10 @@ struct b200sfm_gp_problem {
           }
           a = std::min(std::max(an, lo), hi);
           if (a < 1e-12) break;
-          make_candidate(v, a, o.thres_loss_function, fa, step_norm, x_norm);
+          make_candidate(v, a, o.thres_loss_function, points_var, fa, step_norm, x_norm);
         }
         if (ok) { alpha = a; cand = fa; }
-        else if (a != 1.0) make_candidate(v, 1.0, o.thres_loss_function, cand, step_norm, x_norm);
+        else if (a != 1.0) make_candidate(v, 1.0, o.thres_loss_function, points_var, cand, step_norm, x_norm);
       }
       if (!fixed) {
         if (step_norm <= o.parameter_tolerance * (x_norm + o.parameter_tolerance)) { term = B200SFM_TERM_PARAMETER_TOLERANCE; break; }
@@ -507,5 +521,74 @@ struct b200sfm_gp_problem {
     local.kernel_launches = ctx->launches - launches0;
     if (st) *st = local;
     return B200SFM_OK;
+  }
+
+  // ---- test probe (include/b200sfm_testing.h) ----------------------------------------------------------------------
+  bool probe_ready = false;
+  bool probe_scales_var = true;
+
+  // the first LM iteration of solve() up to the candidate and its cost, without accepting it; with first_radius > 0 the
+  // step at `radius` is the second one and reuses the Jacobi scales of the step at first_radius
+  void test_step(const b200sfm_gp_opts& o, double first_radius, double radius, double alpha, b200sfm_test_gp_step_out* out) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    const bool points_var = o.optimize_points != 0;
+    probe_scales_var = o.optimize_scales != 0;
+    B200_LAUNCH(ctx, k_eff_mask, cdiv(C, 256), 256, 0, C, cam_const_base.p, o.optimize_positions ? 0 : 1, 0, cam_const.p);
+    GPView v = view(probe_scales_var);
+    if (first_radius > 0.0) compute_step(o, v, first_radius, true, points_var, false);
+    const StepResult r = compute_step(o, v, radius, !(first_radius > 0.0), points_var, false);
+    double cand = 0, step_norm = 0, x_norm = 0;
+    make_candidate(v, alpha, o.thres_loss_function, points_var, cand, step_norm, x_norm);
+    probe_ready = true;
+    const int nxt = cur ^ 1;
+    const size_t nb3 = (size_t)CB * 3;
+    if (out->M) M.download(out->M, (size_t)N * 6, s);
+    if (out->bw) bw.download(out->bw, (size_t)N * 4, s);
+    if (out->jscale_s) jscale_s.download(out->jscale_s, N, s);
+    if (out->ds) ds.download(out->ds, N, s);
+    if (out->Vinv) Vinv.download(out->Vinv, (size_t)P * 6, s);
+    if (out->gX) gX.download(out->gX, (size_t)P * 3, s);
+    if (out->Dp) Dp.download(out->Dp, P, s);
+    if (out->jscale_p) jscale_p.download(out->jscale_p, P, s);
+    if (out->dX) dX.download(out->dX, (size_t)P * 3, s);
+    if (out->U) U.download(out->U, (size_t)CB * 6, s);
+    if (out->gc) gc.download(out->gc, nb3, s);
+    if (out->Dc) Dc.download(out->Dc, nb3, s);
+    if (out->Minv) Minv.download(out->Minv, (size_t)CB * 6, s);
+    if (out->jscale_c) jscale_c.download(out->jscale_c, CB, s);
+    if (out->b) bvec.download(out->b, nb3, s);
+    if (out->px) px.download(out->px, nb3, s);
+    if (out->resid) pr.download(out->resid, nb3, s);
+    if (out->cand_centers) centers[nxt].download(out->cand_centers, (size_t)C * 3, s);
+    if (out->cand_points) points[nxt].download(out->cand_points, (size_t)P * 3, s);
+    if (out->cand_scales) scales[nxt].download(out->cand_scales, N, s);
+    if (n_us > 0 && out->cand_ucen) ucen[nxt].download(out->cand_ucen, (size_t)n_us * 3, s);
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    out->cost = r.cost;
+    out->gmax = r.gmax;
+    out->g_dot_delta = r.g_dot_delta;
+    out->model_cost_change = r.model_cost_change;
+    out->cand_cost = cand;
+    out->step_norm = step_norm;
+    out->x_norm = x_norm;
+    out->pcg_iterations = r.pcg_iters;
+    out->schur_jacobi = (points_var && o.preconditioner == 1 && n_us == 0) ? 1 : 0;
+    out->CB = CB;
+    out->n_us = n_us;
+    out->pcg_depth = ctx->pcgh.depth;
+  }
+
+  // y = (S + D) x at the linearisation and damping of the last test_step, through matvec()
+  void test_apply(const double* h_x, double* h_y) {
+    using namespace b200;
+    cudaStream_t s = ctx->stream;
+    PcgCtl* ctl = ctx->pcgh.d_ctl;
+    B200_CUDA_OK(cudaMemsetAsync(ctl, 0, sizeof(PcgCtl), s));   // every kernel of the chain returns early once ctl->done is set
+    pp.upload(h_x, (size_t)CB * 3, s);
+    yw.zero(s);
+    matvec(view(probe_scales_var), pp.p, yw.p, ctx->pcgh.d_part, ctl, false);
+    pq.download(h_y, (size_t)CB * 3, s);
+    B200_CUDA_OK(cudaStreamSynchronize(s));
   }
 };

@@ -58,19 +58,28 @@ __device__ __forceinline__ void write_partial(double v, double* __restrict__ par
 }
 
 // q_c = (A_c + diag(D_c)) p_c + yw_c ; part_pq[blk] = partial p.q
+//   fixed (optional, one entry per block): blocks with fixed[c] < 0 are identity rows, q_c = p_c, whatever yw holds
 template <int B>
 __global__ void __launch_bounds__(kPcgThreads) pcg_apply_diag(int nb, const double* __restrict__ A,
                                                               const double* __restrict__ D,
                                                               const double* __restrict__ p,
                                                               const double* __restrict__ yw, double* __restrict__ q,
                                                               double* __restrict__ part_pq,
-                                                              const PcgCtl* __restrict__ ctl) {
+                                                              const PcgCtl* __restrict__ ctl,
+                                                              const double* __restrict__ fixed = nullptr) {
   constexpr int NP = B * (B + 1) / 2;
   __shared__ double scratch[32];
   if (ctl->done) return;
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   double pq = 0.0;
-  if (c < nb) {
+  if (c < nb && fixed && fixed[c] < 0.0) {
+#pragma unroll
+    for (int k = 0; k < B; ++k) {
+      const double pv = p[(size_t)c * B + k];
+      q[(size_t)c * B + k] = pv;
+      pq += pv * pv;
+    }
+  } else if (c < nb) {
     double a[NP], pv[B], out[B];
 #pragma unroll
     for (int k = 0; k < NP; ++k) a[k] = A ? A[(size_t)c * NP + k] : 0.0;   // A == nullptr: the mat-vec already holds A p

@@ -1,4 +1,5 @@
-/* b200sfm_testing.h -- test-only probes into resident bundle-adjustment and rotation-averaging problems.
+/* b200sfm_testing.h -- test-only probes into resident bundle-adjustment, rotation-averaging and global-positioning
+ * problems.
  *
  * NOT part of the drop-in ABI of b200sfm.h: these entry points exist so that the
  * test suite can compare every quantity one Levenberg-Marquardt step forms on the
@@ -139,6 +140,60 @@ int b200sfm_test_ra_admm_step(b200sfm_test_ra_problem* problem, double rho, cons
 /* theta <- theta (+) step, the frames' update and the unknown cameras' quaternion average, as a solve applies a step.
  * step, theta_out [3n]; sums [3] = average frame step, |step|, NaN flag. */
 int b200sfm_test_ra_update(b200sfm_test_ra_problem* problem, const double* step, double* theta_out, double* sums);
+
+/* ---- global positioning ----------------------------------------------------------------------------------------
+ * A resident global-positioning problem (b200sfm_gp_problem_create, _set_rig_terms, _set_rig_unknown, _set_state).
+ * Block vectors hold CB = C + S_u blocks of 3 doubles: the C frame centres, then the S_u unknown cam_from_rig centres.
+ * Symmetric 3x3 blocks are packed as 6 doubles, upper triangle, row by row.  Observation arrays are in the problem's
+ * observation order, short tracks included (zero rows). */
+
+/* Outputs of b200sfm_test_gp_step.  Every array pointer is caller-owned and may be NULL (not downloaded).
+ * Sizes: M [N*6]; bw [N*4]; jscale_s, ds, cand_scales [N]; Vinv [P*6]; gX, dX, cand_points [P*3]; Dp, jscale_p [P];
+ * U, Minv [CB*6]; gc, Dc, b, px, resid [CB*3]; jscale_c [CB]; cand_centers [C*3]; cand_ucen [S_u*3]. */
+typedef struct {
+  double* M;            /* per observation: the 3x3 block with the scale eliminated, w s^2 (I - w d d^T / h) */
+  double* bw;           /* per observation: (b_o, w s^2), b_o = w s (r - (w / h) d (d.r)) */
+  double* jscale_s;     /* Jacobi scale of each variable scale (0 on constant scales) */
+  double* ds;           /* scale step from the back-substitution */
+  double* Vinv;         /* per point: (V + D_p I)^-1 (0 on constant points) */
+  double* gX;           /* per point: -sum b_o */
+  double* Dp;           /* point damping */
+  double* jscale_p;     /* point Jacobi scales (variable points only) */
+  double* dX;           /* point step from the back-substitution */
+  double* U;            /* per block: sum M_o (R M_o R^T for an unknown sensor); identity on constant blocks */
+  double* gc;           /* per block: sum b_o (R b_o); 0 on constant blocks */
+  double* Dc;           /* block damping */
+  double* Minv;         /* preconditioner blocks */
+  double* jscale_c;     /* block Jacobi scales; -1 marks a constant block */
+  double* b;            /* right-hand side of the reduced system */
+  double* px;           /* the PCG iterate: the block step */
+  double* resid;        /* the PCG residual b - (S + D) px */
+  double* cand_centers; /* candidate state Project(x + alpha delta) (not accepted) */
+  double* cand_points;
+  double* cand_scales;
+  double* cand_ucen;
+  double cost;          /* robust cost at the current state */
+  double gmax;          /* max |g| for the gradient tolerance */
+  double g_dot_delta;   /* g . delta over the full step */
+  double model_cost_change;
+  double cand_cost;     /* robust cost of the candidate */
+  double step_norm;     /* |candidate - x| over the variable blocks */
+  double x_norm;        /* |x| over the variable blocks */
+  int32_t pcg_iterations;
+  /* the paths the step took */
+  int32_t schur_jacobi, CB, n_us, pcg_depth;
+} b200sfm_test_gp_step_out;
+
+/* At the problem's current state: apply the option masks as b200sfm_gp_problem_solve does, linearise as its first LM
+ * iteration and solve one step at `radius` with the PCG settings of `opts`, then form the candidate at step length
+ * `alpha` without accepting it, and download into `out`.  With first_radius > 0 a step at first_radius comes first; the
+ * step at `radius` then reuses its Jacobi scales, as every step of a solve after the first does. */
+int b200sfm_test_gp_step(b200sfm_gp_problem* problem, const b200sfm_gp_opts* opts, double first_radius, double radius,
+                         double alpha, b200sfm_test_gp_step_out* out);
+
+/* y = (S + D) x over the CB*3 block dofs with the linearisation of the last b200sfm_test_gp_step, through the kernels
+ * of one PCG iteration.  x, y: host arrays [CB*3]. */
+int b200sfm_test_gp_apply(b200sfm_gp_problem* problem, const double* x, double* y);
 
 #ifdef __cplusplus
 }

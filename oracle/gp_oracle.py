@@ -49,14 +49,16 @@ class GPOptions:
 
 class GPProblem:
     def __init__(self, centers, points, pt_obs_begin, obs_cam, obs_dir, cam_calibrated, opts: GPOptions, scales=None,
-                 obs_offset=None, rig_unknown=None):
+                 obs_offset=None, rig_unknown=None, cam_const=None, obs_calibrated=None):
         """``obs_offset`` [N,3]: known-rig term of RigBATAPairwiseDirectionError (cost_function.h:49-82) with the rig
         scale held at 1 (global_positioning.cc:493-497): r = t_obs - s (X - c_frame + t_rig), t_rig = R_cw^T t_cam_from_rig
         (.cc:339-345).
         ``rig_unknown`` = dict(obs_sensor [N] (-1: none), R_rw [N,3,3] rig_from_world rotation of the observation's frame,
         centers [S,3]): RigUnknownBATAPairwiseDirectionError (cost_function.h:90-134, global_positioning.cc:347-364) --
         the camera centre in the rig frame u_s of a sensor whose cam_from_rig is not known yet is an unknown block shared
-        by all its images:  r = t_obs - s (X - c_frame - R_rw^T u_s).  Oracle only so far (no device path)."""
+        by all its images:  r = t_obs - s (X - c_frame - R_rw^T u_s).
+        ``cam_const`` [C]: centres held constant (SetParameterBlockConstant) on top of optimize_positions.
+        ``obs_calibrated`` [N]: the prior-focal flag of the observing camera of a rig, overriding cam_calibrated."""
         self.opts = opts
         self.C, self.P = len(centers), len(points)
         lens = np.diff(pt_obs_begin)
@@ -69,7 +71,8 @@ class GPProblem:
         self.obs_off = None if obs_offset is None else np.asarray(obs_offset, dtype=np.float64)[self.keep]
         self.N = len(self.obs_pt)
         cal = np.ones(self.C, bool) if cam_calibrated is None else np.asarray(cam_calibrated).astype(bool)
-        self.loss_scale = np.where(cal[self.obs_cam], 1.0, 0.5)
+        ocal = cal[self.obs_cam] if obs_calibrated is None else np.asarray(obs_calibrated).astype(bool)[self.keep]
+        self.loss_scale = np.where(ocal, 1.0, 0.5)
         s0 = np.ones(self.N) if scales is None else np.asarray(scales, dtype=np.float64)[self.keep]
         self.x0 = dict(centers=np.array(centers, dtype=np.float64), points=np.array(points, dtype=np.float64), scales=s0)
         self.ru = None
@@ -81,6 +84,8 @@ class GPProblem:
         pt_used = np.zeros(self.P, bool); pt_used[self.obs_pt] = True
         col = 0
         self.cam_col = np.full(self.C, -1)
+        if cam_const is not None:
+            cam_used &= ~np.asarray(cam_const).astype(bool)
         if opts.optimize_positions:
             idx = np.nonzero(cam_used)[0]
             self.cam_col[idx] = 3 * np.arange(len(idx)); col = 3 * len(idx)

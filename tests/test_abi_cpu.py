@@ -130,7 +130,7 @@ def test_testing_header_symbols_are_exported_and_mirrored():
 def test_testing_header_is_plain_c99_and_its_struct_matches_ctypes(tmp_path):
     import subprocess
     structs = {"b200sfm_test_ba_step_out": _lib.BAStepProbeOut, "b200sfm_test_ra_info": _lib.RAProbeInfo,
-               "b200sfm_test_ra_system_out": _lib.RASystemProbeOut}
+               "b200sfm_test_ra_system_out": _lib.RASystemProbeOut, "b200sfm_test_gp_step_out": _lib.GPStepProbeOut}
     lines = ["#include <stdio.h>", "#include <stddef.h>", '#include "b200sfm_testing.h"', "int main(void) {"]
     for cname, cls in structs.items():
         lines.append(f'  printf("{cname} %zu\\n", sizeof({cname}));')
@@ -172,3 +172,7 @@ def test_probe_rejects_a_null_problem_without_touching_the_device():
     assert lib.b200sfm_test_ra_pcg(None, 1, None, x, None) == INVALID
     assert lib.b200sfm_test_ra_admm_step(None, 1.0, x, x, x, x, x, x) == INVALID
     assert lib.b200sfm_test_ra_update(None, x, x, x) == INVALID
+    # global positioning
+    o_gp, gp_out = _lib.GPOpts(), _lib.GPStepProbeOut()
+    assert lib.b200sfm_test_gp_step(None, ct.byref(o_gp), 0.0, 1e4, 1.0, ct.byref(gp_out)) == INVALID
+    assert lib.b200sfm_test_gp_apply(None, x, x) == INVALID
