@@ -177,6 +177,8 @@ PROTOTYPES = {
                                             + [c_double, c_void_p, P(c_int64)]),
     "b200sfm_view_graph_keep_largest_component": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, c_int64] + [c_void_p] * 4
                                                   + [P(c_int32)]),
+    "b200sfm_view_graph_update_pairs_config": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int64] + [c_void_p] * 7
+                                              + [P(c_int64)]),
     "b200sfm_tracks_free": (None, [c_void_p]),
     "b200sfm_tracks_select": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int32, c_void_p] + [c_int32] * 4
                               + [c_void_p, P(c_int64)]),

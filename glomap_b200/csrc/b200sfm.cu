@@ -16,6 +16,7 @@
 #include "track_select_kernels.cuh"
 #include "vgc_solver.cuh"
 #include "view_graph_kernels.cuh"
+#include "pair_config_kernels.cuh"
 
 namespace {
 
@@ -669,6 +670,35 @@ int b200sfm_view_graph_keep_largest_component(b200sfm_ctx* ctx, int32_t num_fram
       throw b200::InvalidInput{"pair image index outside [0, num_images) or image_frame outside [0, num_frames)"};
     B200_CUDA_OK(cudaGetLastError());
     *num_registered_images = n;
+    return (int)B200SFM_OK;
+  });
+}
+
+// ---- stage 0: UpdateImagePairsConfig -----------------------------------------------
+int b200sfm_view_graph_update_pairs_config(b200sfm_ctx* ctx, int32_t K, const int32_t* intr_model, const double* intr_params,
+                                           const uint8_t* has_prior_focal, int64_t num_pairs, const int32_t* pair_cam1,
+                                           const int32_t* pair_cam2, const uint8_t* pair_valid, const double* pair_quat_xyzw,
+                                           const double* pair_trans, int32_t* pair_config, double* pair_F, int64_t* num_promoted) {
+  if (!ctx || K < 0 || num_pairs < 0 || !num_promoted) return B200SFM_ERR_INVALID_ARG;
+  *num_promoted = 0;
+  if (num_pairs == 0) return B200SFM_OK;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if ((K > 0 && (!intr_model || !intr_params || !has_prior_focal)) || !pair_cam1 || !pair_cam2 || !pair_valid ||
+      !pair_quat_xyzw || !pair_trans || !pair_config || !pair_F)
+    return invalid("null argument");
+  if (K == 0) return invalid("pair camera index outside [0, K)");
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    long long n = 0;
+    const int r = b200::update_image_pairs_config(ctx, K, intr_model, intr_params, has_prior_focal, num_pairs, pair_cam1, pair_cam2,
+                                                  pair_valid, pair_quat_xyzw, pair_trans, pair_config, pair_F, &n);
+    if (r == 1) throw b200::InvalidInput{"pair camera index outside [0, K)"};
+    if (r == 2) {
+      ctx->err = "camera model outside 0-3 in a pair to be promoted to CALIBRATED";
+      return (int)B200SFM_ERR_UNSUPPORTED;
+    }
+    B200_CUDA_OK(cudaGetLastError());
+    *num_promoted = n;
     return (int)B200SFM_OK;
   });
 }

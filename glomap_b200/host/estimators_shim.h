@@ -1161,6 +1161,75 @@ class ViewGraphCalibrator {
 };
 
 // ---------------------------------------------------------------------------
+// ViewGraphManipulater::UpdateImagePairsConfig (processors/view_graph_manipulation.cc:178-237), the first half of stage 0
+// of GlobalMapper::Solve, on the device (b200sfm_view_graph_update_pairs_config): the cameras are flattened in sorted
+// camera-id order (model_id and params), every pair in sorted pair-id order with its validity.  The promoted pairs get
+// config CALIBRATED and F = K2^-T [t]x R K1^-1 of the cam2_from_cam1 they carry; nothing else changes.  Returns the
+// number of pairs promoted; -1 and nothing changed when a pair names an unknown image, an image an unknown camera, or the
+// device call fails (message on stderr; a promoted pair whose camera model is outside 0-3 fails it).  DecomposeRelPose,
+// the second half of stage 0, is COLMAP code and not part of the shim.
+struct ViewGraphManipulater {
+  template <class ViewGraphT, class CameraMap, class ImageMap>
+  static int64_t UpdateImagePairsConfig(ViewGraphT& view_graph, const CameraMap& cameras, const ImageMap& images) {
+    using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
+    std::map<camera_t, int32_t> cidx;
+    for (auto& [id, c] : cameras) cidx[id] = 0;
+    std::vector<int32_t> model;
+    std::vector<double> params;
+    std::vector<uint8_t> prior;
+    for (auto& [id, k] : cidx) {
+      const auto& c = cameras.at(id);
+      k = (int32_t)model.size();
+      model.push_back(static_cast<int32_t>(c.model_id));
+      double p[B200SFM_INTR_STRIDE] = {0};
+      for (size_t i = 0; i < c.params.size() && i < (size_t)B200SFM_INTR_STRIDE; ++i) p[i] = c.params[i];
+      params.insert(params.end(), p, p + B200SFM_INTR_STRIDE);
+      prior.push_back(c.has_prior_focal_length ? 1 : 0);
+    }
+    std::map<image_pair_t, Pair*> psorted;
+    for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
+    std::vector<Pair*> pairs;
+    std::vector<int32_t> cam1, cam2, config;
+    std::vector<uint8_t> valid;
+    std::vector<double> quat, trans, F;
+    for (auto& [id, pr] : psorted) {
+      auto a = images.find(pr->image_id1), b = images.find(pr->image_id2);
+      if (a == images.end() || b == images.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return -1; }
+      auto ca = cidx.find(a->second.camera_id), cb = cidx.find(b->second.camera_id);
+      if (ca == cidx.end() || cb == cidx.end()) { std::fprintf(stderr, "b200sfm: image with an unknown camera\n"); return -1; }
+      pairs.push_back(pr);
+      cam1.push_back(ca->second);
+      cam2.push_back(cb->second);
+      valid.push_back(pr->is_valid ? 1 : 0);
+      config.push_back((int32_t)pr->config);
+      const double* q = pr->cam2_from_cam1.rotation.coeffs().data();
+      quat.insert(quat.end(), q, q + 4);
+      for (int k = 0; k < 3; ++k) trans.push_back(pr->cam2_from_cam1.translation[k]);
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) F.push_back(pr->F(r, c));
+    }
+    if (pairs.empty()) return 0;
+    b200sfm_ctx* ctx = DefaultContext();
+    if (!ctx) return -1;
+    int64_t n = 0;
+    const int rc = b200sfm_view_graph_update_pairs_config(ctx, (int32_t)model.size(), model.data(), params.data(), prior.data(),
+                                                          (int64_t)pairs.size(), cam1.data(), cam2.data(), valid.data(), quat.data(),
+                                                          trans.data(), config.data(), F.data(), &n);
+    if (rc != B200SFM_OK) {
+      std::fprintf(stderr, "b200sfm: UpdateImagePairsConfig failed: %s\n", b200sfm_last_error(ctx));
+      return -1;
+    }
+    for (size_t e = 0; e < pairs.size(); ++e) {
+      if (config[e] == (int32_t)pairs[e]->config) continue;
+      pairs[e]->config = config[e];
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) pairs[e]->F(r, c) = F[9 * e + 3 * r + c];
+    }
+    return n;
+  }
+};
+
+// ---------------------------------------------------------------------------
 // PruneWeaklyConnectedImages (processors/reconstruction_pruning.{h,cc}), stage 8 of GlobalMapper::Solve, on the device:
 // frames are flattened in sorted frame-id order and tracks in sorted track-id order, each observation becomes the frame
 // index of its image; a frame with >= 2 images present gets a self-loop (its intra-frame edges, :63-104).  Writes

@@ -151,9 +151,10 @@ struct Track {
   std::vector<std::pair<image_t, feature_t>> observations;
   bool is_initialized = false;
 };
-struct Matrix3 {   // Eigen::Matrix3d: the shim reads M(r, c)
+struct Matrix3 {   // Eigen::Matrix3d: the shim reads and writes M(r, c)
   double m[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
   double operator()(int r, int c) const { return m[3 * r + c]; }
+  double& operator()(int r, int c) { return m[3 * r + c]; }
 };
 struct MatchMatrix {   // Eigen::MatrixXi with two columns: (k, 0) feature in image 1, (k, 1) feature in image 2
   std::vector<std::array<int, 2>> rows_;

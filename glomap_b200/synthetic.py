@@ -861,6 +861,39 @@ def make_vgc_pairs(scene: Scene, pairs, seed: int = 1, f_noise: float = 0.0, out
                 is_outlier=is_outlier)
 
 
+def make_calibration_pairs(scene: Scene, pairs, seed: int = 1, uncalibrated_frac: float = 0.3, outlier_frac: float = 0.0):
+    """Image pairs for stages 0 and 1 of the mapper (``view_graph_manipulation`` / ``view_graph_calibration``) over the
+    image pairs ``pairs`` ([E, 2] image indices = image ids) of ``scene``: ``track_establishment.ImagePairMatches``
+    without matches, with the true cam2_from_cam1 (unit translation) and the F of ``make_vgc_pairs``.  A pair is
+    UNCALIBRATED with probability ``uncalibrated_frac``, else CALIBRATED.  ``outlier_frac`` of the pairs are CALIBRATED
+    outliers whose F is that of the true pose with both focal lengths three times too large: its Fetzer residuals at the
+    true focals are -8, far above ViewGraphCalibrator's threshold (a random F often stays under it).  Stage 0 recomputes
+    the F of the UNCALIBRATED pairs it promotes, so no outlier is UNCALIBRATED.  Returns (pairs, is_outlier [E])."""
+    from .track_establishment import ImagePairMatches
+    d = make_vgc_pairs(scene, pairs, seed=seed)
+    rng = np.random.default_rng([seed, 93])
+    img1, img2 = d["img1"].astype(np.int64), d["img2"].astype(np.int64)
+    R = geo.quat_xyzw_to_rotmat(scene.quat)
+    R_rel = R[img2] @ np.swapaxes(R[img1], -1, -2)
+    t_rel = scene.trans[img2] - np.einsum("nij,nj->ni", R_rel, scene.trans[img1])
+    t_rel /= np.linalg.norm(t_rel, axis=1, keepdims=True)
+    q_rel = geo.rotmat_to_quat_xyzw_fast(R_rel)
+    is_outlier = rng.random(len(img1)) < outlier_frac
+    scaled = scene.intr_params.copy()
+    scaled[:, 0] *= 3.0
+    scaled[scene.intr_model == PINHOLE, 1] *= 3.0
+    Kinv = np.array([np.linalg.inv(_pinhole_K(int(m), p)) for m, p in zip(scene.intr_model, scaled)])
+    for e in np.flatnonzero(is_outlier):
+        tx = np.array([[0.0, -t_rel[e, 2], t_rel[e, 1]], [t_rel[e, 2], 0.0, -t_rel[e, 0]], [-t_rel[e, 1], t_rel[e, 0], 0.0]])
+        Fo = Kinv[scene.cam_intr[img2[e]]].T @ tx @ R_rel[e] @ Kinv[scene.cam_intr[img1[e]]]
+        d["F"][e] = (Fo / np.linalg.norm(Fo)).ravel()
+    uncal = (rng.random(len(img1)) < uncalibrated_frac) & ~is_outlier
+    out = [ImagePairMatches(int(img1[e]), int(img2[e]), np.zeros((0, 2), np.int32), np.zeros(0, np.int64),
+                            config=3 if uncal[e] else 2, quat_xyzw=q_rel[e].copy(), trans=t_rel[e].copy(),
+                            F=d["F"][e].reshape(3, 3).copy()) for e in range(len(img1))]
+    return out, is_outlier
+
+
 # ---------------------------------------------------------------------------
 # Covisibility clusters (input of PruneWeaklyConnectedImages)
 # ---------------------------------------------------------------------------

@@ -348,6 +348,31 @@ int b200sfm_view_graph_keep_largest_component(b200sfm_ctx* ctx, int32_t num_fram
                                               int64_t num_pairs, const int32_t* pair_image1, const int32_t* pair_image2,
                                               uint8_t* pair_valid, uint8_t* frame_registered, int32_t* num_registered_images);
 
+/* ---- stage 0: image pair configurations --------------------------------------------------------------------------------
+ * b200sfm_view_graph_update_pairs_config: ViewGraphManipulater::UpdateImagePairsConfig
+ * (glomap/processors/view_graph_manipulation.cc:178-237), the first half of stage 0 of GlobalMapper::Solve
+ * (controllers/global_mapper.cc:22-34).  K cameras: intr_model [K] / intr_params [K][B200SFM_INTR_STRIDE] and
+ * has_prior_focal [K] (Camera::has_prior_focal_length); E pairs: pair_cam1 / pair_cam2 [E] the camera of each image,
+ * pair_valid [E], pair_quat_xyzw [E][4] / pair_trans [E][3] cam2_from_cam1, pair_config [E] (b200sfm_two_view_config,
+ * in/out) and pair_F [E][9] row-major (in/out).
+ *   Counting: a pair with pair_valid[e] != 0 whose two cameras both have a prior focal adds 1 to `total` of both cameras
+ *   when it is CALIBRATED or UNCALIBRATED, and 1 to `calibrated` of both when it is CALIBRATED (a pair inside one camera
+ *   counts twice for it).  A camera is valid when calibrated * 1. / total > 0.5 (FP64, strict); a camera no pair counted
+ *   is not valid.
+ *   Promotion: a valid UNCALIBRATED pair whose two cameras are valid becomes CALIBRATED, and its F becomes
+ *   K2^-T [t]x R K1^-1 (FundamentalFromMotionAndCameras, math/two_view_geometry.cc:38-55; K = Camera::GetK with fx = fy =
+ *   f for the SIMPLE_* models; R = Eigen's toRotationMatrix of the quaternion as given).  F is computed from the
+ *   cam2_from_cam1 the pair carries: the reference runs this pass before DecomposeRelPose, when a pair read from the
+ *   database still has the converter's identity pose, so its promoted F is the zero matrix there too.
+ * num_promoted counts the promoted pairs; pair_valid is not changed.  Host buffers.  A camera index outside [0, K) gives
+ * B200SFM_ERR_INVALID_ARG (checked on the device, never dereferenced); a pair to be promoted whose camera model is
+ * outside 0-3 gives B200SFM_ERR_UNSUPPORTED; the outputs are then untouched.  num_pairs == 0 returns B200SFM_OK with a
+ * zero count.  No collectives: on a distributed context each rank works on the pairs it is given. */
+int b200sfm_view_graph_update_pairs_config(b200sfm_ctx* ctx, int32_t K, const int32_t* intr_model, const double* intr_params,
+                                           const uint8_t* has_prior_focal, int64_t num_pairs, const int32_t* pair_cam1,
+                                           const int32_t* pair_cam2, const uint8_t* pair_valid, const double* pair_quat_xyzw,
+                                           const double* pair_trans, int32_t* pair_config, double* pair_F, int64_t* num_promoted);
+
 /* ---- (ii) global positioning (BATA) ----------------------------------------- */
 /* Mirror of GlobalPositionerOptions (global_positioning.h:9-54) + inherited
  * solver options (optimization_base.h:18-23) + PCG knobs.  Only the
