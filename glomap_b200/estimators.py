@@ -686,20 +686,8 @@ class RotationEstimator:
                 return False, None
             _lib.check(ctx.handle, rc)
             return bool(st.usable), geo.so3_exp(theta)
-        # ---- gravity-aligned frames (host prep: SetupLinearSystem .cc:207-217,311-326) ----
-        g = np.asarray(gravity, dtype=np.float64)
-        hg = ~np.isnan(g).any(axis=1)
-        R_align = np.tile(np.eye(3), (n, 1, 1))
-        for i in np.nonzero(hg)[0]:
-            R_align[i] = get_align_rot(g[i])
-        theta = geo.so3_log(R0)
-        for i in np.nonzero(hg)[0]:
-            theta[i] = [0.0, geo.so3_log((R_align[i].T @ R0[i])[None])[0, 1], 0.0]     # RotUpToAngle
-        Rr = np.array(vg.R_rel, dtype=np.float64, copy=True)
-        gi, gj = hg[vg.ei], hg[vg.ej]
-        Rr[gi] = Rr[gi] @ R_align[vg.ei[gi]]
-        Rr[gj] = np.swapaxes(R_align[vg.ej[gj]], -1, -2) @ Rr[gj]
-        fixed = int(np.nonzero(hg)[0][0]) if hg.any() else fixed                          # .cc:213-217
+        hg, R_align, theta, Rr, g_fixed = gravity_aligned_inputs(vg, R0, gravity)
+        fixed = fixed if g_fixed is None else g_fixed
         theta = _c(theta, np.float64)
         Rr = _c(Rr.reshape(-1, 9), np.float64)
         hg8 = _c(hg, np.uint8)
@@ -712,6 +700,31 @@ class RotationEstimator:
         R = geo.so3_exp(theta)
         R[hg] = R_align[hg] @ R[hg]                                                       # ConvertResults .cc:787-793
         return bool(st.usable), R
+
+
+def gravity_aligned_inputs(vg, R0, gravity):
+    """The host preparation of the gravity-aligned solve (SetupLinearSystem, global_rotation_averaging.cc:207-217,
+    311-326) over the frame graph ``vg``: the frames with a prior (non-NaN rows of ``gravity`` [n,3]) carry
+    theta = (0, RotUpToAngle(R_align^T R0), 0), the others the angle-axis of R0; a pair's R_rel is multiplied by
+    R_align1 on the right when frame 1 has a prior and by R_align2^T on the left when frame 2 has one.  Returns
+    (has_gravity [n], R_align [n,3,3] (identity without a prior), theta [n,3], aligned R_rel [E,3,3], the gauge: the
+    first frame with a prior, or None without one)."""
+    from . import geometry as geo
+    n = vg.n_images
+    g = np.asarray(gravity, dtype=np.float64)
+    hg = ~np.isnan(g).any(axis=1)
+    R_align = np.tile(np.eye(3), (n, 1, 1))
+    for i in np.nonzero(hg)[0]:
+        R_align[i] = get_align_rot(g[i])
+    theta = geo.so3_log(R0)
+    for i in np.nonzero(hg)[0]:
+        theta[i] = [0.0, geo.so3_log((R_align[i].T @ R0[i])[None])[0, 1], 0.0]     # RotUpToAngle
+    Rr = np.array(vg.R_rel, dtype=np.float64, copy=True)
+    gi, gj = hg[vg.ei], hg[vg.ej]
+    Rr[gi] = Rr[gi] @ R_align[vg.ei[gi]]
+    Rr[gj] = np.swapaxes(R_align[vg.ej[gj]], -1, -2) @ Rr[gj]
+    fixed = int(np.nonzero(hg)[0][0]) if hg.any() else None                            # .cc:213-217
+    return hg, R_align, theta, Rr, fixed
 
 
 def estimate_rotations_rig_unknown(est: "RotationEstimator", g: dict, R_frames0, R_cams0, fixed: int = 0):

@@ -6,10 +6,12 @@ largest component, unless there is no such pair or they are more than 95 % of al
 starting from that result.  Frames are the view graph's nodes (trivial rigs; for known rigs pass the frame graph of
 ``estimators.rig_view_graph``).
 
-``solve_rotation_averaging_rig`` is the same driver for rigs given image by image, without gravity.  When a camera's
-cam_from_rig is not known yet it runs the reference's pre-pass (.cc:65-182): a rotation averaging in which every image of
-such a camera is a frame of its own, whose result ``ConvertRotationsFromImageToRig`` turns into first cam_from_rig and
-rig_from_world rotations (rotation_initializer.py, on the device) before the real solve starts from them."""
+``solve_rotation_averaging_rig`` is the same driver for rigs given image by image.  When a camera's cam_from_rig is not
+known yet it runs the reference's pre-pass (.cc:65-182): a rotation averaging in which every image of such a camera is a
+frame of its own, whose result ``ConvertRotationsFromImageToRig`` turns into first cam_from_rig and rig_from_world
+rotations (rotation_initializer.py, on the device) before the real solve starts from them.  With gravity every
+cam_from_rig must be known, as in the reference: the image pairs are folded onto the frames and the frame graph goes
+through the gravity-aligned, stratified driver above."""
 from __future__ import annotations
 
 import dataclasses
@@ -50,8 +52,8 @@ def _subgraph(vg, keep_edge):
                      np.asarray(vg.weight)[keep_edge], vg.R_gt)
 
 
-def _estimate_on(mask, vg, options, R0, gravity, ctx):
-    """EstimateRotations over the nodes of ``mask`` and the pairs between them (nodes renumbered in ascending order)."""
+def _estimate_on(mask, vg, R0, gravity, estimate):
+    """``estimate`` over the nodes of ``mask`` and the pairs between them (nodes renumbered in ascending order)."""
     from .synthetic import ViewGraph
     idx = np.nonzero(mask)[0]
     remap = np.full(vg.n_images, -1, np.int64)
@@ -59,47 +61,80 @@ def _estimate_on(mask, vg, options, R0, gravity, ctx):
     ei, ej = np.asarray(vg.ei), np.asarray(vg.ej)
     k = mask[ei] & mask[ej]
     sub = ViewGraph(len(idx), remap[ei[k]].astype(np.int32), remap[ej[k]].astype(np.int32), np.asarray(vg.R_rel)[k],
-                    np.asarray(vg.weight)[k], np.asarray(vg.R_gt)[idx])
-    ok, R = RotationEstimator(options, ctx).EstimateRotations(sub, R0[idx], gravity=None if gravity is None else gravity[idx])
+                    np.asarray(vg.weight)[k], None if vg.R_gt is None else np.asarray(vg.R_gt)[idx])
+    ok, R = estimate(sub, R0[idx], None if gravity is None else gravity[idx])
     return ok, idx, R
 
 
-def solve_rotation_averaging(vg, gravity=None, options: RotationAveragerOptions | None = None, R_init=None, ctx=None):
-    """``gravity`` [n,3] with NaN rows for frames without a prior (None: no gravity); ``R_init`` [n,3,3] the initial
-    rotations (``ReadGravity`` sets R_align for the frames with gravity, the identity elsewhere).  Returns
-    (ok, R [n,3,3] (R_init outside the solved component), registered [n] bool)."""
-    o = options or RotationAveragerOptions()
+def _estimator_options(o: RotationAveragerOptions) -> RotationEstimatorOptions:
+    return RotationEstimatorOptions(**{f.name: getattr(o, f.name) for f in dataclasses.fields(RotationEstimatorOptions)})
+
+
+def _solve_frames(vg, g, o, R, estimate, solve_1dof, info):
+    """.cc:13-63,183-197 over the frame graph ``vg``: the 1-DoF pass over the largest component of the pairs whose two
+    frames have gravity when ``solve_1dof``, then the whole largest component from its result.  ``estimate(vg, R0,
+    gravity)`` -> (ok, R) is RotationEstimator::EstimateRotations."""
     n = vg.n_images
-    R = np.tile(np.eye(3), (n, 1, 1)) if R_init is None else np.array(R_init, dtype=np.float64, copy=True)
-    g = None if gravity is None else np.asarray(gravity, dtype=np.float64)
     has = np.zeros(n, bool) if g is None else ~np.isnan(g).any(axis=1)
     ei, ej = np.asarray(vg.ei), np.asarray(vg.ej)
     reg = largest_component(n, ei, ej)                                           # .cc:13
     grav_pair = reg[ei] & reg[ej] & has[ei] & has[ej]
-    solve_1dof = o.use_gravity and o.use_stratified and g is not None and stratified_branch(vg, g, reg)
-    est_opts = RotationEstimatorOptions(**{f.name: getattr(o, f.name) for f in dataclasses.fields(RotationEstimatorOptions)})
+    if solve_1dof is None:
+        if g is not None:
+            info["gravity_pairs"], info["total_pairs"] = _count_gravity_pairs(ei, ej, reg, has)
+        solve_1dof = o.use_gravity and o.use_stratified and g is not None and _stratify(info["gravity_pairs"], info["total_pairs"])
+    info["stratified"] = bool(solve_1dof)
     if solve_1dof:
         sub = _subgraph(vg, grav_pair)
         mask = largest_component(n, sub.ei, sub.ej, reg)                          # .cc:56
-        ok, idx, R_sub = _estimate_on(mask, sub, est_opts, R, g, ctx)            # .cc:57-61
+        ok, idx, R_sub = _estimate_on(mask, sub, R, g, estimate)                  # .cc:57-61
         if not ok:
             return False, R, mask
         R[idx] = R_sub
-    ok, idx, R_all = _estimate_on(reg, vg, est_opts, R, g if o.use_gravity else None, ctx)   # .cc:184-195
+    ok, idx, R_all = _estimate_on(reg, vg, R, g if o.use_gravity else None, estimate)   # .cc:184-195
     if R_all is not None:
         R[idx] = R_all
     return ok, R, reg
+
+
+def solve_rotation_averaging(vg, gravity=None, options: RotationAveragerOptions | None = None, R_init=None, ctx=None,
+                             info=None):
+    """``gravity`` [n,3] with NaN rows for frames without a prior (None: no gravity); ``R_init`` [n,3,3] the initial
+    rotations (``ReadGravity`` sets R_align for the frames with gravity, the identity elsewhere).  Returns
+    (ok, R [n,3,3] (R_init outside the solved component), registered [n] bool).  ``info``, when a dict, receives
+    ``gravity_pairs`` / ``total_pairs`` (the pairs of the largest component with gravity at both ends / all of them) and
+    ``stratified`` (whether the 1-DoF pass ran)."""
+    o = options or RotationAveragerOptions()
+    n = vg.n_images
+    R = np.tile(np.eye(3), (n, 1, 1)) if R_init is None else np.array(R_init, dtype=np.float64, copy=True)
+    g = None if gravity is None else np.asarray(gravity, dtype=np.float64)
+    est_opts = _estimator_options(o)
+    info = {} if info is None else info
+
+    def estimate(sub, R0, grav):
+        return RotationEstimator(est_opts, ctx).EstimateRotations(sub, R0, gravity=grav)
+
+    return _solve_frames(vg, g, o, R, estimate, None, info)
+
+
+def _count_gravity_pairs(ei, ej, registered, has_gravity):
+    """(pairs between registered nodes whose two nodes have gravity, pairs between registered nodes) (.cc:22-40)."""
+    ei, ej = np.asarray(ei), np.asarray(ej)
+    pair_in = registered[ei] & registered[ej]
+    return int((pair_in & has_gravity[ei] & has_gravity[ej]).sum()), int(pair_in.sum())
 
 
 def stratified_branch(vg, gravity, registered=None) -> bool:
     """Whether SolveRotationAveraging solves the 1-DoF subsystem first (.cc:42-50), given gravity and use_stratified."""
     g = np.asarray(gravity, dtype=np.float64)
     has = ~np.isnan(g).any(axis=1)
-    ei, ej = np.asarray(vg.ei), np.asarray(vg.ej)
-    reg = largest_component(vg.n_images, ei, ej) if registered is None else np.asarray(registered, bool)
-    pair_in = reg[ei] & reg[ej]
-    grav_pairs = int((pair_in & has[ei] & has[ej]).sum())
-    return not (grav_pairs == 0 or grav_pairs > int(pair_in.sum()) * 0.95)
+    reg = largest_component(vg.n_images, vg.ei, vg.ej) if registered is None else np.asarray(registered, bool)
+    return _stratify(*_count_gravity_pairs(vg.ei, vg.ej, reg, has))
+
+
+def _stratify(grav_pairs: int, total_pairs: int) -> bool:
+    """.cc:49-50: no 1-DoF pass without a gravity pair or with more than 95 % of the pairs gravity pairs."""
+    return not (grav_pairs == 0 or grav_pairs > total_pairs * 0.95)
 
 
 # ---------------------------------------------------------------------------
@@ -163,6 +198,11 @@ class _DeviceOps:
         ok, R = est.EstimateRotations(vg, R0)
         return ok, R, (est.summary.l1_iterations, est.summary.irls_iterations)
 
+    def estimate_gravity(self, vg, R0, gravity):
+        """RotationEstimator with use_gravity over a frame graph: the frames with a prior (non-NaN rows of ``gravity``)
+        are 1-DoF.  Returns (ok, R)."""
+        return RotationEstimator(self.options, self.ctx).EstimateRotations(vg, R0, gravity=gravity)
+
     def estimate_rig(self, g, R_frames0, R_cams0):
         """RotationEstimator with unknown cam_from_rig rotations over rig_view_graph_unknown's layout."""
         from .estimators import estimate_rotations_rig_unknown
@@ -188,7 +228,34 @@ def _image_rotations(vg, image_mask, ops):
     return R, reached
 
 
-def _solve_rig(vg, image_frame, image_camera, camera_known, cam_from_rig, frame_ref_camera, o, R_init, ops, info):
+def image_has_gravity(image_frame, image_camera, frame_ref_camera, camera_known, frame_gravity):
+    """Image::HasGravity (scene/image.h:78-84): the image's frame has a prior (a non-NaN row of ``frame_gravity`` [F,3])
+    and its camera is the frame's reference camera or has a known cam_from_rig.  Returns [I] bool."""
+    fr, cam = np.asarray(image_frame, np.int64), np.asarray(image_camera, np.int64)
+    has_frame = ~np.isnan(np.asarray(frame_gravity, np.float64)).any(axis=1)
+    return has_frame[fr] & ((cam == np.asarray(frame_ref_camera, np.int64)[fr]) | np.asarray(camera_known, bool)[cam])
+
+
+def _solve_rig_gravity(vg, fr, cam, known, R_cam, ref_cam, gravity, o, R, reg, ops, info):
+    """.cc:13-63,183-197 with use_gravity and every cam_from_rig known: the image pairs folded onto the frames with the
+    known rotations (self loops dropped), then the frame-graph driver with the frames' priors.  The 1-DoF pass is chosen
+    on the image pairs, as the reference counts them (.cc:22-50)."""
+    from .synthetic import ViewGraph
+    F = len(ref_cam)
+    ei, ej = np.asarray(vg.ei), np.asarray(vg.ej)
+    img_g = image_has_gravity(fr, cam, ref_cam, known, gravity)
+    pair_in = reg[fr[ei]] & reg[fr[ej]]
+    n_grav, n_total = int((pair_in & img_g[ei] & img_g[ej]).sum()), int(pair_in.sum())
+    info["gravity_pairs"], info["total_pairs"] = n_grav, n_total
+    solve_1dof = o.use_stratified and _stratify(n_grav, n_total)
+    keep, fi, fj, R_rel = fold_pairs(vg, fr, R_cam, cam)
+    fg = ViewGraph(F, fi.astype(np.int32), fj.astype(np.int32), R_rel, np.asarray(vg.weight)[keep], np.tile(np.eye(3), (F, 1, 1)))
+    ok, R, mask = _solve_frames(fg, gravity, o, R, ops.estimate_gravity, solve_1dof, info)
+    return ok, R, R_cam, mask
+
+
+def _solve_rig(vg, image_frame, image_camera, camera_known, cam_from_rig, frame_ref_camera, o, R_init, ops, info,
+               gravity=None):
     from . import geometry as geo
     from .estimators import rig_view_graph, rig_view_graph_unknown
     fr = np.asarray(image_frame, np.int64)
@@ -205,7 +272,12 @@ def _solve_rig(vg, image_frame, image_camera, camera_known, cam_from_rig, frame_
     reg = largest_component(F, fr[ei], fr[ej])                                    # .cc:13
     unknown = ~known
     if o.use_gravity and unknown.any():                                           # global_rotation_averaging.cc:47-59
+        info.setdefault("log", []).append(
+            f"rotation averaging: use_gravity needs every cam_from_rig, camera(s) {np.flatnonzero(unknown).tolist()} "
+            "have none")
         return False, R, R_cam, reg
+    if o.use_gravity and gravity is not None:
+        return _solve_rig_gravity(vg, fr, cam, known, R_cam, ref_cam, np.asarray(gravity, np.float64), o, R, reg, ops, info)
     img_reg = reg[fr]
     pair_ok = np.ones(len(ei), bool)
     cam_init = np.zeros(K, bool)                                                  # unknown cameras with an average
@@ -284,8 +356,9 @@ def _solve_rig(vg, image_frame, image_camera, camera_known, cam_from_rig, frame_
 
 
 def solve_rotation_averaging_rig(vg, image_frame, image_camera, camera_known, cam_from_rig, frame_ref_camera,
-                                 options: RotationAveragerOptions | None = None, R_init=None, ctx=None, info=None):
-    """SolveRotationAveraging (.cc:8-197) for rigs, without gravity.
+                                 options: RotationAveragerOptions | None = None, R_init=None, ctx=None, info=None,
+                                 gravity=None):
+    """SolveRotationAveraging (.cc:8-197) for rigs.
 
     ``vg``: the image-level view graph (cam2_from_cam1 per pair); image_frame [I] and image_camera [I]: every image's
     frame and camera; camera_known [K] and cam_from_rig [K,4] (xyzw): the cameras whose cam_from_rig is known and those
@@ -300,12 +373,22 @@ def solve_rotation_averaging_rig(vg, image_frame, image_camera, camera_known, ca
     Pairs with an image outside the trivial largest component leave the view graph, as in the reference.  Otherwise
     (.cc:183-196) the initialisation is forced on when a camera is unknown: images of unknown cameras are skipped and
     those cameras start from zero (global_rotation_averaging.cc:239-242).  The solve runs over the largest component of
-    the remaining pairs.  With use_gravity and an unknown camera the call returns False (.cc:47-59).
+    the remaining pairs.
+
+    ``gravity`` [F,3]: one prior per frame (NaN rows: none), read only with use_gravity.  With use_gravity and a camera
+    whose cam_from_rig is not known the call returns False (.cc:47-59) before any solve, and says why in
+    ``info["log"]``.  With every cam_from_rig known and ``gravity``, the image pairs are folded onto the frames
+    (global_rotation_averaging.cc:274-309, pairs inside one frame dropped) and aligned with their frames' R_align
+    (.cc:311-326); the frames with a prior are 1-DoF, the first of them is the gauge (.cc:207-217); with use_stratified
+    the pairs whose two images have gravity (``image_has_gravity``) are solved first on their largest component unless
+    there is none or they are more than 95 % of the pairs (rotation_averager.cc:15-63), and the whole graph then starts
+    from that result.  This is ``solve_rotation_averaging`` on the frame graph of ``estimators.rig_view_graph``, except
+    that the 95 % rule counts image pairs, pairs inside one frame included, as the reference does.
 
     Returns (ok, R [F,3,3] rig_from_world rotations (R_init outside the solved frames), R_cam [K,3,3] cam_from_rig
     rotations (the estimates for the unknown cameras with images; known ones unchanged), registered [F] bool).  ``info``,
-    when a dict, receives the (L1, IRLS) iteration counts of the trivial and the final solve."""
+    when a dict, receives the (L1, IRLS) iteration counts of the trivial and the final solve; with gravity,
+    ``gravity_pairs`` / ``total_pairs`` / ``stratified``."""
     o = options or RotationAveragerOptions()
-    est_opts = RotationEstimatorOptions(**{f.name: getattr(o, f.name) for f in dataclasses.fields(RotationEstimatorOptions)})
     return _solve_rig(vg, image_frame, image_camera, camera_known, cam_from_rig, frame_ref_camera, o, R_init,
-                      _DeviceOps(est_opts, ctx), {} if info is None else info)
+                      _DeviceOps(_estimator_options(o), ctx), {} if info is None else info, gravity)

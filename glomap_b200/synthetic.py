@@ -974,6 +974,16 @@ def make_gravity(R_gt: np.ndarray, noise_deg: float = 0.0, outlier_ratio: float 
     return g, out
 
 
+def make_frame_gravity(R_frames: np.ndarray, share: float = 1.0, noise_deg: float = 0.0, outlier_ratio: float = 0.0,
+                       seed: int = 1) -> np.ndarray:
+    """Gravity priors for the frames of a dataset (``GlobalMapper.Solve(..., gravity=...)``): ``make_gravity`` of the
+    ground-truth rig_from_world (or cam_from_world) rotations ``R_frames`` [F,3,3], with each frame left without a prior
+    (a NaN row) with probability 1 - ``share``.  Returns [F,3]."""
+    g, _ = make_gravity(R_frames, noise_deg, outlier_ratio, seed)
+    g[np.random.default_rng([seed, 13]).uniform(size=len(g)) >= share] = np.nan
+    return g
+
+
 def write_gravity_file(path: str, names, gravity: np.ndarray) -> None:
     """IMAGE_NAME GX GY GZ (glomap/io/pose_io.cc:139-180); rows of NaN (no prior) are not written."""
     with open(path, "w") as f:
