@@ -153,6 +153,7 @@ PROTOTYPES = {
     "b200sfm_ba_solve": (c_int32, [c_void_p, P(BAOpts), c_int32, c_int32, c_int64, c_int32] + [c_void_p] * 10 + [P(LMStats)]),
     "b200sfm_ba_problem_create": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32] + [c_void_p] * 6 + [c_int32, P(c_void_p)]),
     "b200sfm_ba_problem_create_rig": (c_int32, [c_void_p, c_int32, c_int32, c_int64, c_int32, c_int32] + [c_void_p] * 9 + [c_int32, P(c_void_p)]),
+    "b200sfm_ba_problem_set_images": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p]),
     "b200sfm_ba_problem_set_sensor_variable": (c_int32, [c_void_p, c_void_p]),
     "b200sfm_ba_problem_get_sensor_poses": (c_int32, [c_void_p, c_void_p, c_void_p]),
     "b200sfm_ba_problem_set_state": (c_int32, [c_void_p] * 5),

@@ -345,6 +345,21 @@ int b200sfm_ba_problem_create_rig(b200sfm_ctx* ctx, int32_t F, int32_t P, int64_
   return B200SFM_OK;
 }
 
+int b200sfm_ba_problem_set_images(b200sfm_ba_problem* p, int32_t I, const int32_t* image_frame, const int32_t* image_sensor) {
+  if (!p || I <= 0 || !image_frame || !image_sensor) return B200SFM_ERR_INVALID_ARG;
+  if (p->S <= 0) { p->ctx->err = "the problem has no rig sensors (b200sfm_ba_problem_create_rig)"; return B200SFM_ERR_INVALID_ARG; }
+  for (int32_t i = 0; i < I; ++i)
+    if (image_frame[i] < 0 || image_frame[i] >= p->C || image_sensor[i] < 0 || image_sensor[i] >= p->S) {
+      p->ctx->err = "image_frame / image_sensor out of range";
+      return B200SFM_ERR_INVALID_ARG;
+    }
+  return guarded(p->ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(p->ctx->device));
+    p->set_images(I, image_frame, image_sensor);
+    return (int)B200SFM_OK;
+  });
+}
+
 int b200sfm_ba_problem_set_sensor_variable(b200sfm_ba_problem* p, const uint8_t* sensor_variable) {
   if (!p || !sensor_variable) return B200SFM_ERR_INVALID_ARG;
   if (p->S <= 0) { p->ctx->err = "the problem has no rig sensors (b200sfm_ba_problem_create_rig)"; return B200SFM_ERR_INVALID_ARG; }

@@ -641,18 +641,31 @@ struct b200sfm_ba_problem {
     if (h_out) bear_res.download(h_out, (size_t)N * 3, s);
     B200_CUDA_OK(cudaStreamSynchronize(s));
   }
+  // the image table of a rig problem (b200sfm_ba_problem_set_images): image i = frame img_frame[i] through sensor
+  // img_sensor[i]; n_images = 0 means the dense layout, every frame through every sensor
+  int n_images = 0;
+  DevBuf<int> img_frame, img_sensor;
+  void set_images(int I, const int32_t* h_frame, const int32_t* h_sensor) {
+    img_frame.alloc(I); img_sensor.alloc(I);
+    img_frame.upload(h_frame, I, ctx->stream);
+    img_sensor.upload(h_sensor, I, ctx->stream);
+    B200_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+    n_images = I;
+  }
   // NormalizeReconstruction (reconstruction_normalizer.cc:5-104) on the current state; returns the similarity
   // X' = scale X + t (identity rotation)
   void normalize(bool fixed_scale, double extent, double p0, double p1, double* scale_out, double* t_out) {
     using namespace b200;
     cudaStream_t s = ctx->stream;
-    const int n_img = S > 0 ? C * S : C;
+    const int n_img = S > 0 ? (n_images > 0 ? n_images : C * S) : C;
     double scale = 1.0, t[3] = {0, 0, 0};
     if (n_img > 0) {
       DevBuf<float> c_in, c_out;
       DevBuf<double> stats;
       c_in.alloc((size_t)n_img * 3); c_out.alloc((size_t)n_img * 3); stats.alloc(9);
-      B200_LAUNCH(ctx, proc_image_centres, cdiv(n_img, 256), 256, 0, C, S, quat[cur].p, trans[cur].p, S > 0 ? sens_q[cur].p : nullptr,
+      const bool table = S > 0 && n_images > 0;
+      B200_LAUNCH(ctx, proc_image_centres, cdiv(n_img, 256), 256, 0, n_img, S, table ? img_frame.p : nullptr,
+                  table ? img_sensor.p : nullptr, quat[cur].p, trans[cur].p, S > 0 ? sens_q[cur].p : nullptr,
                   S > 0 ? sens_t[cur].p : nullptr, c_in.p, c_in.p + n_img, c_in.p + 2 * (size_t)n_img);
       size_t need = 0;
       cub::DeviceRadixSort::SortKeys(nullptr, need, c_in.p, c_out.p, n_img, 0, 32, s);

@@ -151,7 +151,10 @@ __global__ void filter_triangulation_angle(BAView v, const double* __restrict__ 
       const double c1 = -(R[1] * tx + R[4] * ty + R[7] * tz);
       const double c2 = -(R[2] * tx + R[5] * ty + R[8] * tz);
       const double d0 = X0 - c0, d1 = X1 - c1, d2 = X2 - c2;
-      const double inv = 1.0 / sqrt(d0 * d0 + d1 * d1 + d2 * d2);
+      // Eigen's normalized() leaves a zero vector as it is: a point on a camera centre gives a zero ray, whose dot
+      // product 0 counts as a wide pair
+      const double n2 = d0 * d0 + d1 * d1 + d2 * d2;
+      const double inv = n2 > 0.0 ? 1.0 / sqrt(n2) : 0.0;
       ray[s][0] = d0 * inv; ray[s][1] = d1 * inv; ray[s][2] = d2 * inv;
     }
     if (ray[0][0] * ray[1][0] + ray[0][1] * ray[1][1] + ray[0][2] * ray[1][2] < thres) status = true;

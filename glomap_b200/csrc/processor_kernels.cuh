@@ -6,27 +6,28 @@
 //     points.  The mapper calls it between the BA solves (controllers/global_mapper.cc:185,232,336): on a resident
 //     problem that is three small kernels instead of a download / upload of the whole state.
 //   * UndistortImages (glomap/processors/image_undistorter.cc:7-53): pixel -> unit bearing per observation,
-//     CamFromImg(xy).homogeneous().normalized().  Radial models are inverted with the 50-step fixed-point iteration of the
-//     host restatement (glomap_b200/synthetic.py bearings_from_scene; colmap iterates Newton steps to the same point).
+//     CamFromImg(xy).homogeneous().normalized().  Radial models are inverted on the radius with a safeguarded Newton
+//     iteration, the same steps as the host restatement (glomap_b200/synthetic.py bearings_from_pixels).
 #pragma once
 #include "ba_kernels.cuh"
 
 namespace b200 {
 
-// projection centre of every image as float: trivial frames -> C images; rigs -> F x S images (frame-major)
-__global__ void proc_image_centres(int F, int S, const double* __restrict__ quat, const double* __restrict__ trans,
+// projection centre of every image as float: trivial frames -> n = C images; rigs -> n images (frame img_frame[i] seen
+// through sensor img_sensor[i]), or with null tables the dense layout of n = F x S images (frame-major)
+__global__ void proc_image_centres(int n, int S, const int* __restrict__ img_frame, const int* __restrict__ img_sensor,
+                                   const double* __restrict__ quat, const double* __restrict__ trans,
                                    const double* __restrict__ sens_q, const double* __restrict__ sens_t,
                                    float* __restrict__ cx, float* __restrict__ cy, float* __restrict__ cz) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const int n = S > 0 ? F * S : F;
   if (i >= n) return;
-  const int f = S > 0 ? i / S : i;
+  const int f = S > 0 ? (img_frame ? img_frame[i] : i / S) : i;
   const double q[4] = {quat[4 * (size_t)f], quat[4 * (size_t)f + 1], quat[4 * (size_t)f + 2], quat[4 * (size_t)f + 3]};
   double R[9];
   quat_to_R(q, R);
   double t[3] = {trans[3 * (size_t)f], trans[3 * (size_t)f + 1], trans[3 * (size_t)f + 2]};
   if (S > 0) {   // cam_from_world = cam_from_rig o rig_from_world
-    const int s = i % S;
+    const int s = img_sensor ? img_sensor[i] : i % S;
     const double qs[4] = {sens_q[4 * s], sens_q[4 * s + 1], sens_q[4 * s + 2], sens_q[4 * s + 3]};
     double Rs[9], Rc[9], tc[3];
     quat_to_R(qs, Rs);
@@ -86,6 +87,43 @@ __global__ void proc_scale_shift3(long long n, double scale, double t0, double t
   y[3 * i + 2] = scale * y[3 * i + 2] + t2;
 }
 
+// Radial undistortion on the radius: the r in [0, r_fold] with g(r) = r (1 + k1 r^2 + k2 r^4) = rd, returned as the
+// scale r / rd (1 at rd = 0).  g increases from 0 up to its fold r_fold, the first root of g'(r) = 1 + 3 k1 r^2 + 5 k2 r^4
+// (none: g increases for good, and the root is below 2.25 rd because d(r^2) > 4/9 there).  Newton from r = rd inside the
+// bracket [lo, hi] that the signs of g - rd maintain, a bisection where a step leaves it; stops when a step no longer
+// moves r, or after kUndistortMaxIters.  Past the fold (rd > g(r_fold)) there is no inverse and the result, r_fold at
+// most, is not meant to be used.  The host restatement (synthetic.undistort_radius_scale) takes the same steps.
+constexpr int kUndistortMaxIters = 100;
+__device__ __forceinline__ double undistort_radius_scale(double k1, double k2, double rd) {
+  if (!(rd > 0.0)) return 1.0;
+  // smallest positive root s of 1 + 3 k1 s + 5 k2 s^2 (s = r^2), or none
+  double s_fold = -1.0;
+  if (k2 == 0.0) {
+    if (k1 < 0.0) s_fold = -1.0 / (3.0 * k1);
+  } else {
+    const double disc = 9.0 * k1 * k1 - 20.0 * k2;
+    if (disc >= 0.0) {
+      const double q = -0.5 * (3.0 * k1 + copysign(sqrt(disc), k1));   // roots q / (5 k2) and 1 / q
+      const double a = q / (5.0 * k2), b = 1.0 / q;
+      if (a > 0.0) s_fold = a;
+      if (b > 0.0 && (s_fold < 0.0 || b < s_fold)) s_fold = b;
+    }
+  }
+  double lo = 0.0, hi = s_fold > 0.0 ? sqrt(s_fold) : 2.25 * rd;
+  double r = fmin(rd, hi);
+  for (int it = 0; it < kUndistortMaxIters; ++it) {
+    const double s = r * r;
+    const double f = r * (1.0 + s * (k1 + k2 * s)) - rd;
+    if (f < 0.0) lo = r; else hi = r;
+    const double df = 1.0 + s * (3.0 * k1 + 5.0 * k2 * s);
+    double rn = r - f / df;
+    if (!(rn >= lo && rn <= hi)) rn = 0.5 * (lo + hi);   // outside the bracket, or df <= 0 / NaN
+    if (rn == r) break;
+    r = rn;
+  }
+  return r / rd;
+}
+
 // CamFromImg(xy).homogeneous().normalized() of one pixel for camera model m (0-3) with parameters p; writes out[0..2].
 // Shared by UndistortImages below and the per-feature bearings of ImagePairsInlierCount (pair_kernels.cuh).
 __device__ __forceinline__ void bearing_from_pixel(int m, const double* __restrict__ p, double2 xy, double* __restrict__ out) {
@@ -96,13 +134,8 @@ __device__ __forceinline__ void bearing_from_pixel(int m, const double* __restri
     u = (xy.x - p[2]) / p[0]; v = (xy.y - p[3]) / p[1];
   } else {               // SIMPLE_RADIAL f cx cy k / RADIAL f cx cy k1 k2
     const double ud = (xy.x - p[1]) / p[0], vd = (xy.y - p[2]) / p[0];
-    const double k1 = p[3], k2 = (m == 3) ? p[4] : 0.0;
-    u = ud; v = vd;
-    for (int it = 0; it < 50; ++it) {
-      const double r2 = u * u + v * v;
-      const double dd = 1.0 + k1 * r2 + k2 * r2 * r2;
-      u = ud / dd; v = vd / dd;
-    }
+    const double sc = undistort_radius_scale(p[3], (m == 3) ? p[4] : 0.0, sqrt(ud * ud + vd * vd));
+    u = ud * sc; v = vd * sc;
   }
   const double inv = 1.0 / sqrt(u * u + v * v + 1.0);
   out[0] = u * inv;

@@ -156,6 +156,14 @@ class BAProblem:
             _lib.check(ctx.handle, rc)
             self.handle = h
             self.S = scene.S
+            # the image table, unless it is the dense layout the problem assumes without it (normalize() reads it)
+            fr, se = np.asarray(scene.image_frame), np.asarray(scene.image_sensor)
+            dense = len(fr) == scene.F * scene.S and np.array_equal(fr, np.arange(len(fr)) // scene.S) \
+                and np.array_equal(se, np.arange(len(se)) % scene.S)
+            if not dense:
+                self._keep += [_c(fr, np.int32), _c(se, np.int32)]
+                _lib.check(ctx.handle, self.lib.b200sfm_ba_problem_set_images(h, len(fr), _ptr(self._keep[-2]),
+                                                                              _ptr(self._keep[-1])))
             return
         self.S = 0
         self._keep = [_c(scene.pt_obs_begin, np.int64), _c(scene.obs_cam, np.int32), _c(scene.obs_xy, np.float64),

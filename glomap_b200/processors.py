@@ -1,12 +1,14 @@
 """Host-side steps on either side of the solvers (SURVEY.md 8(f) item 2), on the flat SoA scene:
 
 * ``normalize_reconstruction`` -- glomap/processors/reconstruction_normalizer.cc:5-104: robust (p0..p1 percentile, float32
-  coordinates as in the reference) bounding box of the projection centres -> Sim3 with identity rotation that moves the
+  coordinates as in the reference) bounding box of the projection centres of the registered images (on rigs: the image
+  table, not every frame-sensor combination) -> Sim3 with identity rotation that moves the
   trimmed mean to the origin and scales the box diagonal to ``extent``; applied to the frame poses
   (colmap::TransformCameraWorld), the non-reference cam_from_rig translations and the points.  It runs between the BA
   solves of the mapper (controllers/global_mapper.cc:185,232,336) and fixes the gauge / scale BA leaves free.
 * ``undistort_images`` -- glomap/processors/image_undistorter.cc:7-53: pixel -> unit bearing per feature
-  (``CamFromImg(xy).homogeneous().normalized()``), the input of global positioning and of the angle filter.
+  (``CamFromImg(xy).homogeneous().normalized()``), the input of global positioning and of the angle filter; radial
+  models are inverted on the radius by a safeguarded Newton iteration (``synthetic.undistort_radius_scale``).
 
 Both are O(N) host work in the reference as well; the device-resident versions are a later row."""
 from __future__ import annotations
@@ -20,7 +22,7 @@ from . import synthetic as S
 def normalize_reconstruction(scene, fixed_scale: bool = False, extent: float = 10.0, p0: float = 0.1, p1: float = 0.9):
     """In place on a ``Scene`` or ``RigScene``; returns the applied Sim3 as (scale, translation): X' = scale * X + t."""
     R = geo.quat_xyzw_to_rotmat(scene.quat)
-    if hasattr(scene, "obs_sensor"):      # image centres of all F*S images (reconstruction_normalizer.cc:23-29)
+    if hasattr(scene, "obs_sensor"):      # centres of the images of the table, the registered ones (reconstruction_normalizer.cc:23-29)
         Ri, ti = scene.image_poses()
         centers = geo.centers_from_pose(Ri, ti)
     else:

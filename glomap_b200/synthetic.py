@@ -485,7 +485,7 @@ def bearings_from_scene(scene: Scene) -> np.ndarray:
     """Unit bearing of each observation in the camera frame -- what the
     reference keeps in ``Image::features_undist`` (glomap/scene/image.h:31,
     processors/image_undistorter.cc).  Exact inverse for the pinhole models;
-    radial models are inverted by fixed-point iteration."""
+    radial models are inverted on the radius (``undistort_radius_scale``)."""
     out = np.empty((scene.N, 3))
     ci = scene.cam_intr[scene.obs_cam]
     for k in range(len(scene.intr_model)):
@@ -496,6 +496,58 @@ def bearings_from_scene(scene: Scene) -> np.ndarray:
     return out
 
 
+UNDISTORT_MAX_ITERS = 100
+
+
+def radial_fold_s(k1: float, k2: float) -> float:
+    """The smallest positive s = r^2 where d/dr [r (1 + k1 r^2 + k2 r^4)] = 1 + 3 k1 s + 5 k2 s^2 reaches 0, or -1 when
+    there is none."""
+    if k2 == 0.0:
+        return -1.0 / (3.0 * k1) if k1 < 0.0 else -1.0
+    disc = 9.0 * k1 * k1 - 20.0 * k2
+    if disc < 0.0:
+        return -1.0
+    q = -0.5 * (3.0 * k1 + np.copysign(np.sqrt(disc), k1))      # roots q / (5 k2) and 1 / q
+    a, b = q / (5.0 * k2), 1.0 / q
+    s = a if a > 0.0 else -1.0
+    if b > 0.0 and (s < 0.0 or b < s):
+        s = b
+    return s
+
+
+def undistort_radius_scale(k1: float, k2: float, rd: np.ndarray) -> np.ndarray:
+    """r / rd for the r in [0, r_fold] with r (1 + k1 r^2 + k2 r^4) = rd (1 where rd = 0): Newton from r = rd inside a
+    bracket kept by the sign of the residual, a bisection where a step leaves it, until a step no longer moves r or
+    after ``UNDISTORT_MAX_ITERS``.  g(r) = r d(r^2) increases up to its fold (``radial_fold_s``); without one the root is
+    below 2.25 rd, as d(r^2) > 4/9 there.  Past the fold there is no inverse and the result (r_fold at most) is not
+    meant to be used.  The same steps as ``undistort_radius_scale`` in csrc/processor_kernels.cuh."""
+    rd = np.asarray(rd, np.float64)
+    s_fold = radial_fold_s(float(k1), float(k2))
+    lo = np.zeros_like(rd)
+    hi = np.full_like(rd, np.sqrt(s_fold)) if s_fold > 0.0 else 2.25 * rd
+    r = np.minimum(rd, hi)
+    act = rd > 0.0
+    for _ in range(UNDISTORT_MAX_ITERS):
+        if not act.any():
+            break
+        ra = r[act]
+        s = ra * ra
+        f = ra * (1.0 + s * (k1 + k2 * s)) - rd[act]
+        la, ha = lo[act], hi[act]
+        la = np.where(f < 0.0, ra, la)
+        ha = np.where(f < 0.0, ha, ra)
+        df = 1.0 + s * (3.0 * k1 + 5.0 * k2 * s)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            rn = ra - f / df
+        rn = np.where((rn >= la) & (rn <= ha), rn, 0.5 * (la + ha))
+        lo[act], hi[act] = la, ha
+        moved = rn != ra
+        r[act] = rn
+        act[act] = moved
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(rd > 0.0, r / rd, 1.0)
+
+
 def bearings_from_pixels(m: int, p: np.ndarray, xy: np.ndarray) -> np.ndarray:
     """``CamFromImg(xy).homogeneous().normalized()`` of [n,2] pixels of one camera (model ``m``, parameters ``p``)."""
     if m == SIMPLE_PINHOLE:
@@ -504,11 +556,8 @@ def bearings_from_pixels(m: int, p: np.ndarray, xy: np.ndarray) -> np.ndarray:
         u, v = (xy[:, 0] - p[2]) / p[0], (xy[:, 1] - p[3]) / p[1]
     else:
         ud, vd = (xy[:, 0] - p[1]) / p[0], (xy[:, 1] - p[2]) / p[0]
-        u, v = ud.copy(), vd.copy()
-        for _ in range(50):
-            r2 = u * u + v * v
-            dd = 1 + p[3] * r2 + (p[4] * r2 * r2 if m == RADIAL else 0.0)
-            u, v = ud / dd, vd / dd
+        sc = undistort_radius_scale(p[3], p[4] if m == RADIAL else 0.0, np.sqrt(ud * ud + vd * vd))
+        u, v = ud * sc, vd * sc
     b = np.stack([u, v, np.ones_like(u)], 1)
     return b / np.linalg.norm(b, axis=1, keepdims=True)
 

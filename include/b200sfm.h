@@ -188,6 +188,11 @@ int b200sfm_ba_problem_create_rig(b200sfm_ctx* ctx, int32_t F, int32_t P, int64_
                                   const double* sensor_trans /*[S][3]*/, const int32_t* sensor_intr /*[S]*/,
                                   const int32_t* intr_model, const uint8_t* frame_const_mask,
                                   int32_t min_num_view_per_track, b200sfm_ba_problem** out);
+/* The image table of a rig problem: image i is frame image_frame[i] seen through sensor image_sensor[i] (I > 0 images,
+ * frames in [0, F), sensors in [0, S)).  Only b200sfm_ba_problem_normalize reads it: its box and mean run over these
+ * images, the registered ones, as reconstruction_normalizer.cc:23-29 does.  Without the call the problem assumes the
+ * dense layout, every frame through every sensor (F * S images). */
+int b200sfm_ba_problem_set_images(b200sfm_ba_problem* p, int32_t I, const int32_t* image_frame, const int32_t* image_sensor);
 /* optimize_rig_poses (bundle_adjustment.cc:162-180,296-308, colmap::RigReprojErrorCostFunctor): mark the sensors whose
  * cam_from_rig is an UNKNOWN of the following solves (the reference: every non-reference camera sensor); takes effect
  * when b200sfm_ba_opts::optimize_rig_poses is set.  sensor_variable[S]: 1 = unknown.  The optimised poses are read
@@ -223,7 +228,8 @@ int b200sfm_ba_problem_filter_reprojection_normalized(b200sfm_ba_problem* p, con
                                                       int64_t* num_tracks_changed);
 /* The two per-element processors the mapper runs between the solvers, on the resident problem (SURVEY.md 8(f) item 2).
  * b200sfm_ba_problem_normalize -- glomap/processors/reconstruction_normalizer.cc:5-104 (NormalizeReconstruction): robust
- * p0..p1 percentile box and trimmed mean of the image centres (float coordinates, sorted per axis), similarity with
+ * p0..p1 percentile box and trimmed mean of the image centres (float coordinates, sorted per axis; on rigs the images of
+ * b200sfm_ba_problem_set_images, or all F * S frame-sensor combinations without it), similarity with
  * identity rotation X' = scale X + t applied to the frame poses, the cam_from_rig translations and the points of the
  * CURRENT state; returns the similarity (either pointer may be NULL).
  * b200sfm_ba_problem_undistort -- glomap/processors/image_undistorter.cc:7-53 (UndistortImages): unit bearing

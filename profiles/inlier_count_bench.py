@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """ImagePairsInlierCount on the GPU (b200sfm_image_pairs_inlier_count) on seeded match sets.
 
-  python profiles/inlier_count_bench.py [--sizes config2,config4] [--reps 5] [--host-pairs 300]
+  python profiles/inlier_count_bench.py [--sizes config2,config4] [--reps 5] [--host-pairs 300] [--model 0]
 
-Match set: every pair of observations inside a track of ``synthetic.make_scene`` is a match, plus 20 % random outlier
+Match set: every pair of observations inside a track of ``synthetic.make_scene`` (camera model ``--model``, 0-3; 2 and 3
+exercise the radial undistortion of the bearing kernel) is a match, plus 20 % random outlier
 matches; pairs are 80 % CALIBRATED, 15 % UNCALIBRATED, 5 % PLANAR (``synthetic.make_pair_matches``).  Sizes: config2 =
 make_scene(1000, 200k) (about 9 M matches), config4 = make_scene(1000, 2M) (about 90 M matches; the 1000-camera view
 graph keeps about 180 matches per pair, where 10k cameras with random candidate sets would leave about 2).
@@ -49,12 +50,13 @@ def main():
     ap.add_argument("--sizes", default="config2,config4")
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--host-pairs", type=int, default=300)
+    ap.add_argument("--model", type=int, default=0, choices=[0, 1, 2, 3])
     args = ap.parse_args()
     sizes = args.sizes.split(",")
     if len(sizes) > 1:   # one process per size: a second torch.profiler session in a process records no kernels
         for size in sizes:
             subprocess.check_call([sys.executable, os.path.abspath(__file__), "--sizes", size, "--reps", str(args.reps),
-                                   "--host-pairs", str(args.host_pairs)])
+                                   "--host-pairs", str(args.host_pairs), "--model", str(args.model)])
         return
     import numpy as np
     import torch
@@ -68,7 +70,7 @@ def main():
     for size in sizes:
         C, P = SIZES[size]
         t0 = time.perf_counter()
-        d = S.make_pair_matches(S.make_scene(C, P, 10.0, seed=1, pixel_sigma=0.5), seed=1)
+        d = S.make_pair_matches(S.make_scene(C, P, 10.0, seed=1, pixel_sigma=0.5, model=args.model), seed=1)
         t_gen = time.perf_counter() - t0
         Ep, M = len(d["img1"]), len(d["matches"])
 

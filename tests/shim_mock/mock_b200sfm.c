@@ -127,6 +127,12 @@ int b200sfm_ba_problem_get_sensor_poses(b200sfm_ba_problem* p, double* q, double
   }
   return B200SFM_OK;
 }
+int b200sfm_ba_problem_set_images(b200sfm_ba_problem* p, int32_t I, const int32_t* image_frame, const int32_t* image_sensor) {
+  (void)p;
+  dump_call("ba_problem_set_images");
+  DUMP_INT("image_frame", image_frame, I); DUMP_INT("image_sensor", image_sensor, I);
+  return B200SFM_OK;
+}
 int b200sfm_ba_problem_normalize(b200sfm_ba_problem* p, int32_t fixed_scale, double extent, double p0, double p1, double* sc,
                                  double* t) {
   (void)p; (void)fixed_scale; (void)extent; (void)p0; (void)p1;

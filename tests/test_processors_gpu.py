@@ -5,6 +5,8 @@ import numpy as np
 import pytest
 
 from glomap_b200 import estimators as E, geometry as G, processors as PR, synthetic as S
+from oracle import filter_oracle as FO
+from test_filters_cpu import ALL_CAMERAS, _params, centres_scene, missing_sensor_rig_scene, rig_dataset_scene, sweep_pixels
 
 pytestmark = pytest.mark.gpu
 
@@ -70,3 +72,63 @@ def test_normalize_rig_problem_scales_cam_from_rig():
     sq, st = prob.get_sensor_poses()
     assert np.abs(st - ref.sensor_trans).max() < 1e-12
     prob.free()
+
+
+# ---- undistortion against the exact inverse ---------------------------------------------------------------------------
+@pytest.mark.parametrize("model,k1,k2", ALL_CAMERAS)
+def test_undistort_is_the_exact_inverse_up_to_the_fold(model, k1, k2):
+    """Pixels from the centre out to where d/dr [r d(r^2)] falls to 0.05, plus the image box: bearings within 1e-12 of
+    the long-double inverse, and within 1e-14 of the host restatement.  (Past the fold there is no inverse; what the
+    kernel returns there is not pinned.)"""
+    p = _params(model, 1000.0, 500.0, k1, k2)
+    xy = sweep_pixels(model, p)
+    n = len(xy)
+    sc = S.Scene(np.array([[0.0, 0, 0, 1]]), np.array([[0.0, 0, 5]]), np.zeros((1, 3)), np.array([0, n]),
+                 np.zeros(n, np.int32), xy, np.zeros(1, np.int32), np.array([model], np.int32), p[None])
+    prob = _problem(sc)
+    got = prob.undistort()
+    prob.free()
+    want = FO.bearings_exact(model, p, xy).astype(np.float64)
+    assert np.abs(got - want).max() <= 1e-12, np.abs(got - want).max()
+    assert np.abs(got - PR.undistort_images(sc)).max() <= 1e-14
+
+
+# ---- normalisation over image counts, offsets, duplicates and rig tables ---------------------------------------------
+def _compare_normalize(sc, fixed_scale=False, min_views=3):
+    prob = E.BAProblem(E.default_context(), sc, min_views, E.first_frame_mask(sc.C))
+    try:
+        prob.set_state(sc.intr_params, sc.quat, sc.trans, sc.points)
+        ref = sc.copy()
+        s_ref, t_ref = PR.normalize_reconstruction(ref, fixed_scale=fixed_scale)
+        s_dev, t_dev = prob.normalize(fixed_scale=fixed_scale)
+        assert abs(s_dev - s_ref) <= 1e-12 * s_ref and np.abs(t_dev - t_ref).max() <= 1e-10 * max(1.0, np.abs(t_ref).max())
+        _, _, t, X = prob.get_state()
+        assert np.abs(t - ref.trans).max() < 1e-9 and np.abs(X - ref.points).max() < 1e-9
+        if hasattr(sc, "obs_sensor"):
+            assert np.abs(prob.get_sensor_poses()[1] - ref.sensor_trans).max() < 1e-12
+    finally:
+        prob.free()
+    return s_ref
+
+
+@pytest.mark.parametrize("fixed_scale", [False, True])
+@pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 330, 100_000])
+def test_normalize_matches_host_for_every_image_count(n, fixed_scale):
+    """1-3 images use the whole range; 330 images trim to 265 (more than one per thread of the 256-thread block sum)."""
+    _compare_normalize(centres_scene(n, seed=n), fixed_scale, min_views=1)
+
+
+@pytest.mark.parametrize("kw", [dict(offset=1e4), dict(duplicate=True)])
+def test_normalize_offset_and_duplicate_centres(kw):
+    """Centres near 1e4 (the float coordinates round at 1e-3); all centres at one point (zero extent: scale stays 1)."""
+    s = _compare_normalize(centres_scene(50, seed=5, **kw), min_views=1)
+    assert (s == 1.0) == bool(kw.get("duplicate"))
+
+
+@pytest.mark.parametrize("fixed_scale", [False, True])
+@pytest.mark.parametrize("which", ["rig_dataset", "missing_sensor"])
+def test_normalize_rigs_over_the_image_table(which, fixed_scale):
+    """Three rigs (36 images of 108 frame-sensor combinations) and a dense rig with missing images: the box and the mean
+    run over the images of the table, which BAProblem passes with b200sfm_ba_problem_set_images."""
+    sc = rig_dataset_scene()[0] if which == "rig_dataset" else missing_sensor_rig_scene()[0]
+    _compare_normalize(sc, fixed_scale)
