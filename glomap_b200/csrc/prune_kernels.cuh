@@ -231,16 +231,10 @@ struct PruneRunner {
     cub::DeviceSelect::Flagged(tmp.p, nb, in, flags, out, d_n, (int)n, s);
     return read(d_n);
   }
-  // union of the M endpoint pairs ends[e], ends[M + e] into parent (trk_hook sweeps until nothing changes), then flatten
+  // union of the M endpoint pairs ends[e], ends[M + e] into parent (trk_sweep), then flatten (trk_flatten)
   void unite(const int* ends, long long M, int* parent, int F, int* changed) {
-    if (M > 0) {
-      for (int sweep = 0; sweep < 64; ++sweep) {
-        B200_CUDA_OK(cudaMemsetAsync(changed, 0, sizeof(int), s));
-        B200_LAUNCH(ctx, trk_hook, cdiv(M, 256), 256, 0, M, ends, parent, changed);
-        if (!read(changed)) break;
-      }
-    }
-    B200_LAUNCH(ctx, trk_flatten, cdiv(F, 256), 256, 0, (long long)F, parent);
+    trk_sweep(ctx, M, ends, parent, changed);
+    trk_flatten(ctx, (long long)F, parent, changed);
   }
   // the endpoint array [lo..., hi...] of the selected edges of ends [2E]
   long long compact_ends(const int* ends, long long E, const unsigned char* sel, int* out, int* d_n) {

@@ -4,15 +4,19 @@
 //   1. nodes = sorted unique global feature ids (image_id << 32 | feature_id, :48-53) of both endpoints  (radix sort)
 //   2. endpoints -> node indices (binary search), pixel of every node from any match that touches it
 //   3. connected components: lock-free union-find (compare-and-swap hooking of roots, path halving), swept until a pass
-//      changes nothing; the
-//      nodes are sorted by id, so the root of a component is its SMALLEST global id -- the reference's rule (:56-60)
+//      changes nothing (trk_sweep: two sweeps; a cap reached is an error, not a partial union), then flattened by
+//      pointer jumping (trk_flatten); the nodes are sorted
+//      by id, so the root of a component is its SMALLEST global id (the reference's root depends on the match order;
+//      the smallest id is its canonical form)
 //   4. stable sort of the nodes by root -> tracks in ascending track id, observations of a track in ascending global id
 //   5. a track is discarded (observations cleared, id kept, :118-131) when two of its features inside ONE image are
-//      further apart than thres_inconsistency pixels
+//      further apart than thres_inconsistency pixels: (feature - other).norm() > thres, i.e.
+//      sqrt(fl(fl(dx * dx) + fl(dy * dy))) > thres in FP64, the rounding pinned so no FMA contraction moves the bound
 // The selection FindTracksForProblem (:153-227) is track_select_kernels.cuh.
 #pragma once
 #include <cub/cub.cuh>
 
+#include <stdexcept>
 #include <vector>
 
 #include "context.cuh"
@@ -64,19 +68,62 @@ __global__ void trk_hook(long long M, const int* __restrict__ ep_node, int* __re
     rb = trk_find(parent, rb);
   }
 }
-__global__ void trk_flatten(long long n, int* __restrict__ parent) {
+// one round of pointer jumping: parent[i] <- parent[parent[i]].  Thread i is the only writer of parent[i], so no store
+// can put back an older ancestor; a find with path halving here could (its halving store to a node may land after that
+// node's own root store), leaving a node pointing at a non-root and its component split in two tracks.
+__global__ void trk_jump(long long n, int* __restrict__ parent, int* __restrict__ changed) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) parent[i] = trk_find(parent, (int)i);
+  if (i >= n) return;
+  const int p = parent[i], g = parent[p];
+  if (g != p) {
+    parent[i] = g;
+    *changed = 1;
+  }
 }
 // nodes sorted by (root, id): head flags of the tracks
 __global__ void trk_track_heads(long long n, const int* __restrict__ root_sorted, int* __restrict__ flags) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) flags[i] = (i == 0 || root_sorted[i] != root_sorted[i - 1]) ? 1 : 0;
 }
-// inconsistency: node i against the following nodes of the same track AND image (adjacent: sorted by global id)
+// Union of the M endpoint pairs ends[e], ends[M + e] into parent: trk_hook sweeps until one changes nothing; returns the
+// number of sweeps.  trk_hook retries until both ends of its match share a root, so the first sweep joins every match
+// and the second finds nothing to do.  A sweep that still changes something at the cap can only be a defect: it throws
+// (the call fails) instead of leaving a partial union behind as wrong tracks or clusters.
+inline int trk_sweep(b200sfm_ctx* ctx, long long M, const int* ends, int* parent, int* changed) {
+  constexpr int kMaxSweeps = 64;
+  if (M <= 0) return 0;
+  cudaStream_t s = ctx->stream;
+  for (int sweep = 1; sweep <= kMaxSweeps; ++sweep) {
+    B200_CUDA_OK(cudaMemsetAsync(changed, 0, sizeof(int), s));
+    B200_LAUNCH(ctx, trk_hook, cdiv(M, 256), 256, 0, M, ends, parent, changed);
+    int h_changed = 0;
+    B200_CUDA_OK(cudaMemcpyAsync(&h_changed, changed, sizeof(int), cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    if (!h_changed) return sweep;
+  }
+  throw std::runtime_error("union-find still changing after 64 sweeps");
+}
+// parent[i] <- the root of i for all n nodes: trk_jump until a round changes nothing (at most ~log2(depth) + 1 rounds;
+// a 2^31-deep tree needs 32, so 64 rounds still changing is a defect and throws)
+inline void trk_flatten(b200sfm_ctx* ctx, long long n, int* parent, int* changed) {
+  constexpr int kMaxRounds = 64;
+  if (n <= 0) return;
+  cudaStream_t s = ctx->stream;
+  for (int round = 0; round < kMaxRounds; ++round) {
+    B200_CUDA_OK(cudaMemsetAsync(changed, 0, sizeof(int), s));
+    B200_LAUNCH(ctx, trk_jump, cdiv(n, 256), 256, 0, n, parent, changed);
+    int h_changed = 0;
+    B200_CUDA_OK(cudaMemcpyAsync(&h_changed, changed, sizeof(int), cudaMemcpyDeviceToHost, s));
+    B200_CUDA_OK(cudaStreamSynchronize(s));
+    if (!h_changed) return;
+  }
+  throw std::runtime_error("union-find flattening still changing after 64 rounds");
+}
+// inconsistency: node i against the following nodes of the same track AND image (adjacent: sorted by global id), decided
+// as the reference's (feature - other).norm() > thres: both squares and their sum rounded on their own, then sqrt
 __global__ void trk_inconsistent(long long n, const int* __restrict__ root_sorted, const int* __restrict__ node_sorted,
                                  const int* __restrict__ track_of, const unsigned long long* __restrict__ node_gid,
-                                 const double2* __restrict__ node_xy, double thres2, int* __restrict__ bad) {
+                                 const double2* __restrict__ node_xy, double thres, int* __restrict__ bad) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int ni = node_sorted[i];
@@ -86,7 +133,7 @@ __global__ void trk_inconsistent(long long n, const int* __restrict__ root_sorte
     const int nj = node_sorted[j];
     if ((unsigned)(node_gid[nj] >> 32) != img) break;
     const double dx = node_xy[nj].x - a.x, dy = node_xy[nj].y - a.y;
-    if (dx * dx + dy * dy > thres2) { bad[track_of[i] - 1] = 1; break; }
+    if (sqrt(__dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy))) > thres) { bad[track_of[i] - 1] = 1; break; }
   }
 }
 // per track: id = smallest global id, kept length
@@ -171,15 +218,8 @@ struct b200sfm_tracks {
     DevBuf<int> parent, changed;
     parent.alloc(n_nodes); changed.alloc(1);
     B200_LAUNCH(ctx, trk_iota, cdiv(n_nodes, 256), 256, 0, n_nodes, parent.p);
-    for (sweeps = 0; sweeps < 64; ++sweeps) {
-      changed.zero(s);
-      B200_LAUNCH(ctx, trk_hook, cdiv(M, 256), 256, 0, M, ep_node.p, parent.p, changed.p);
-      int h_changed = 0;
-      B200_CUDA_OK(cudaMemcpyAsync(&h_changed, changed.p, sizeof(int), cudaMemcpyDeviceToHost, s));
-      B200_CUDA_OK(cudaStreamSynchronize(s));
-      if (!h_changed) break;
-    }
-    B200_LAUNCH(ctx, trk_flatten, cdiv(n_nodes, 256), 256, 0, n_nodes, parent.p);
+    sweeps = trk_sweep(ctx, M, ep_node.p, parent.p, changed.p);
+    trk_flatten(ctx, n_nodes, parent.p, changed.p);
     // tracks: stable sort of the (id-sorted) nodes by root
     DevBuf<int> node_idx, root_sorted, node_sorted, tflags, track_of;
     node_idx.alloc(n_nodes); root_sorted.alloc(n_nodes); node_sorted.alloc(n_nodes); tflags.alloc(n_nodes); track_of.alloc(n_nodes);
@@ -199,7 +239,7 @@ struct b200sfm_tracks {
     track_id.alloc(T); begin.alloc((size_t)T + 1);
     bad.zero(s);
     B200_LAUNCH(ctx, trk_inconsistent, cdiv(n_nodes, 256), 256, 0, n_nodes, root_sorted.p, node_sorted.p, track_of.p, node_gid.p, node_xy.p,
-                thres * thres, bad.p);
+                thres, bad.p);
     B200_LAUNCH(ctx, trk_track_table, cdiv(n_nodes, 256), 256, 0, n_nodes, T, tflags.p, track_of.p, node_sorted.p, node_gid.p, track_id.p,
                 track_start.p);
     B200_LAUNCH(ctx, trk_kept_len, cdiv(T + 1, 256), 256, 0, T, track_start.p, bad.p, len.p);

@@ -4,7 +4,10 @@
 * ``establish_full_tracks``  = EstablishFullTracks (:5-17): union-find over the inlier matches of the valid image
   pairs (BlindConcatenation :19-63; here connected components of the match graph), then TrackCollection (:65-150):
   a track whose features inside ONE image are further apart than ``thres_inconsistency`` pixels is discarded (its
-  observation list is cleared, the track id stays, as in the reference).
+  observation list is cleared, the track id stays, as in the reference).  "Further apart" is the reference's
+  ``(feature - other).norm() > thres`` in FP64, ``sqrt(fl(fl(dx*dx) + fl(dy*dy))) > thres`` (``inconsistent``): not
+  the squared form ``dx*dx + dy*dy > thres*thres``, which decides differently at the bound (dx = 10, dy = 1.2e-7 is
+  kept at thres = 10), and never fused into an FMA.
 * ``find_tracks_for_problem`` = FindTracksForProblem (:153-234): tracks sorted by (length, id) descending, too short /
   too long ones skipped, observations restricted to registered images, greedy per-camera quota
   ``min_num_tracks_per_view`` -- compared as an UNSIGNED 64-bit value exactly like the reference (``track_t`` counters
@@ -80,62 +83,8 @@ def _global_ids(pairs):
     return np.concatenate(g1), np.concatenate(g2)
 
 
-def establish_full_tracks(pairs, features: dict, options: TrackEstablishmentOptions | None = None):
-    """Returns (Tracks, number of tracks discarded for inconsistency).  ``features[image_id]`` is the [n,2] pixel table
-    (Image::features)."""
-    o = options or TrackEstablishmentOptions()
-    g1, g2 = _global_ids(pairs)
-    nodes, inv = np.unique(np.concatenate([g1, g2]), return_inverse=True)
-    n = len(nodes)
-    if n == 0:
-        return Tracks(np.zeros(0, np.uint64), np.zeros(1, np.int64), np.zeros(0, np.uint32), np.zeros(0, np.uint32)), 0
-    a, b = inv[:len(g1)], inv[len(g1):]
-    ncomp, lab = connected_components(sp.coo_matrix((np.ones(len(a), np.int8), (a, b)), shape=(n, n)), directed=False)
-    order = np.lexsort((nodes, lab))                       # by component, then by global id
-    lab_s, nodes_s = lab[order], nodes[order]
-    starts = np.concatenate([[0], np.nonzero(np.diff(lab_s))[0] + 1, [n]])
-    track_ids = nodes_s[starts[:-1]]                        # smallest global id of each component
-    img = (nodes_s >> np.uint64(32)).astype(np.uint32)
-    feat = (nodes_s & np.uint64(0xFFFFFFFF)).astype(np.uint32)
-    # consistency: inside a track, features of one image must lie within thres_inconsistency of each other (:118-131)
-    keep = np.ones(ncomp, bool)
-    same = (lab_s[1:] == lab_s[:-1]) & (img[1:] == img[:-1])        # (sorted by gid => same-image features are adjacent)
-    discarded = 0
-    comp_label = lab_s[starts[:-1]]                         # ascending (lexsort by label)
-    for t in np.unique(lab_s[1:][same]):
-        ti = int(np.searchsorted(comp_label, t))
-        s, e = int(starts[ti]), int(starts[ti + 1])
-        im_t, ft_t = img[s:e], feat[s:e]
-        bad = False
-        for im in np.unique(im_t[np.concatenate([[False], im_t[1:] == im_t[:-1]])]):
-            xy = np.asarray(features[int(im)], dtype=np.float64)[ft_t[im_t == im]]
-            d = np.linalg.norm(xy[:, None, :] - xy[None, :, :], axis=-1)
-            if (d > o.thres_inconsistency).any():
-                bad = True
-                break
-        if bad:
-            keep[ti] = False
-            discarded += 1
-    lens = np.diff(starts)
-    lens_kept = np.where(keep, lens, 0)
-    sel = np.repeat(keep, lens)
-    # component order above is by label; present the tracks in ascending track id
-    perm = np.argsort(track_ids, kind="stable")
-    begin = np.concatenate([[0], np.cumsum(lens_kept[perm])]).astype(np.int64)
-    pos = np.concatenate([np.arange(starts[t], starts[t + 1]) for t in perm if keep[t]]) if sel.any() else np.zeros(0, np.int64)
-    return Tracks(track_ids[perm], begin, img[pos], feat[pos]), discarded
-
-
-def establish_full_tracks_device(pairs, features: dict, options: TrackEstablishmentOptions | None = None, ctx=None):
-    """EstablishFullTracks on the GPU (b200sfm_tracks_establish: union-find, track collection, inconsistency rule); same
-    return value as ``establish_full_tracks``.  The host only concatenates the inlier matches of the valid pairs."""
-    import ctypes as ct
-
-    from . import _lib, estimators as E
-    o = options or TrackEstablishmentOptions()
-    ctx = ctx or E.default_context()
-    g1, g2 = _global_ids(pairs)
-    M = len(g1)
+def _match_pixels(pairs, features: dict, M: int):
+    """(xy1, xy2) [M,2]: the pixels of both features of every inlier match of the valid pairs, in ``_global_ids`` order."""
     xy1, xy2 = np.empty((M, 2)), np.empty((M, 2))
     pos = 0
     for p in pairs:
@@ -146,13 +95,107 @@ def establish_full_tracks_device(pairs, features: dict, options: TrackEstablishm
         xy1[pos:pos + k] = np.asarray(features[int(p.image_id1)], dtype=np.float64)[m[:, 0]]
         xy2[pos:pos + k] = np.asarray(features[int(p.image_id2)], dtype=np.float64)[m[:, 1]]
         pos += k
+    return xy1, xy2
+
+
+def inconsistent(dx, dy, thres):
+    """The reference's inconsistency decision ``(feature - other).norm() > thres`` (:127-128) in FP64: both squares and
+    their sum rounded on their own (no fused multiply-add), then sqrt.  Elementwise over arrays."""
+    return np.sqrt(np.multiply(dx, dx) + np.multiply(dy, dy)) > thres
+
+
+def _far_groups(xy, gstart, gend, thres, pairs_per_batch=1 << 24):
+    """bool per group [gstart[g], gend[g]) of ``xy``: does any two of its pixels decide ``inconsistent``?  A group whose
+    bounding box does not is consistent: |fl(a - b)| <= fl(max - min) per axis and rounding, squares, sum and sqrt are
+    monotone, so no pair decides more than the box.  The others are checked pair by pair, in batches."""
+    far = np.zeros(len(gstart), bool)
+    if len(gstart) == 0:
+        return far
+    x, y = xy[:, 0], xy[:, 1]
+    box = inconsistent(np.maximum.reduceat(x, gstart) - np.minimum.reduceat(x, gstart),
+                       np.maximum.reduceat(y, gstart) - np.minimum.reduceat(y, gstart), thres)
+    # reduceat runs each group to the next group's start; groups here are contiguous and cover [gstart[0], gend[-1])
+    g = np.nonzero(box)[0]
+    if len(g) == 0:
+        return far
+    lens = gend[g] - gstart[g]
+    elem = np.repeat(gstart[g] - np.concatenate([[0], np.cumsum(lens)[:-1]]), lens) + np.arange(lens.sum())
+    grp = np.repeat(g, lens)
+    cnt = np.repeat(gend[g], lens) - elem - 1                 # partners after each element inside its group
+    cum = np.cumsum(cnt)
+    lo = 0
+    while lo < len(elem):
+        hi = max(int(np.searchsorted(cum, (cum[lo - 1] if lo else 0) + pairs_per_batch, side="right")), lo + 1)
+        c = cnt[lo:hi]
+        i = np.repeat(elem[lo:hi], c)
+        j = i + 1 + np.arange(c.sum()) - np.repeat(np.cumsum(c) - c, c)
+        hit = inconsistent(x[j] - x[i], y[j] - y[i], thres)
+        far[np.repeat(grp[lo:hi], c)[hit]] = True
+        lo = hi
+    return far
+
+
+def establish_tracks_from_matches(g1, g2, xy1, xy2, thres_inconsistency: float = 10.0):
+    """``establish_full_tracks`` on the concatenated inlier matches: global ids ``g1``, ``g2`` [M] and their pixels
+    ``xy1``, ``xy2`` [M,2] (the input of b200sfm_tracks_establish).  Returns (Tracks, number discarded)."""
+    g1, g2 = np.asarray(g1, np.uint64), np.asarray(g2, np.uint64)
+    nodes, first, inv = np.unique(np.concatenate([g1, g2]), return_index=True, return_inverse=True)
+    n = len(nodes)
+    if n == 0:
+        return Tracks(np.zeros(0, np.uint64), np.zeros(1, np.int64), np.zeros(0, np.uint32), np.zeros(0, np.uint32)), 0
+    node_xy = np.concatenate([np.asarray(xy1, np.float64).reshape(-1, 2), np.asarray(xy2, np.float64).reshape(-1, 2)])[first]
+    a, b = inv[:len(g1)], inv[len(g1):]
+    ncomp, lab = connected_components(sp.coo_matrix((np.ones(len(a), np.int8), (a, b)), shape=(n, n)), directed=False)
+    # renumber the components by their smallest global id (the nodes are sorted): tracks in ascending track id
+    _, comp_first = np.unique(lab, return_index=True)
+    rank = np.empty(ncomp, np.int64)
+    rank[np.argsort(comp_first, kind="stable")] = np.arange(ncomp)
+    order = np.argsort(rank[lab], kind="stable")            # by track, then by global id
+    lab_s, nodes_s, xy_s = rank[lab][order], nodes[order], node_xy[order]
+    starts = np.concatenate([[0], np.nonzero(np.diff(lab_s))[0] + 1, [n]])
+    track_ids = nodes_s[starts[:-1]]                        # smallest global id of each component
+    img = (nodes_s >> np.uint64(32)).astype(np.uint32)
+    feat = (nodes_s & np.uint64(0xFFFFFFFF)).astype(np.uint32)
+    # consistency: inside a track, features of one image must lie within thres_inconsistency of each other (:118-131);
+    # sorted by global id, the features of one (track, image) are adjacent
+    gstart = np.concatenate([[0], np.nonzero((lab_s[1:] != lab_s[:-1]) | (img[1:] != img[:-1]))[0] + 1])
+    gend = np.concatenate([gstart[1:], [n]])
+    multi = gend - gstart > 1
+    keep = np.ones(ncomp, bool)
+    far = _far_groups(xy_s, gstart, gend, thres_inconsistency)
+    keep[lab_s[gstart[multi & far]]] = False
+    lens_kept = np.where(keep, np.diff(starts), 0)
+    begin = np.concatenate([[0], np.cumsum(lens_kept)]).astype(np.int64)
+    pos = np.nonzero(keep[lab_s])[0]
+    return Tracks(track_ids, begin, img[pos], feat[pos]), int(ncomp - keep.sum())
+
+
+def establish_full_tracks(pairs, features: dict, options: TrackEstablishmentOptions | None = None):
+    """Returns (Tracks, number of tracks discarded for inconsistency).  ``features[image_id]`` is the [n,2] pixel table
+    (Image::features)."""
+    o = options or TrackEstablishmentOptions()
+    g1, g2 = _global_ids(pairs)
+    xy1, xy2 = _match_pixels(pairs, features, len(g1))
+    return establish_tracks_from_matches(g1, g2, xy1, xy2, o.thres_inconsistency)
+
+
+def establish_tracks_from_matches_device(g1, g2, xy1, xy2, thres_inconsistency: float = 10.0, ctx=None):
+    """``establish_tracks_from_matches`` on the GPU (b200sfm_tracks_establish: union-find, track collection,
+    inconsistency rule); same return value."""
+    import ctypes as ct
+
+    from . import _lib, estimators as E
+    ctx = ctx or E.default_context()
     g1, g2 = np.ascontiguousarray(g1, np.uint64), np.ascontiguousarray(g2, np.uint64)
+    M = len(g1)
+    xy1 = np.ascontiguousarray(np.asarray(xy1, np.float64).reshape(M, 2))
+    xy2 = np.ascontiguousarray(np.asarray(xy2, np.float64).reshape(M, 2))
     h = ct.c_void_p()
     nt, nobs, ndis = ct.c_int64(), ct.c_int64(), ct.c_int64()
     ptr = lambda a: a.ctypes.data_as(ct.c_void_p) if len(a) else None   # noqa: E731
     _lib.check(ctx.handle, ctx.lib.b200sfm_tracks_establish(ctx.handle, M, ptr(g1), ptr(g2), ptr(xy1), ptr(xy2),
-                                                            float(o.thres_inconsistency), ct.byref(h), ct.byref(nt), ct.byref(nobs),
-                                                            ct.byref(ndis)))
+                                                            float(thres_inconsistency), ct.byref(h), ct.byref(nt),
+                                                            ct.byref(nobs), ct.byref(ndis)))
     try:
         T, n = nt.value, nobs.value
         ids, begin = np.zeros(T, np.uint64), np.zeros(T + 1, np.int64)
@@ -161,6 +204,15 @@ def establish_full_tracks_device(pairs, features: dict, options: TrackEstablishm
     finally:
         ctx.lib.b200sfm_tracks_free(h)
     return Tracks(ids, begin, img, feat), int(ndis.value)
+
+
+def establish_full_tracks_device(pairs, features: dict, options: TrackEstablishmentOptions | None = None, ctx=None):
+    """EstablishFullTracks on the GPU (b200sfm_tracks_establish: union-find, track collection, inconsistency rule); same
+    return value as ``establish_full_tracks``.  The host only concatenates the inlier matches of the valid pairs."""
+    o = options or TrackEstablishmentOptions()
+    g1, g2 = _global_ids(pairs)
+    xy1, xy2 = _match_pixels(pairs, features, len(g1))
+    return establish_tracks_from_matches_device(g1, g2, xy1, xy2, o.thres_inconsistency, ctx)
 
 
 def find_tracks_for_problem(tracks: Tracks, registered_images, options: TrackEstablishmentOptions | None = None) -> Tracks:
