@@ -169,6 +169,7 @@ PROTOTYPES = {
     "b200sfm_ba_problem_filter_triangulation_angle": (c_int32, [c_void_p, c_double, c_void_p, P(c_int64)]),
     "b200sfm_ba_problem_normalize": (c_int32, [c_void_p, c_int32, c_double, c_double, c_double, P(c_double), c_void_p]),
     "b200sfm_ba_problem_undistort": (c_int32, [c_void_p, c_void_p]),
+    "b200sfm_undistort_features": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_int64, c_void_p, c_void_p, c_void_p]),
     "b200sfm_tracks_establish": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_double, P(c_void_p),
                                            P(c_int64), P(c_int64), P(c_int64)]),
     "b200sfm_tracks_get": (c_int32, [c_void_p] * 5),

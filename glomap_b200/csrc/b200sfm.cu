@@ -508,6 +508,26 @@ int b200sfm_ba_problem_filter_triangulation_angle(b200sfm_ba_problem* p, double 
   });
 }
 
+int b200sfm_undistort_features(b200sfm_ctx* ctx, int32_t K, const int32_t* intr_model, const double* intr_params, int64_t n,
+                               const int32_t* feat_intr, const double* xy, double* bearings_out) {
+  if (!ctx || K < 0 || n < 0) return B200SFM_ERR_INVALID_ARG;
+  if (n == 0) return B200SFM_OK;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if ((K > 0 && (!intr_model || !intr_params)) || !feat_intr || !xy || !bearings_out) return invalid("null argument");
+  if (K == 0) return invalid("feature camera block outside [0, K)");
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    const int r = b200::undistort_features(ctx, K, intr_model, intr_params, n, feat_intr, xy, bearings_out);
+    if (r & 1) throw b200::InvalidInput{"feature camera block outside [0, K)"};
+    if (r & 2) {
+      ctx->err = "camera model outside 0-3";
+      return (int)B200SFM_ERR_UNSUPPORTED;
+    }
+    B200_CUDA_OK(cudaGetLastError());
+    return (int)B200SFM_OK;
+  });
+}
+
 // ---- test probe (include/b200sfm_testing.h) ----------------------------------------------------------------------
 int b200sfm_test_ba_step(b200sfm_ba_problem* p, const b200sfm_ba_opts* opts, double first_radius, double radius,
                          b200sfm_test_ba_step_out* out) {

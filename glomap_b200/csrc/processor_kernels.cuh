@@ -7,9 +7,11 @@
 //     problem that is three small kernels instead of a download / upload of the whole state.
 //   * UndistortImages (glomap/processors/image_undistorter.cc:7-53): pixel -> unit bearing per observation,
 //     CamFromImg(xy).homogeneous().normalized().  Radial models are inverted on the radius with a safeguarded Newton
-//     iteration, the same steps as the host restatement (glomap_b200/synthetic.py bearings_from_pixels).
+//     iteration, the same steps as the host restatement (glomap_b200/synthetic.py bearings_from_pixels).  The same
+//     per pixel over Image::features, outside a BA problem: proc_undistort_features (b200sfm_undistort_features).
 #pragma once
 #include "ba_kernels.cuh"
+#include "context.cuh"
 
 namespace b200 {
 
@@ -152,6 +154,41 @@ __global__ void proc_undistort(long long N, int S, const int* __restrict__ obs_c
   if (o >= N) return;
   const int blk = S > 0 ? sensor_intr[obs_sensor[o]] : cam_intr[obs_cam[o]];
   bearing_from_pixel(intr_model[blk], intr + (size_t)blk * 12, obs_xy[o], out + 3 * o);
+}
+
+// unit bearing of every feature (UndistortImages over Image::features, b200sfm_undistort_features); a block index outside
+// [0, K) sets bit 0 of err, a camera model outside 0-3 bit 1, and the feature is then not written
+__global__ void proc_undistort_features(long long n, int K, const int* __restrict__ feat_intr, const int* __restrict__ intr_model,
+                                        const double* __restrict__ intr /*[K][12]*/, const double2* __restrict__ xy,
+                                        double* __restrict__ out, int* __restrict__ err) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int blk = feat_intr[i];
+  if (blk < 0 || blk >= K) { atomicOr(err, 1); return; }
+  const int m = intr_model[blk];
+  if (m < 0 || m > 3) { atomicOr(err, 2); return; }
+  bearing_from_pixel(m, intr + (size_t)blk * 12, xy[i], out + 3 * i);
+}
+
+// host side of b200sfm_undistort_features: 0 = bearings written to h_out, else the err bits of the kernel (h_out untouched)
+inline int undistort_features(b200sfm_ctx* ctx, int K, const int* h_model, const double* h_intr, long long n, const int* h_feat_intr,
+                              const double* h_xy, double* h_out) {
+  cudaStream_t s = ctx->stream;
+  DevBuf<int> model, feat_intr, err;
+  DevBuf<double> intr, out;
+  DevBuf<double2> xy;
+  model.alloc(K); intr.alloc((size_t)K * 12); feat_intr.alloc(n); xy.alloc(n); out.alloc(3 * (size_t)n); err.alloc(1);
+  model.upload(h_model, K, s); intr.upload(h_intr, (size_t)K * 12, s); feat_intr.upload(h_feat_intr, n, s);
+  xy.upload(reinterpret_cast<const double2*>(h_xy), n, s);
+  err.zero(s);
+  B200_LAUNCH(ctx, proc_undistort_features, cdiv(n, 256), 256, 0, n, K, feat_intr.p, model.p, intr.p, xy.p, out.p, err.p);
+  int h_err = 0;
+  B200_CUDA_OK(cudaMemcpyAsync(&h_err, err.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  B200_CUDA_OK(cudaStreamSynchronize(s));
+  if (h_err) return h_err;
+  out.download(h_out, 3 * (size_t)n, s);
+  B200_CUDA_OK(cudaStreamSynchronize(s));
+  return 0;
 }
 
 }  // namespace b200

@@ -23,6 +23,7 @@
 #include <random>
 #include <string>
 #include <type_traits>
+#include <unordered_map>
 #include <vector>
 
 #include "../../include/b200sfm.h"
@@ -1891,5 +1892,406 @@ inline bool SolveRotationAveraging(ViewGraph& view_graph, std::unordered_map<rig
   KeepLargestConnectedComponents(view_graph, frames, images);                                 // .cc:195
   return ok;
 }
+
+// ---------------------------------------------------------------------------
+// The processors GlobalMapper::Solve runs between its solvers (controllers/global_mapper.cc:62,155-186,231-337) on the
+// device.  Each call stands alone: it flattens the maps in sorted-id order, runs the device and writes back only what the
+// reference writes.  A call that fails -- a failed device call, an observation of an unknown image, an image of an unknown
+// camera or without a posed frame, a feature outside its image, a rig sensor without cam_from_rig, a camera model outside
+// 0-3 where the intrinsics are read -- prints a message on stderr and changes nothing.
+namespace processors_detail {
+
+// The tracks' observations as a device problem: trivial frames -> one pose block per image (b200sfm_ba_problem_create),
+// otherwise frames plus (rig, camera) sensors (b200sfm_ba_problem_create_rig).  Only the pixel filter reads intrinsics
+// (`pixels`); the other filters get one placeholder SIMPLE_PINHOLE block, so that a camera model they never read cannot
+// refuse them.  `cameras` null: the filter reads no camera at all (no calibration flag either).
+struct FlatTracks {
+  bool rig = false;
+  int32_t F = 0, S = 0, K = 0, P = 0;
+  std::vector<int64_t> ptb{0};
+  std::vector<int32_t> obs_frame, cam_intr, sensor_intr, intr_model;
+  std::vector<uint16_t> obs_sensor;
+  std::vector<double> obs_xy, bearings, quat, trans, sensor_q, sensor_t, intr, points;
+  std::vector<uint8_t> calibrated;   // has_prior_focal_length per pose block (trivial frames) or per sensor (rigs)
+  int64_t N() const { return (int64_t)obs_frame.size(); }
+};
+
+template <class CameraMap, class ImageMap, class TrackPtrs>
+bool Flatten(const CameraMap* cameras, const ImageMap& images, const TrackPtrs& tsorted, bool pixels, bool bearings,
+             FlatTracks& out) {
+  using Img = typename ImageMap::mapped_type;
+  auto fail = [](const char* msg) { std::fprintf(stderr, "b200sfm: %s\n", msg); return false; };
+  // pass 1: every observation is resolved to a record of its image with one hash lookup; an image is looked up in
+  // `images` and checked once, when it is first seen
+  struct Rec { image_t id; const Img* im; int32_t block = 0, sensor = 0; };
+  std::vector<Rec> recs;
+  std::unordered_map<image_t, int32_t> rec_of;
+  size_t n_obs = 0;
+  for (const auto& [id, t] : tsorted) n_obs += t->observations.size();
+  std::vector<int32_t> obs_rec;
+  obs_rec.reserve(n_obs);
+  for (const auto& [id, t] : tsorted)
+    for (const auto& ob : t->observations) {
+      auto r = rec_of.find(ob.first);
+      if (r == rec_of.end()) {
+        auto it = images.find(ob.first);
+        if (it == images.end()) return fail("track observation of an unknown image");
+        const Img& im = it->second;
+        if (!im.frame_ptr || !im.frame_ptr->HasPose()) return fail("image without a posed frame");
+        r = rec_of.emplace(ob.first, (int32_t)recs.size()).first;
+        recs.push_back(Rec{ob.first, &im});
+        out.rig = out.rig || !im.HasTrivialFrame();
+      }
+      const Img& im = *recs[r->second].im;
+      const size_t nf = bearings ? im.features_undist.size() : im.features.size();
+      if ((pixels || bearings) && (size_t)ob.second >= nf) return fail("track observation of a feature outside its image");
+      obs_rec.push_back(r->second);
+    }
+  // cameras of the observed images, in sorted camera-id order
+  std::map<camera_t, int32_t> cidx;
+  if (cameras)
+    for (const Rec& r : recs) {
+      if (cameras->find(r.im->camera_id) == cameras->end()) return fail("image of an unknown camera");
+      cidx[r.im->camera_id] = 0;
+    }
+  if (pixels) {
+    for (auto& [id, k] : cidx) {
+      const auto& c = cameras->at(id);
+      k = (int32_t)out.intr_model.size();
+      out.intr_model.push_back(static_cast<int32_t>(c.model_id));
+      out.intr.resize(out.intr.size() + B200SFM_INTR_STRIDE, 0.0);
+      for (size_t j = 0; j < c.params.size() && j < (size_t)B200SFM_INTR_STRIDE; ++j) out.intr[(size_t)k * B200SFM_INTR_STRIDE + j] = c.params[j];
+    }
+  } else {
+    out.intr_model.push_back(B200SFM_SIMPLE_PINHOLE);
+    out.intr.assign(B200SFM_INTR_STRIDE, 0.0);
+    out.intr[0] = 1.0;
+  }
+  out.K = (int32_t)out.intr_model.size();
+  auto block = [&](camera_t c) { return pixels ? cidx[c] : 0; };
+  auto prior = [&](camera_t c) -> uint8_t { return cameras && cameras->at(c).has_prior_focal_length ? 1 : 0; };
+  // pose blocks: the images (trivial frames) or their frames, in sorted id order
+  std::map<uint64_t, std::vector<Rec*>> by_block;
+  for (Rec& r : recs) by_block[out.rig ? (uint64_t)r.im->frame_id : (uint64_t)r.id].push_back(&r);
+  for (auto& [key, rs] : by_block) {
+    for (Rec* r : rs) r->block = out.F;
+    ++out.F;
+    const Img* im = rs.front()->im;
+    const auto& pose = im->frame_ptr->RigFromWorld();
+    for (int k = 0; k < 4; ++k) out.quat.push_back(pose.rotation.coeffs().data()[k]);
+    for (int k = 0; k < 3; ++k) out.trans.push_back(pose.translation[k]);
+    if (!out.rig) {
+      out.cam_intr.push_back(block(im->camera_id));
+      out.calibrated.push_back(prior(im->camera_id));
+    }
+  }
+  // rigs: the (rig, camera) sensors in sorted order; a reference sensor carries the identity
+  if (out.rig) {
+    std::map<std::pair<rig_t, camera_t>, std::vector<Rec*>> by_sensor;
+    for (Rec& r : recs) by_sensor[{r.im->frame_ptr->RigId(), r.im->camera_id}].push_back(&r);
+    for (auto& [key, rs] : by_sensor) {
+      for (Rec* r : rs) r->sensor = out.S;
+      ++out.S;
+      const Img* im = rs.front()->im;
+      Rigid3d cfr;   // identity
+      auto* rig = im->frame_ptr->RigPtr();
+      if (!im->HasTrivialFrame() && !(rig && b200host_adapt::IsRefSensor(*rig, key.second))) {
+        if (!rig || !b200host_adapt::HasCamFromRig(*rig, key.second)) return fail("image of a rig sensor without cam_from_rig");
+        cfr = b200host_adapt::CamFromRig(*rig, key.second);
+      }
+      for (int k = 0; k < 4; ++k) out.sensor_q.push_back(cfr.rotation.coeffs().data()[k]);
+      for (int k = 0; k < 3; ++k) out.sensor_t.push_back(cfr.translation[k]);
+      out.sensor_intr.push_back(block(key.second));
+      out.calibrated.push_back(prior(key.second));
+    }
+    if (out.S > 65535) return fail("too many rig sensors");
+  }
+  // pass 2: observations in track order from their records, points
+  out.obs_frame.resize(n_obs);
+  if (out.rig) out.obs_sensor.resize(n_obs);
+  out.obs_xy.assign(2 * n_obs, 0.0);
+  if (bearings) out.bearings.resize(3 * n_obs);
+  out.ptb.reserve(tsorted.size() + 1);
+  out.points.reserve(3 * tsorted.size());
+  size_t o = 0;
+  for (const auto& [id, t] : tsorted) {
+    for (const auto& ob : t->observations) {
+      const Rec& r = recs[obs_rec[o]];
+      out.obs_frame[o] = r.block;
+      if (out.rig) out.obs_sensor[o] = (uint16_t)r.sensor;
+      if (pixels) {
+        const auto& xy = r.im->features[ob.second];
+        out.obs_xy[2 * o] = xy[0];
+        out.obs_xy[2 * o + 1] = xy[1];
+      }
+      if (bearings) {
+        const auto& u = r.im->features_undist[ob.second];
+        for (int k = 0; k < 3; ++k) out.bearings[3 * o + k] = u[k];
+      }
+      ++o;
+    }
+    out.ptb.push_back((int64_t)o);
+    for (int k = 0; k < 3; ++k) out.points.push_back(t->xyz[k]);
+    ++out.P;
+  }
+  return true;
+}
+
+// Creates the problem of `f` and loads its state; min_num_view_per_track = 1 keeps every non-empty track in the problem
+// (the filters read every observation of every track, whatever its length).
+inline int CreateProblem(b200sfm_ctx* ctx, FlatTracks& f, b200sfm_ba_problem** prob) {
+  int rc;
+  if (f.rig)
+    rc = b200sfm_ba_problem_create_rig(ctx, f.F, f.P, f.N(), f.K, f.S, f.ptb.data(), f.obs_frame.data(), f.obs_sensor.data(),
+                                       f.obs_xy.data(), f.sensor_q.data(), f.sensor_t.data(), f.sensor_intr.data(),
+                                       f.intr_model.data(), nullptr, 1, prob);
+  else
+    rc = b200sfm_ba_problem_create(ctx, f.F, f.P, f.N(), f.K, f.ptb.data(), f.obs_frame.data(), f.obs_xy.data(), f.cam_intr.data(),
+                                   f.intr_model.data(), nullptr, 1, prob);
+  if (rc == B200SFM_OK) rc = b200sfm_ba_problem_set_state(*prob, f.intr.data(), f.quat.data(), f.trans.data(), f.points.data());
+  return rc;
+}
+
+// mode 0: pixel reprojection, 1: angle, 2: triangulation angle, 3: reprojection in the normalised image plane
+template <class CameraMap, class ImageMap, class TrackMap>
+int RunTrackFilter(int mode, const CameraMap* cameras, const ImageMap& images, TrackMap& tracks, double threshold, const char* name) {
+  using Trk = typename TrackMap::mapped_type;
+  std::vector<std::pair<track_t, Trk*>> tsorted;   // sorted track-id order
+  tsorted.reserve(tracks.size());
+  for (auto& [id, t] : tracks) tsorted.emplace_back(id, &t);
+  std::sort(tsorted.begin(), tsorted.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  if (tsorted.empty()) return 0;
+  FlatTracks f;
+  if (!Flatten(cameras, images, tsorted, mode == 0, mode == 1 || mode == 3, f)) return 0;
+  if (f.N() == 0) {   // no observation: nothing changes, except that every track fails the triangulation angle
+    if (mode != 2) return 0;
+    for (auto& [id, t] : tsorted) t->observations.clear();
+    return (int)tsorted.size();
+  }
+  b200sfm_ctx* ctx = DefaultContext();
+  if (!ctx) return 0;
+  b200sfm_ba_problem* prob = nullptr;
+  int rc = CreateProblem(ctx, f, &prob);
+  std::vector<uint8_t> keep(mode == 2 ? (size_t)f.P : (size_t)f.N());
+  int64_t n = 0;
+  if (rc == B200SFM_OK) {
+    if (mode == 0) rc = b200sfm_ba_problem_filter_reprojection(prob, threshold, keep.data(), &n);
+    if (mode == 1) rc = b200sfm_ba_problem_filter_angle(prob, f.bearings.data(), f.calibrated.data(), threshold, keep.data(), &n);
+    if (mode == 2) rc = b200sfm_ba_problem_filter_triangulation_angle(prob, threshold, keep.data(), &n);
+    if (mode == 3) rc = b200sfm_ba_problem_filter_reprojection_normalized(prob, f.bearings.data(), threshold, keep.data(), &n);
+  }
+  b200sfm_ba_problem_free(prob);
+  if (rc != B200SFM_OK) {
+    std::fprintf(stderr, "b200sfm: TrackFilter::%s failed: %s\n", name, b200sfm_last_error(ctx));
+    return 0;
+  }
+  int64_t p = 0;
+  for (auto& [id, t] : tsorted) {
+    if (mode == 2) {
+      if (!keep[p]) t->observations.clear();                                                  // track_filter.cc:118-121
+    } else {
+      const int64_t b = f.ptb[p], e = f.ptb[p + 1];
+      if (std::find(keep.begin() + b, keep.begin() + e, 0) != keep.begin() + e) {            // .cc:44-47
+        std::vector<std::pair<image_t, feature_t>> kept;
+        for (int64_t o = b; o < e; ++o)
+          if (keep[o]) kept.emplace_back(t->observations[o - b].first, t->observations[o - b].second);
+        t->observations.assign(kept.begin(), kept.end());
+      }
+    }
+    ++p;
+  }
+  return (int)n;
+}
+
+}  // namespace processors_detail
+
+// TrackFilter (processors/track_filter.{h,cc}) on the device: the tracks in sorted track-id order over
+// b200sfm_ba_problem_create / _create_rig, then b200sfm_ba_problem_filter_*.  Track::observations are rewritten as the
+// reference rewrites them and the number of tracks changed (removed, for the triangulation angle) is returned; 0 and
+// nothing changed on failure.
+//   FilterTracksByReprojection: in_normalized_image (the mapper's default) reads Image::features_undist
+//     (_filter_reprojection_normalized), otherwise the pixels of Image::features and the cameras' intrinsics.
+//   FilterTracksByAngle: features_undist, the threshold doubled for a camera without has_prior_focal_length (.cc:61-76).
+//   FilterTrackTriangulationAngle: a track without a pair of rays wider than min_angle loses all its observations.
+struct TrackFilter {
+  template <class ViewGraphT, class CameraMap, class ImageMap, class TrackMap>
+  static int FilterTracksByReprojection(const ViewGraphT& view_graph, const CameraMap& cameras, const ImageMap& images,
+                                        TrackMap& tracks, double max_reprojection_error = 1e-2, bool in_normalized_image = true) {
+    (void)view_graph;
+    // the normalised-plane variant reads no camera (track_filter.cc:23-31)
+    return processors_detail::RunTrackFilter(in_normalized_image ? 3 : 0, in_normalized_image ? nullptr : &cameras, images, tracks,
+                                             max_reprojection_error, "FilterTracksByReprojection");
+  }
+  template <class ViewGraphT, class CameraMap, class ImageMap, class TrackMap>
+  static int FilterTracksByAngle(const ViewGraphT& view_graph, const CameraMap& cameras, const ImageMap& images, TrackMap& tracks,
+                                 double max_angle_error = 1.) {
+    (void)view_graph;
+    return processors_detail::RunTrackFilter(1, &cameras, images, tracks, max_angle_error, "FilterTracksByAngle");
+  }
+  template <class ViewGraphT, class ImageMap, class TrackMap>
+  static int FilterTrackTriangulationAngle(const ViewGraphT& view_graph, const ImageMap& images, TrackMap& tracks,
+                                           double min_angle = 1.) {
+    (void)view_graph;
+    using Cam = std::unordered_map<camera_t, Camera>;
+    return processors_detail::RunTrackFilter(2, static_cast<const Cam*>(nullptr), images, tracks, min_angle,
+                                             "FilterTrackTriangulationAngle");
+  }
+};
+
+// UndistortImages (processors/image_undistorter.{h,cc}) on the device (b200sfm_undistort_features): the images in sorted
+// id order whose features_undist does not hold one bearing per feature, or all of them with clean_points, have their
+// features undistorted through the camera blocks of their cameras (sorted camera-id order) and features_undist replaced.
+template <class CameraMap, class ImageMap>
+void UndistortImages(CameraMap& cameras, ImageMap& images, bool clean_points) {
+  using Img = typename ImageMap::mapped_type;
+  std::map<image_t, Img*> todo;
+  for (auto& [id, im] : images)
+    if (clean_points || im.features_undist.size() != im.features.size()) todo[id] = &im;   // image_undistorter.cc:11-16
+  if (todo.empty()) return;
+  std::map<camera_t, int32_t> cidx;
+  for (auto& [id, im] : todo) {
+    if (cameras.find(im->camera_id) == cameras.end()) { std::fprintf(stderr, "b200sfm: image of an unknown camera\n"); return; }
+    cidx[im->camera_id] = 0;
+  }
+  std::vector<int32_t> model, feat_intr;
+  std::vector<double> params, xy;
+  for (auto& [id, k] : cidx) {
+    const auto& c = cameras.at(id);
+    k = (int32_t)model.size();
+    model.push_back(static_cast<int32_t>(c.model_id));
+    params.resize(params.size() + B200SFM_INTR_STRIDE, 0.0);
+    for (size_t j = 0; j < c.params.size() && j < (size_t)B200SFM_INTR_STRIDE; ++j) params[(size_t)k * B200SFM_INTR_STRIDE + j] = c.params[j];
+  }
+  for (auto& [id, im] : todo)
+    for (const auto& f : im->features) {
+      feat_intr.push_back(cidx[im->camera_id]);
+      xy.push_back(f[0]);
+      xy.push_back(f[1]);
+    }
+  const int64_t n = (int64_t)feat_intr.size();
+  std::vector<double> b(3 * (size_t)n);
+  if (n > 0) {
+    b200sfm_ctx* ctx = DefaultContext();
+    if (!ctx) return;
+    const int rc = b200sfm_undistort_features(ctx, (int32_t)model.size(), model.data(), params.data(), n, feat_intr.data(), xy.data(),
+                                              b.data());
+    if (rc != B200SFM_OK) { std::fprintf(stderr, "b200sfm: UndistortImages failed: %s\n", b200sfm_last_error(ctx)); return; }
+  }
+  size_t o = 0;
+  for (auto& [id, im] : todo) {
+    im->features_undist.resize(im->features.size());
+    for (auto& u : im->features_undist) {
+      for (int k = 0; k < 3; ++k) u[k] = b[3 * o + k];
+      ++o;
+    }
+  }
+}
+
+#ifdef B200SFM_SHIM_HAS_SIM3D
+// NormalizeReconstruction (processors/reconstruction_normalizer.{h,cc}) on the device (b200sfm_ba_problem_normalize): the
+// posed frames in sorted frame-id order as a rig problem -- (rig, camera) sensors, a trivial frame's camera with the
+// identity -- whose image table (b200sfm_ba_problem_set_images) is the registered images, so that the robust box and mean
+// run over their centres as in the reference.  The similarity moves the frames' translations and the tracks' points;
+// every non-reference cam_from_rig translation of every rig is scaled on the host (.cc:70-78).  Returns the similarity;
+// the identity and nothing changed on failure, and also without a registered image (the reference indexes an empty
+// vector there).  The problem carries the points and one placeholder observation: the normalisation reads no observation.
+template <class RigMap, class CameraMap, class FrameMap, class ImageMap, class TrackMap>
+b200host_adapt::Sim3d NormalizeReconstruction(RigMap& rigs, CameraMap& cameras, FrameMap& frames, ImageMap& images, TrackMap& tracks,
+                                              bool fixed_scale = false, double extent = 10., double p0 = 0.1, double p1 = 0.9) {
+  (void)cameras;
+  using Frm = typename FrameMap::mapped_type;
+  using Img = typename ImageMap::mapped_type;
+  using Trk = typename TrackMap::mapped_type;
+  const double zero[3] = {0, 0, 0};
+  const b200host_adapt::Sim3d identity = b200host_adapt::MakeSim3d(1.0, zero);
+  std::map<frame_t, Frm*> fsorted;
+  for (auto& [id, f] : frames)
+    if (f.HasPose()) fsorted[id] = &f;
+  std::map<frame_t, int32_t> fidx;
+  std::vector<Frm*> fr;
+  std::vector<double> quat, trans;
+  for (auto& [id, f] : fsorted) {
+    fidx[id] = (int32_t)fr.size();
+    fr.push_back(f);
+    for (int k = 0; k < 4; ++k) quat.push_back(f->RigFromWorld().rotation.coeffs().data()[k]);
+    for (int k = 0; k < 3; ++k) trans.push_back(f->RigFromWorld().translation[k]);
+  }
+  std::map<image_t, const Img*> reg;
+  for (auto& [id, im] : images)
+    if (im.IsRegistered()) reg[id] = &im;
+  if (reg.empty()) { std::fprintf(stderr, "b200sfm: NormalizeReconstruction without a registered image\n"); return identity; }
+  std::map<std::pair<rig_t, camera_t>, int32_t> sidx;
+  std::vector<int32_t> image_frame, image_sensor;
+  std::vector<double> sensor_q, sensor_t;
+  for (auto& [id, im] : reg) {
+    const auto f = fidx.find(im->frame_id);
+    if (f == fidx.end()) { std::fprintf(stderr, "b200sfm: registered image without a posed frame\n"); return identity; }
+    const auto key = std::make_pair(fr[f->second]->RigId(), im->camera_id);
+    auto s = sidx.find(key);
+    if (s == sidx.end()) {
+      s = sidx.emplace(key, (int32_t)sidx.size()).first;
+      Rigid3d cfr;   // identity
+      auto* rig = fr[f->second]->RigPtr();
+      if (!im->HasTrivialFrame() && !(rig && b200host_adapt::IsRefSensor(*rig, im->camera_id))) {
+        if (!rig || !b200host_adapt::HasCamFromRig(*rig, im->camera_id)) {
+          std::fprintf(stderr, "b200sfm: image of a rig sensor without cam_from_rig\n");
+          return identity;
+        }
+        cfr = b200host_adapt::CamFromRig(*rig, im->camera_id);
+      }
+      for (int k = 0; k < 4; ++k) sensor_q.push_back(cfr.rotation.coeffs().data()[k]);
+      for (int k = 0; k < 3; ++k) sensor_t.push_back(cfr.translation[k]);
+    }
+    image_frame.push_back(f->second);
+    image_sensor.push_back(s->second);
+  }
+  const int32_t S = (int32_t)sidx.size();
+  if (S > 65535) { std::fprintf(stderr, "b200sfm: too many rig sensors\n"); return identity; }
+  std::map<track_t, Trk*> tsorted;
+  for (auto& [id, t] : tracks) tsorted[id] = &t;
+  const int32_t P = std::max<int32_t>((int32_t)tsorted.size(), 1);
+  std::vector<double> points(3 * (size_t)P, 0.0);
+  {
+    size_t p = 0;
+    for (auto& [id, t] : tsorted) { for (int k = 0; k < 3; ++k) points[3 * p + k] = t->xyz[k]; ++p; }
+  }
+  std::vector<int64_t> ptb(P + 1, 1);
+  ptb[0] = 0;   // the placeholder observation belongs to point 0
+  const int32_t obs_frame = 0, sensor_intr = 0, intr_model = B200SFM_SIMPLE_PINHOLE;
+  const uint16_t obs_sensor = 0;
+  const double obs_xy[2] = {0, 0};
+  std::vector<double> intr(B200SFM_INTR_STRIDE, 0.0);
+  intr[0] = 1.0;
+  std::vector<int32_t> sensor_intrs(S, sensor_intr);
+  b200sfm_ctx* ctx = DefaultContext();
+  if (!ctx) return identity;
+  b200sfm_ba_problem* prob = nullptr;
+  double scale = 1.0, t[3] = {0, 0, 0};
+  int rc = b200sfm_ba_problem_create_rig(ctx, (int32_t)fr.size(), P, 1, 1, S, ptb.data(), &obs_frame, &obs_sensor, obs_xy, sensor_q.data(),
+                                         sensor_t.data(), sensor_intrs.data(), &intr_model, nullptr, 1, &prob);
+  if (rc == B200SFM_OK) rc = b200sfm_ba_problem_set_state(prob, intr.data(), quat.data(), trans.data(), points.data());
+  if (rc == B200SFM_OK) rc = b200sfm_ba_problem_set_images(prob, (int32_t)image_frame.size(), image_frame.data(), image_sensor.data());
+  if (rc == B200SFM_OK) rc = b200sfm_ba_problem_normalize(prob, fixed_scale ? 1 : 0, extent, p0, p1, &scale, t);
+  if (rc == B200SFM_OK) rc = b200sfm_ba_problem_get_state(prob, nullptr, nullptr, trans.data(), points.data());
+  b200sfm_ba_problem_free(prob);
+  if (rc != B200SFM_OK) {
+    std::fprintf(stderr, "b200sfm: NormalizeReconstruction failed: %s\n", b200sfm_last_error(ctx));
+    return identity;
+  }
+  for (size_t f = 0; f < fr.size(); ++f)                                                       // .cc:64-68
+    for (int k = 0; k < 3; ++k) fr[f]->RigFromWorld().translation[k] = trans[3 * f + k];
+  for (auto& [id, rig] : rigs) b200host_adapt::ScaleCamFromRigTranslations(rig, scale);        // .cc:70-78
+  size_t p = 0;
+  for (auto& [id, tr] : tsorted) { for (int k = 0; k < 3; ++k) tr->xyz[k] = points[3 * p + k]; ++p; }   // .cc:80-82
+  return b200host_adapt::MakeSim3d(scale, t);
+}
+#else
+// A glomap build without <colmap/geometry/sim3.h> on its include path: NormalizeReconstruction cannot return
+// colmap::Sim3d, and a call says so instead of the function going missing.
+template <class RigMap, class... Rest>
+void NormalizeReconstruction(RigMap&, Rest&&...) {
+  static_assert(sizeof(RigMap) == 0, "b200sfm_shim::NormalizeReconstruction needs <colmap/geometry/sim3.h> on the include path");
+}
+#endif
 
 }  // namespace b200sfm_shim

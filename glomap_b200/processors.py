@@ -10,7 +10,8 @@
   (``CamFromImg(xy).homogeneous().normalized()``), the input of global positioning and of the angle filter; radial
   models are inverted on the radius by a safeguarded Newton iteration (``synthetic.undistort_radius_scale``).
 
-Both are O(N) host work in the reference as well; the device-resident versions are a later row."""
+Both are O(N) host work in the reference as well; the device-resident versions are ``estimators.BAProblem.normalize`` /
+``undistort``, and ``undistort_features_device`` undistorts pixels outside a problem (``b200sfm_undistort_features``)."""
 from __future__ import annotations
 
 import numpy as np
@@ -52,3 +53,25 @@ def undistort_images(scene) -> np.ndarray:
     if hasattr(scene, "obs_sensor"):
         return S.bearings_from_scene(scene.images_scene())
     return S.bearings_from_scene(scene)
+
+
+def undistort_features_device(intr_model, intr_params, feat_intr, xy, ctx=None) -> np.ndarray:
+    """``b200sfm_undistort_features``: unit bearing [n,3] of every pixel xy [n,2] through intrinsics block feat_intr [n]
+    (``Image::features`` -> ``features_undist`` as UndistortImages computes it).  Raises ``_lib.B200Error`` with code 1 for a
+    block index outside [0, K) and code 5 for a camera model outside 0-3."""
+    import ctypes as ct
+
+    from . import _lib, estimators as E
+    model = np.ascontiguousarray(intr_model, np.int32)
+    params = np.zeros((len(model), S.INTR_STRIDE))
+    p = np.asarray(intr_params, np.float64).reshape(len(model), -1)
+    params[:, :min(p.shape[1], S.INTR_STRIDE)] = p[:, :S.INTR_STRIDE]
+    fi = np.ascontiguousarray(feat_intr, np.int32)
+    xy = np.ascontiguousarray(xy, np.float64).reshape(-1, 2)
+    assert len(fi) == len(xy)
+    out = np.empty((len(fi), 3))
+    ctx = ctx or E.default_context()
+    ptr = lambda a: a.ctypes.data_as(ct.c_void_p) if a.size else None   # noqa: E731
+    _lib.check(ctx.handle, ctx.lib.b200sfm_undistort_features(ctx.handle, len(model), ptr(model), ptr(params), len(fi), ptr(fi),
+                                                              ptr(xy), ptr(out)))
+    return out

@@ -242,6 +242,15 @@ int b200sfm_ba_problem_undistort(b200sfm_ba_problem* p, double* bearings_out /*[
 int b200sfm_ba_problem_filter_triangulation_angle(b200sfm_ba_problem* p, double min_angle_deg, uint8_t* keep_track /*[P]*/,
                                                   int64_t* num_tracks_removed);
 void b200sfm_ba_problem_free(b200sfm_ba_problem* p);
+/* UndistortImages (glomap/processors/image_undistorter.cc:7-53) per FEATURE, outside a BA problem: bearings_out[i] =
+ * CamFromImg(xy[i]).homogeneous().normalized() with the intrinsics block feat_intr[i] -- the arithmetic of
+ * b200sfm_ba_problem_undistort, over Image::features instead of the observations of a problem.
+ *   intr_model [K], intr_params [K][B200SFM_INTR_STRIDE]; feat_intr [n], xy [n][2] distorted pixels; bearings_out [n][3].
+ * n == 0 returns B200SFM_OK.  A feat_intr outside [0, K) gives B200SFM_ERR_INVALID_ARG, a camera model outside 0-3 of a
+ * block some feature uses B200SFM_ERR_UNSUPPORTED; both are checked on the device (never dereferenced) and bearings_out is
+ * then untouched.  No collectives: on a distributed context each rank undistorts the features it is given. */
+int b200sfm_undistort_features(b200sfm_ctx* ctx, int32_t K, const int32_t* intr_model, const double* intr_params, int64_t n,
+                               const int32_t* feat_intr, const double* xy, double* bearings_out);
 
 /* ---- track establishment (SURVEY.md 8(f) item 4) ---------------------------------------------------------------------
  * TrackEngine::EstablishFullTracks (glomap/controllers/track_establishment.cc:5-17): the union-find over all inlier
