@@ -152,7 +152,7 @@ static int RunRotationAverager(int argc, char** argv) {
       Frame& f = frames[name_idx[name]];
       f.gravity_info.SetGravity(g);
       GetAlignRotHouseholder(g.data(), f.gravity_info.R_align);
-      RotationEstimator::RToQuat(f.gravity_info.R_align, f.RigFromWorld().rotation.coeffs().data());
+      detail::RToQuat(f.gravity_info.R_align, f.RigFromWorld().rotation.coeffs().data());
     }
     KeepLargestConnectedComponents(view_graph, frames, images);                               // exe/rotation_averager.cc:95
     if (refine_gravity) {                                                                      // :99-102
@@ -218,13 +218,13 @@ static int RunRotationAverager(int argc, char** argv) {
     while (!bfs.empty()) {
       image_t c = bfs.front(); bfs.pop();
       double Rc[9];
-      QuatToR(frames[c].RigFromWorld().rotation.coeffs().data(), Rc);
+      detail::QuatToR(frames[c].RigFromWorld().rotation.coeffs().data(), Rc);
       for (image_t nb : adj[c]) {
         if (seen.count(nb)) continue;
         seen.insert(nb);
         const ImagePair& pr = view_graph.image_pairs[ImagePairToPairId(c, nb)];
         double Rr[9], Rn[9];
-        QuatToR(pr.cam2_from_cam1.rotation.coeffs().data(), Rr);
+        detail::QuatToR(pr.cam2_from_cam1.rotation.coeffs().data(), Rr);
         for (int i = 0; i < 3; ++i)
           for (int j = 0; j < 3; ++j) {
             double s = 0;

@@ -55,7 +55,73 @@ inline b200sfm_ctx* DefaultContext(const std::string& gpu_index = "-1") {
   return ctx;
 }
 
-// small quaternion helpers (xyzw, Eigen coeffs() order)
+// How every entry point turns the scene into flat arrays: the sorted-id order, the camera blocks, an image's
+// cam_from_rig and the rotation algebra.  Which entities become blocks, how they are numbered and what an entry point
+// does with a missing entity stay with each entry point.
+namespace detail {
+
+// The entries of an id-keyed map as (id, pointer) in ascending id, only those `keep` accepts.
+template <class Map, class Keep>
+auto SortedEntries(Map& m, Keep keep) {
+  std::vector<std::pair<typename Map::key_type, decltype(&m.begin()->second)>> out;
+  for (auto& [id, v] : m)
+    if (keep(v)) out.emplace_back(id, &v);
+  std::sort(out.begin(), out.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  return out;
+}
+template <class Map>
+auto SortedEntries(Map& m) {
+  return SortedEntries(m, [](const auto&) { return true; });
+}
+// id -> position in a vector of SortedEntries
+template <class Id, class T>
+std::unordered_map<Id, int32_t> PositionOf(const std::vector<std::pair<Id, T>>& sorted) {
+  std::unordered_map<Id, int32_t> pos;
+  for (size_t i = 0; i < sorted.size(); ++i) pos.emplace(sorted[i].first, (int32_t)i);
+  return pos;
+}
+
+// Camera blocks: model_id and params zero-padded to B200SFM_INTR_STRIDE (params beyond the stride are not passed),
+// one block per camera of `cams` ((id, Camera*) pairs) in their order.
+template <class CameraPtrs>
+void PackCameras(const CameraPtrs& cams, std::vector<int32_t>& model, std::vector<double>& intr) {
+  model.clear();
+  intr.assign(cams.size() * B200SFM_INTR_STRIDE, 0.0);
+  for (size_t k = 0; k < cams.size(); ++k) {
+    const auto& c = *cams[k].second;
+    model.push_back(static_cast<int32_t>(c.model_id));   // colmap::CameraModelId is an enum class
+    for (size_t j = 0; j < c.params.size() && j < (size_t)B200SFM_INTR_STRIDE; ++j) intr[k * B200SFM_INTR_STRIDE + j] = c.params[j];
+  }
+}
+// the inverse of PackCameras: the blocks' params back into the cameras
+template <class CameraPtrs>
+void UnpackCameras(const std::vector<double>& intr, const CameraPtrs& cams) {
+  for (size_t k = 0; k < cams.size(); ++k) {
+    auto& c = *cams[k].second;
+    for (size_t j = 0; j < c.params.size() && j < (size_t)B200SFM_INTR_STRIDE; ++j) c.params[j] = intr[k * B200SFM_INTR_STRIDE + j];
+  }
+}
+// one SIMPLE_PINHOLE block with f = 1, for a device problem whose intrinsics are never read, so that a camera model the
+// call does not read cannot refuse it
+inline void PlaceholderCamera(std::vector<int32_t>& model, std::vector<double>& intr) {
+  model.assign(1, B200SFM_SIMPLE_PINHOLE);
+  intr.assign(B200SFM_INTR_STRIDE, 0.0);
+  intr[0] = 1.0;
+}
+
+// An image's cam_from_rig through the rig the caller holds (null: none): the identity for a trivial frame or the rig's
+// reference sensor, the rig's stored pose when it has one, otherwise missing (`pose` is then the identity).
+enum class CamFromRigStatus { kIdentity, kKnown, kMissing };
+template <class RigT, class ImageT>
+CamFromRigStatus ResolveCamFromRig(RigT* rig, const ImageT& im, Rigid3d& pose) {
+  pose = Rigid3d();
+  if (im.HasTrivialFrame() || (rig && b200host_adapt::IsRefSensor(*rig, im.camera_id))) return CamFromRigStatus::kIdentity;
+  if (!rig || !b200host_adapt::HasCamFromRig(*rig, im.camera_id)) return CamFromRigStatus::kMissing;
+  pose = b200host_adapt::CamFromRig(*rig, im.camera_id);
+  return CamFromRigStatus::kKnown;
+}
+
+// Rotation algebra: quaternions xyzw (Eigen's coeffs() order), matrices row-major.
 inline void QuatMul(const double* a, const double* b, double* o) {   // o = a (x) b
   const double x = a[3] * b[0] + a[0] * b[3] + a[1] * b[2] - a[2] * b[1];
   const double y = a[3] * b[1] - a[0] * b[2] + a[1] * b[3] + a[2] * b[0];
@@ -64,6 +130,69 @@ inline void QuatMul(const double* a, const double* b, double* o) {   // o = a (x
   o[0] = x; o[1] = y; o[2] = z; o[3] = w;
 }
 inline void QuatConj(const double* a, double* o) { o[0] = -a[0]; o[1] = -a[1]; o[2] = -a[2]; o[3] = a[3]; }
+inline void QuatToR(const double* q, double R[9]) {
+  const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  const double x = q[0] / n, y = q[1] / n, z = q[2] / n, w = q[3] / n;
+  R[0] = 1 - 2 * (y * y + z * z); R[1] = 2 * (x * y - z * w); R[2] = 2 * (x * z + y * w);
+  R[3] = 2 * (x * y + z * w); R[4] = 1 - 2 * (x * x + z * z); R[5] = 2 * (y * z - x * w);
+  R[6] = 2 * (x * z - y * w); R[7] = 2 * (y * z + x * w); R[8] = 1 - 2 * (x * x + y * y);
+}
+// rotation matrix -> unit quaternion, w >= 0 (Shepperd's branches, as Eigen's conversion)
+inline void RToQuat(const double* R, double* q) {
+  const double tr = R[0] + R[4] + R[8];
+  if (tr > 0) {
+    const double s = std::sqrt(tr + 1.0) * 2;
+    q[3] = 0.25 * s; q[0] = (R[7] - R[5]) / s; q[1] = (R[2] - R[6]) / s; q[2] = (R[3] - R[1]) / s;
+  } else if (R[0] > R[4] && R[0] > R[8]) {
+    const double s = std::sqrt(1.0 + R[0] - R[4] - R[8]) * 2;
+    q[3] = (R[7] - R[5]) / s; q[0] = 0.25 * s; q[1] = (R[1] + R[3]) / s; q[2] = (R[2] + R[6]) / s;
+  } else if (R[4] > R[8]) {
+    const double s = std::sqrt(1.0 + R[4] - R[0] - R[8]) * 2;
+    q[3] = (R[2] - R[6]) / s; q[0] = (R[1] + R[3]) / s; q[1] = 0.25 * s; q[2] = (R[5] + R[7]) / s;
+  } else {
+    const double s = std::sqrt(1.0 + R[8] - R[0] - R[4]) * 2;
+    q[3] = (R[3] - R[1]) / s; q[0] = (R[2] + R[6]) / s; q[1] = (R[5] + R[7]) / s; q[2] = 0.25 * s;
+  }
+  if (q[3] < 0) for (int k = 0; k < 4; ++k) q[k] = -q[k];
+}
+inline void QuatToAngleAxis(const double* q, double* v) {
+  double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+  if (n > 0) {
+    const double ang = 2 * std::atan2(n, std::fabs(q[3]));
+    const double f = (q[3] < 0 ? -ang : ang) / n;
+    v[0] = q[0] * f; v[1] = q[1] * f; v[2] = q[2] * f;
+  } else {
+    v[0] = v[1] = v[2] = 0;
+  }
+}
+inline void AngleAxisToQuat(const double* v, double* q) {
+  const double n = std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+  if (n > 0) {
+    const double s = std::sin(n / 2) / n;
+    q[0] = v[0] * s; q[1] = v[1] * s; q[2] = v[2] * s; q[3] = std::cos(n / 2);
+  } else {
+    q[0] = q[1] = q[2] = 0; q[3] = 1;
+  }
+}
+// C = A B and C = A^T B for a 3x3 A and a 3xN B (N = 1: a vector); every element is summed left to right,
+// a[r][0] b[0][c] + a[r][1] b[1][c] + a[r][2] b[2][c].  C may be A or B.
+template <int N = 3>
+inline void MulAB(const double* A, const double* B, double* C) {
+  double T[3 * N];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < N; ++c) T[N * r + c] = A[3 * r] * B[c] + A[3 * r + 1] * B[N + c] + A[3 * r + 2] * B[2 * N + c];
+  std::copy(T, T + 3 * N, C);
+}
+template <int N = 3>
+inline void MulAtB(const double* A, const double* B, double* C) {
+  double T[3 * N];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < N; ++c) T[N * r + c] = A[r] * B[c] + A[3 + r] * B[N + c] + A[6 + r] * B[2 * N + c];
+  std::copy(T, T + 3 * N, C);
+}
+
+}  // namespace detail
+
 // colmap::AverageQuaternions with unit weights: dominant eigenvector of sum q q^T (sign-invariant), by power iteration
 inline void AverageQuaternions(const std::vector<std::array<double, 4>>& qs, double* out) {
   double M[4][4] = {};
@@ -80,14 +209,6 @@ inline void AverageQuaternions(const std::vector<std::array<double, 4>>& qs, dou
     for (int k = 0; k < 4; ++k) v[k] = u[k] / n;
   }
   for (int k = 0; k < 4; ++k) out[k] = v[k];
-}
-
-inline void QuatToR(const double* q, double R[9]) {
-  const double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
-  const double x = q[0] / n, y = q[1] / n, z = q[2] / n, w = q[3] / n;
-  R[0] = 1 - 2 * (y * y + z * z); R[1] = 2 * (x * y - z * w); R[2] = 2 * (x * z + y * w);
-  R[3] = 2 * (x * y + z * w); R[4] = 1 - 2 * (x * x + z * z); R[5] = 2 * (y * z - x * w);
-  R[6] = 2 * (x * z - y * w); R[7] = 2 * (y * z + x * w); R[8] = 1 - 2 * (x * x + y * y);
 }
 
 // ---------------------------------------------------------------------------
@@ -135,81 +256,79 @@ class BundleAdjuster {
     if (tracks.empty()) { std::fprintf(stderr, "Number of tracks = 0\n"); return false; }     // .cc:21-24
     b200sfm_ctx* ctx = DefaultContext(options_.gpu_index);
     if (!ctx) return false;
-    // frames / cameras / tracks in sorted-id order
-    std::map<frame_t, Frame*> fsorted;
-    for (auto& [id, f] : frames) fsorted[id] = &f;
-    std::map<frame_t, int> fidx;
-    for (auto& [id, f] : fsorted) { const int i = (int)fidx.size(); fidx[id] = i; }
-    std::map<camera_t, Camera*> csorted;
-    for (auto& [id, c] : cameras) csorted[id] = &c;
-    std::map<camera_t, int> cidx;
-    for (auto& [id, c] : csorted) { const int i = (int)cidx.size(); cidx[id] = i; }
+    // every frame and every camera is a block, in sorted-id order; the gauge frame is chosen below, once it is known
+    // which frames carry observations (.cc:252-266)
+    const auto fsorted = detail::SortedEntries(frames);
+    auto fidx = detail::PositionOf(fsorted);
+    const auto csorted = detail::SortedEntries(cameras);
+    auto cidx = detail::PositionOf(csorted);
     const int C = (int)fsorted.size(), K = (int)csorted.size();
-    std::vector<double> quat(4 * (size_t)C), trans(3 * (size_t)C), intr((size_t)K * B200SFM_INTR_STRIDE, 0.0);
-    std::vector<int32_t> cam_intr(C, 0), intr_model(K);
+    std::vector<double> quat(4 * (size_t)C), trans(3 * (size_t)C), intr;
+    std::vector<int32_t> cam_intr(C, 0), intr_model;
     std::vector<uint8_t> mask(C, 0);
-    for (auto& [id, f] : fsorted) {
-      const int i = fidx[id];
-      for (int k = 0; k < 4; ++k) quat[4 * i + k] = f->RigFromWorld().rotation.coeffs().data()[k];
-      for (int k = 0; k < 3; ++k) trans[3 * i + k] = f->RigFromWorld().translation[k];
+    for (int i = 0; i < C; ++i) {
+      const Rigid3d& pose = fsorted[i].second->RigFromWorld();
+      for (int k = 0; k < 4; ++k) quat[4 * i + k] = pose.rotation.coeffs().data()[k];
+      for (int k = 0; k < 3; ++k) trans[3 * i + k] = pose.translation[k];
     }
-    // the gauge frame is chosen below, once it is known which frames carry observations (.cc:252-266)
-    for (auto& [id, c] : csorted) {
-      const int k = cidx[id];
-      intr_model[k] = static_cast<int32_t>(c->model_id);   // colmap::CameraModelId is an enum class
-      for (size_t j = 0; j < c->params.size() && j < B200SFM_INTR_STRIDE; ++j) intr[(size_t)k * B200SFM_INTR_STRIDE + j] = c->params[j];
-    }
-    // sensors = (rig, camera) pairs in sorted order; trivial frames use the identity cam_from_rig
+    detail::PackCameras(csorted, intr_model, intr);
+    // sensors = the (rig, camera) pairs of all images in sorted order, each resolved from the first of its images met
     bool any_rig = false;
     for (auto& [id, im] : images) any_rig = any_rig || !im.HasTrivialFrame();
-    std::map<std::pair<rig_t, camera_t>, int> sidx;
+    struct ImageBlocks { const Image* im; int32_t frame, sensor; };
+    std::unordered_map<image_t, ImageBlocks> blocks_of;
+    std::map<std::pair<rig_t, camera_t>, std::pair<int32_t, Rigid3d>> sensors;   // (index, cam_from_rig)
     std::vector<double> sensor_q, sensor_t;
     std::vector<int32_t> sensor_intr;
     std::vector<uint8_t> sensor_var;   // optimize_rig_poses: every non-reference sensor is an unknown (.cc:162-180,296-308)
     if (any_rig) {
-      for (auto& [id, im] : images) sidx[{frames[im.frame_id].RigId(), im.camera_id}] = 0;
-      int n = 0;
-      for (auto& [key, idx] : sidx) {
-        idx = n++;
-        Rigid3d cfr;   // identity
-        bool trivial = true;
-        for (auto& [iid, im] : images)
-          if (frames[im.frame_id].RigId() == key.first && im.camera_id == key.second) { trivial = im.HasTrivialFrame(); break; }
-        if (!trivial) cfr = b200host_adapt::CamFromRig(rigs[key.first], key.second);
-        for (int k = 0; k < 4; ++k) sensor_q.push_back(cfr.rotation.coeffs().data()[k]);
-        for (int k = 0; k < 3; ++k) sensor_t.push_back(cfr.translation[k]);
+      for (auto& [id, im] : images) {
+        const auto key = std::make_pair(frames[im.frame_id].RigId(), im.camera_id);
+        auto s = sensors.find(key);
+        if (s != sensors.end()) continue;
+        s = sensors.emplace(key, std::make_pair(0, Rigid3d())).first;
+        detail::ResolveCamFromRig(im.HasTrivialFrame() ? nullptr : &rigs[key.first], im, s->second.second);   // missing: identity
+      }
+      int32_t n = 0;
+      for (auto& [key, s] : sensors) {
+        s.first = n++;
+        for (int k = 0; k < 4; ++k) sensor_q.push_back(s.second.rotation.coeffs().data()[k]);
+        for (int k = 0; k < 3; ++k) sensor_t.push_back(s.second.translation[k]);
         sensor_intr.push_back(cidx[key.second]);
         // NonRefSensors() of the rig (.cc:299); Image::HasTrivialFrame() is exactly IsRefSensor (scene/image.h:73-76)
         sensor_var.push_back((options_.optimize_rig_poses && !b200host_adapt::IsRefSensor(rigs[key.first], key.second)) ? 1 : 0);
       }
       if (n > 65535) { std::fprintf(stderr, "b200sfm: too many rig sensors\n"); return false; }
+      for (auto& [id, im] : images)
+        blocks_of[id] = {&im, fidx[im.frame_id], sensors[{frames[im.frame_id].RigId(), im.camera_id}].first};
     } else {
-      for (auto& [id, im] : images) cam_intr[fidx[im.frame_id]] = cidx[im.camera_id];
+      for (auto& [id, im] : images) {
+        blocks_of[id] = {&im, fidx[im.frame_id], 0};
+        cam_intr[fidx[im.frame_id]] = cidx[im.camera_id];
+      }
     }
-    std::map<track_t, Track*> tsorted;
-    for (auto& [id, t] : tracks) tsorted[id] = &t;
+    const auto tsorted = detail::SortedEntries(tracks);
     const int P = (int)tsorted.size();
     std::vector<int64_t> ptb(1, 0);
     std::vector<int32_t> obs_cam;
     std::vector<uint16_t> obs_sensor;
     std::vector<double> obs_xy, points(3 * (size_t)P);
-    int p = 0;
-    for (auto& [id, t] : tsorted) {
+    for (int p = 0; p < P; ++p) {
+      const Track& t = *tsorted[p].second;
       // .cc:122: the track is skipped on ITS observation count; observations of missing images are dropped afterwards
       // (.cc:125), so the device gets min_num_view_per_track = 1 and a skipped track simply carries no observation
-      const bool keep = (int)t->observations.size() >= options_.min_num_view_per_track;
-      for (const auto& ob : t->observations) {
+      const bool keep = (int)t.observations.size() >= options_.min_num_view_per_track;
+      for (const auto& ob : t.observations) {
         if (!keep) break;
-        auto it = images.find(ob.first);
-        if (it == images.end()) continue;                                                     // .cc:125
-        obs_cam.push_back(fidx[it->second.frame_id]);
-        if (any_rig) obs_sensor.push_back((uint16_t)sidx[{frames[it->second.frame_id].RigId(), it->second.camera_id}]);
-        obs_xy.push_back(it->second.features[ob.second][0]);
-        obs_xy.push_back(it->second.features[ob.second][1]);
+        auto it = blocks_of.find(ob.first);
+        if (it == blocks_of.end()) continue;                                                  // .cc:125
+        obs_cam.push_back(it->second.frame);
+        if (any_rig) obs_sensor.push_back((uint16_t)it->second.sensor);
+        obs_xy.push_back(it->second.im->features[ob.second][0]);
+        obs_xy.push_back(it->second.im->features[ob.second][1]);
       }
       ptb.push_back((int64_t)obs_cam.size());
-      for (int k = 0; k < 3; ++k) points[3 * (size_t)p + k] = t->xyz[k];
-      ++p;
+      for (int k = 0; k < 3; ++k) points[3 * (size_t)p + k] = t.xyz[k];
     }
     {   // .cc:252-266: the first frame (map order; here sorted-id order) that HAS a parameter block is held constant
       std::vector<uint8_t> used(C, 0);
@@ -242,7 +361,8 @@ class BundleAdjuster {
       if (rc == B200SFM_OK && options_.optimize_rig_poses) {   // the optimised cam_from_rig back into the rigs, in place
         rc = b200sfm_ba_problem_get_sensor_poses(prob, sensor_q.data(), sensor_t.data());
         if (rc == B200SFM_OK)
-          for (auto& [key, idx] : sidx) {
+          for (auto& [key, s] : sensors) {
+            const int32_t idx = s.first;
             if (!sensor_var[idx]) continue;
             Rigid3d cfr;
             for (int k = 0; k < 4; ++k) cfr.rotation.coeffs().data()[k] = sensor_q[4 * (size_t)idx + k];
@@ -257,15 +377,14 @@ class BundleAdjuster {
                             points.data(), &summary);
     }
     if (rc != B200SFM_OK) { std::fprintf(stderr, "b200sfm_ba_solve: %s\n", b200sfm_last_error(ctx)); return false; }
-    for (auto& [id, f] : fsorted) {                                                           // results in place (.cc:140-146)
-      const int i = fidx[id];
-      for (int k = 0; k < 4; ++k) f->RigFromWorld().rotation.coeffs().data()[k] = quat[4 * i + k];
-      for (int k = 0; k < 3; ++k) f->RigFromWorld().translation[k] = trans[3 * i + k];
+    for (int i = 0; i < C; ++i) {                                                             // results in place (.cc:140-146)
+      Rigid3d& pose = fsorted[i].second->RigFromWorld();
+      for (int k = 0; k < 4; ++k) pose.rotation.coeffs().data()[k] = quat[4 * i + k];
+      for (int k = 0; k < 3; ++k) pose.translation[k] = trans[3 * i + k];
     }
-    p = 0;
-    for (auto& [id, t] : tsorted) { for (int k = 0; k < 3; ++k) t->xyz[k] = points[3 * (size_t)p + k]; ++p; }
-    for (auto& [id, c] : csorted)
-      for (size_t j = 0; j < c->params.size() && j < B200SFM_INTR_STRIDE; ++j) c->params[j] = intr[(size_t)cidx[id] * B200SFM_INTR_STRIDE + j];
+    for (int p = 0; p < P; ++p)
+      for (int k = 0; k < 3; ++k) tsorted[p].second->xyz[k] = points[3 * (size_t)p + k];
+    detail::UnpackCameras(intr, csorted);
     return summary.usable != 0;                                                               // .cc:105
   }
 
@@ -309,25 +428,22 @@ class GlobalPositioner {
     }
     b200sfm_ctx* ctx = DefaultContext(options_.gpu_index);
     if (!ctx) return false;
-    std::map<frame_t, Frame*> fsorted;
-    for (auto& [id, f] : frames) fsorted[id] = &f;
-    std::map<frame_t, int> fidx;
-    for (auto& [id, f] : fsorted) { const int i = (int)fidx.size(); fidx[id] = i; }
+    const auto fsorted = detail::SortedEntries(frames);   // every frame is a block
+    auto fidx = detail::PositionOf(fsorted);
     const int C = (int)fsorted.size();
     std::uniform_real_distribution<double> U(-1, 1);
     std::vector<double> centers(3 * (size_t)C), Rm(9 * (size_t)C);
     std::vector<uint8_t> calibrated(C, 1);
-    for (auto& [id, f] : fsorted) {
-      const int i = fidx[id];
-      QuatToR(f->RigFromWorld().rotation.coeffs().data(), &Rm[9 * (size_t)i]);
-      for (int k = 0; k < 3; ++k) {
-        if (options_.generate_random_positions && options_.optimize_positions) {
-          centers[3 * i + k] = 100.0 * U(random_generator_);                                  // .cc:158-159
-        } else {                                                                              // CenterFromPose: -R^T t
-          const double* R = &Rm[9 * (size_t)i];
-          const auto& t = f->RigFromWorld().translation;
-          centers[3 * i + k] = -(R[k] * t[0] + R[3 + k] * t[1] + R[6 + k] * t[2]);
-        }
+    for (int i = 0; i < C; ++i) {
+      const Rigid3d& pose = fsorted[i].second->RigFromWorld();
+      double* R = &Rm[9 * (size_t)i];
+      detail::QuatToR(pose.rotation.coeffs().data(), R);
+      if (options_.generate_random_positions && options_.optimize_positions) {
+        for (int k = 0; k < 3; ++k) centers[3 * i + k] = 100.0 * U(random_generator_);        // .cc:158-159
+      } else {                                                                                // CenterFromPose: -R^T t
+        const double t[3] = {pose.translation[0], pose.translation[1], pose.translation[2]};
+        detail::MulAtB<1>(R, t, &centers[3 * i]);
+        for (int k = 0; k < 3; ++k) centers[3 * i + k] = -centers[3 * i + k];
       }
     }
     bool any_rig = false;
@@ -339,61 +455,64 @@ class GlobalPositioner {
     std::vector<uint8_t> obs_cal;     // the loss is chosen per CAMERA (.cc:313-316)
     // sensors whose cam_from_rig translation is still NaN (rotation averaging estimated their rotation only): their
     // centre in the rig frame is an unknown of this solve, RigUnknownBATAPairwiseDirectionError (.cc:355-372)
+    // (numbered in order of first appearance; `urot` holds their cam_from_rig for the write-back)
     std::map<std::pair<rig_t, camera_t>, int> usens;
+    std::vector<Rigid3d> urot;
     std::vector<int32_t> obs_usens;
-    std::map<track_t, Track*> tsorted;
-    for (auto& [id, t] : tracks) tsorted[id] = &t;
+    const auto tsorted = detail::SortedEntries(tracks);
     const int P = (int)tsorted.size();
     std::vector<int64_t> ptb(1, 0);
     std::vector<int32_t> obs_cam;
     std::vector<double> obs_dir, points(3 * (size_t)P);
-    int p = 0;
-    for (auto& [id, t] : tsorted) {
-      const bool keep = (int)t->observations.size() >= options_.min_num_view_per_track;        // .cc:257-258
-      for (const auto& ob : t->observations) {
+    for (int p = 0; p < P; ++p) {
+      Track& t = *tsorted[p].second;
+      const bool keep = (int)t.observations.size() >= options_.min_num_view_per_track;         // .cc:257-258
+      for (const auto& ob : t.observations) {
         if (!keep) break;
         auto it = images.find(ob.first);
         if (it == images.end() || !it->second.IsRegistered()) continue;                      // .cc:279-282
-        const auto& b = it->second.features_undist[ob.second];
+        const Image& im = it->second;
+        const double b[3] = {im.features_undist[ob.second][0], im.features_undist[ob.second][1], im.features_undist[ob.second][2]};
         if (std::isnan(b[0]) || std::isnan(b[1]) || std::isnan(b[2])) continue;               // .cc:286-292
-        const int ci = fidx[it->second.frame_id];
+        const int ci = fidx[im.frame_id];
         const double* R = &Rm[9 * (size_t)ci];
+        double dir[3];
         if (any_rig) {
           // cam_from_world = cam_from_rig * rig_from_world;  t_obs = R_cw^T b,  t_rig = R_cw^T t_cam_from_rig
-          Rigid3d cfr;
-          if (!it->second.HasTrivialFrame())
-            cfr = b200host_adapt::CamFromRig(rigs[frames[it->second.frame_id].RigId()], it->second.camera_id);
+          Rigid3d cfr;   // a missing cam_from_rig stays the identity
+          detail::ResolveCamFromRig(im.HasTrivialFrame() ? nullptr : &rigs[frames[im.frame_id].RigId()], im, cfr);
           int us = -1;
           if (std::isnan(cfr.translation[0]) || std::isnan(cfr.translation[1]) || std::isnan(cfr.translation[2])) {
-            const auto key = std::make_pair(frames[it->second.frame_id].RigId(), it->second.camera_id);
+            const auto key = std::make_pair(frames[im.frame_id].RigId(), im.camera_id);
             auto u = usens.find(key);
-            if (u == usens.end()) u = usens.emplace(key, (int)usens.size()).first;
+            if (u == usens.end()) {
+              u = usens.emplace(key, (int)usens.size()).first;
+              urot.push_back(cfr);
+            }
             us = u->second;
             cfr.translation[0] = cfr.translation[1] = cfr.translation[2] = 0.0;   // no known offset: the centre is the unknown
           }
           obs_usens.push_back(us);
-          double Rs[9], bb[3], tt[3];
-          QuatToR(cfr.rotation.coeffs().data(), Rs);
-          for (int k = 0; k < 3; ++k) {   // R_cr^T b, R_cr^T t_cr
-            bb[k] = Rs[k] * b[0] + Rs[3 + k] * b[1] + Rs[6 + k] * b[2];
-            tt[k] = Rs[k] * cfr.translation[0] + Rs[3 + k] * cfr.translation[1] + Rs[6 + k] * cfr.translation[2];
-          }
-          for (int k = 0; k < 3; ++k) {
-            obs_dir.push_back(R[k] * bb[0] + R[3 + k] * bb[1] + R[6 + k] * bb[2]);
-            obs_off.push_back(R[k] * tt[0] + R[3 + k] * tt[1] + R[6 + k] * tt[2]);
-          }
-          obs_cal.push_back(cameras[it->second.camera_id].has_prior_focal_length ? 1 : 0);
+          double Rs[9], off[3];
+          detail::QuatToR(cfr.rotation.coeffs().data(), Rs);
+          const double t_cr[3] = {cfr.translation[0], cfr.translation[1], cfr.translation[2]};
+          detail::MulAtB<1>(Rs, b, dir);          // R_cr^T b
+          detail::MulAtB<1>(Rs, t_cr, off);       // R_cr^T t_cr
+          detail::MulAtB<1>(R, dir, dir);
+          detail::MulAtB<1>(R, off, off);
+          obs_off.insert(obs_off.end(), off, off + 3);
+          obs_cal.push_back(cameras[im.camera_id].has_prior_focal_length ? 1 : 0);
         } else {
-          for (int k = 0; k < 3; ++k) obs_dir.push_back(R[k] * b[0] + R[3 + k] * b[1] + R[6 + k] * b[2]);   // R^T b (.cc:294-296)
+          detail::MulAtB<1>(R, b, dir);           // R^T b (.cc:294-296)
         }
+        obs_dir.insert(obs_dir.end(), dir, dir + 3);
         obs_cam.push_back(ci);
       }
       ptb.push_back((int64_t)obs_cam.size());
       const bool rnd = options_.optimize_points && options_.generate_random_points &&
-                       (int)t->observations.size() >= options_.min_num_view_per_track;
-      for (int k = 0; k < 3; ++k) points[3 * (size_t)p + k] = rnd ? 100.0 * U(random_generator_) : t->xyz[k];   // .cc:261-264
-      if (rnd) t->is_initialized = true;
-      ++p;
+                       (int)t.observations.size() >= options_.min_num_view_per_track;
+      for (int k = 0; k < 3; ++k) points[3 * (size_t)p + k] = rnd ? 100.0 * U(random_generator_) : t.xyz[k];   // .cc:261-264
+      if (rnd) t.is_initialized = true;
     }
     std::vector<double> scales(obs_cam.size(), 1.0);                                          // .cc:298
     b200sfm_gp_opts o;
@@ -426,11 +545,11 @@ class GlobalPositioner {
         rc = b200sfm_gp_problem_get_rig_unknown(prob, ucen.data());
         if (rc == B200SFM_OK)
           for (auto& [key, idx] : usens) {   // ConvertResults: centre -> translation = -(R_cr u)  (.cc:578-582)
-            Rigid3d cfr = b200host_adapt::CamFromRig(rigs[key.first], key.second);
-            double Rs[9];
-            QuatToR(cfr.rotation.coeffs().data(), Rs);
-            for (int k = 0; k < 3; ++k)
-              cfr.translation[k] = -(Rs[3 * k] * ucen[3 * idx] + Rs[3 * k + 1] * ucen[3 * idx + 1] + Rs[3 * k + 2] * ucen[3 * idx + 2]);
+            Rigid3d cfr = urot[idx];
+            double Rs[9], t[3];
+            detail::QuatToR(cfr.rotation.coeffs().data(), Rs);
+            detail::MulAB<1>(Rs, &ucen[3 * (size_t)idx], t);
+            for (int k = 0; k < 3; ++k) cfr.translation[k] = -t[k];
             b200host_adapt::SetCamFromRig(rigs[key.first], key.second, cfr);
           }
       }
@@ -440,14 +559,13 @@ class GlobalPositioner {
                             calibrated.data(), nullptr, centers.data(), points.data(), scales.data(), &summary);
     }
     if (rc != B200SFM_OK) { std::fprintf(stderr, "b200sfm_gp_solve: %s\n", b200sfm_last_error(ctx)); return false; }
-    for (auto& [id, f] : fsorted) {                                                           // ConvertResults: t = -R c (.cc:566-568)
-      const int i = fidx[id];
-      const double* R = &Rm[9 * (size_t)i];
-      for (int k = 0; k < 3; ++k)
-        f->RigFromWorld().translation[k] = -(R[3 * k] * centers[3 * i] + R[3 * k + 1] * centers[3 * i + 1] + R[3 * k + 2] * centers[3 * i + 2]);
+    for (int i = 0; i < C; ++i) {                                                             // ConvertResults: t = -R c (.cc:566-568)
+      double t[3];
+      detail::MulAB<1>(&Rm[9 * (size_t)i], &centers[3 * (size_t)i], t);
+      for (int k = 0; k < 3; ++k) fsorted[i].second->RigFromWorld().translation[k] = -t[k];
     }
-    p = 0;
-    for (auto& [id, t] : tsorted) { for (int k = 0; k < 3; ++k) t->xyz[k] = points[3 * (size_t)p + k]; ++p; }
+    for (int p = 0; p < P; ++p)
+      for (int k = 0; k < 3; ++k) tsorted[p].second->xyz[k] = points[3 * (size_t)p + k];
     return summary.usable != 0;
   }
 
@@ -470,6 +588,20 @@ struct RotationEstimatorOptions {   // global_rotation_averaging.h:39-75
   double pcg_rel_tolerance = 1e-8;
 };
 
+namespace detail {
+inline b200sfm_ra_opts RaOpts(const RotationEstimatorOptions& options) {
+  b200sfm_ra_opts o;
+  b200sfm_ra_default_opts(&o);
+  o.max_num_l1_iterations = options.max_num_l1_iterations; o.max_num_irls_iterations = options.max_num_irls_iterations;
+  o.l1_step_convergence_threshold = options.l1_step_convergence_threshold;
+  o.irls_step_convergence_threshold = options.irls_step_convergence_threshold;
+  o.irls_loss_parameter_sigma = options.irls_loss_parameter_sigma;
+  o.weight_type = options.weight_type == RotationEstimatorOptions::HALF_NORM ? 1 : 0;
+  o.use_weight = options.use_weight; o.pcg_rel_tolerance = options.pcg_rel_tolerance;
+  return o;
+}
+}  // namespace detail
+
 class RotationEstimator {
  public:
   explicit RotationEstimator(const RotationEstimatorOptions& options) : options_(options) {}
@@ -487,21 +619,14 @@ class RotationEstimator {
       auto f = frames.find(im.frame_id);
       return f != frames.end() && f->second.is_registered;
     };
-    std::map<image_t, int> idx;
-    std::vector<image_t> ids;
-    {
-      std::map<image_t, const Image*> isorted;
-      for (const auto& [id, im] : images) isorted[id] = &im;
-      for (const auto& [id, im] : isorted)
-        if (registered(*im)) { idx[id] = (int)ids.size(); ids.push_back(id); }
-    }
-    const int n = (int)ids.size();
+    const auto isorted = detail::SortedEntries(images, registered);
+    const auto idx = detail::PositionOf(isorted);
+    const int n = (int)isorted.size();
     if (n == 0) return;
     struct Edge { double w; int a, b; const ImagePair* pr; };
-    std::map<image_pair_t, const ImagePair*> psorted;
+    const auto psorted = detail::SortedEntries(view_graph.image_pairs, [](const ImagePair& pr) { return pr.is_valid; });
     double max_w = 0;
-    for (const auto& [id, pr] : view_graph.image_pairs)
-      if (pr.is_valid) { psorted[id] = &pr; max_w = std::max(max_w, (double)pr.inliers.size()); }   // tree.cc:93-100 (INLIER_NUM)
+    for (const auto& [id, pr] : psorted) max_w = std::max(max_w, (double)pr->inliers.size());   // tree.cc:93-100 (INLIER_NUM)
     std::vector<Edge> edges;
     for (const auto& [id, pr] : psorted) {
       auto a = idx.find(pr->image_id1), b = idx.find(pr->image_id2);
@@ -533,12 +658,12 @@ class RotationEstimator {
         if (seen[nb]) continue;
         seen[nb] = 1;
         const double* r21 = pr->cam2_from_cam1.rotation.coeffs().data();
-        if (pr->image_id1 == ids[nb]) {          // 1_R_w = 2_R_1^T * 2_R_w   (.cc:125-129)
+        if (pr->image_id1 == isorted[nb].first) {   // 1_R_w = 2_R_1^T * 2_R_w   (.cc:125-129)
           double inv[4];
-          QuatConj(r21, inv);
-          QuatMul(inv, q[cur].data(), q[nb].data());
-        } else {                                 // 2_R_w = 2_R_1 * 1_R_w     (.cc:130-134)
-          QuatMul(r21, q[cur].data(), q[nb].data());
+          detail::QuatConj(r21, inv);
+          detail::QuatMul(inv, q[cur].data(), q[nb].data());
+        } else {                                    // 2_R_w = 2_R_1 * 1_R_w     (.cc:130-134)
+          detail::QuatMul(r21, q[cur].data(), q[nb].data());
         }
         bfs.push(nb);
       }
@@ -547,17 +672,15 @@ class RotationEstimator {
     std::map<frame_t, std::vector<std::array<double, 4>>> per_frame;
     for (int i = 0; i < n; ++i) {
       if (!seen[i]) continue;                    // not reached by the tree: not estimated (rotation_initializer.cc:101-102)
-      const Image& im = images.at(ids[i]);
+      const Image& im = *isorted[i].second;
       std::array<double, 4> r = q[i];
-      if (!im.HasTrivialFrame()) {
-        Rig& rig = rigs[frames[im.frame_id].RigId()];
-        if (!b200host_adapt::IsRefSensor(rig, im.camera_id)) {
-          if (!b200host_adapt::HasCamFromRig(rig, im.camera_id)) continue;                    // .cc:108-111
-          const Rigid3d c = b200host_adapt::CamFromRig(rig, im.camera_id);
-          double inv[4];
-          QuatConj(c.rotation.coeffs().data(), inv);
-          QuatMul(inv, q[i].data(), r.data());
-        }
+      Rigid3d c;
+      const auto s = detail::ResolveCamFromRig(im.HasTrivialFrame() ? nullptr : &rigs[frames[im.frame_id].RigId()], im, c);
+      if (s == detail::CamFromRigStatus::kMissing) continue;                                  // .cc:108-111
+      if (s == detail::CamFromRigStatus::kKnown) {
+        double inv[4];
+        detail::QuatConj(c.rotation.coeffs().data(), inv);
+        detail::QuatMul(inv, q[i].data(), r.data());
       }
       per_frame[im.frame_id].push_back(r);
     }
@@ -585,43 +708,33 @@ class RotationEstimator {
     if (!ctx) return false;
     if (!options_.skip_initialization && !options_.use_gravity)                               // .cc:60-63
       InitializeFromMaximumSpanningTree(view_graph, rigs, frames, images);
-    std::map<frame_t, Frame*> fsorted;
-    for (auto& [id, f] : frames)
-      if (f.is_registered) fsorted[id] = &f;
-    std::map<frame_t, int> fidx;
-    for (auto& [id, f] : fsorted) { const int i = (int)fidx.size(); fidx[id] = i; }
+    const auto fsorted = detail::SortedEntries(frames, [](const Frame& f) { return f.is_registered; });
+    const auto fidx = detail::PositionOf(fsorted);
     const int n = (int)fsorted.size();
     if (n == 0) return false;
     std::vector<double> theta(3 * (size_t)n);
-    for (auto& [id, f] : fsorted) QuatToAngleAxis(f->RigFromWorld().rotation.coeffs().data(), &theta[3 * (size_t)fidx[id]]);   // .cc:223-224
+    for (int i = 0; i < n; ++i) detail::QuatToAngleAxis(fsorted[i].second->RigFromWorld().rotation.coeffs().data(), &theta[3 * (size_t)i]);   // .cc:223-224
     // Cameras whose cam_from_rig rotation has to be estimated (.cc:162-194): non-reference sensors of the rigs of the
     // registered images without a cam_from_rig, or with one whose translation is still NaN (its rotation is then the
     // initial value, .cc:186-190; else zero, .cc:239-241).  They become nodes n, n + 1, ... in ascending camera id.
-    std::map<camera_t, rig_t> cam_rig;
+    std::map<camera_t, std::pair<rig_t, const Image*>> cam_rig;   // the rig and an image of the camera
     for (auto& [id, im] : images) {
       const auto fit = frames.find(im.frame_id);
       if (fit == frames.end() || !fit->second.is_registered) continue;
       if (im.HasTrivialFrame()) continue;   // == IsRefSensor of its rig (scene/image.h:73-76): never estimated
-      cam_rig[im.camera_id] = fit->second.RigId();
+      cam_rig[im.camera_id] = {fit->second.RigId(), &im};
     }
     std::map<camera_t, int> ucam;
-    for (auto& [cam, rig_id] : cam_rig) {
-      Rig& rig = rigs[rig_id];
-      if (b200host_adapt::IsRefSensor(rig, cam)) continue;
-      const bool has = b200host_adapt::HasCamFromRig(rig, cam);
-      bool nan_t = false;
-      if (has) {
-        const Rigid3d c = b200host_adapt::CamFromRig(rig, cam);
-        for (int k = 0; k < 3; ++k) nan_t = nan_t || std::isnan(c.translation[k]);
-      }
-      if (!has || nan_t) {
+    for (auto& [cam, rig_im] : cam_rig) {
+      Rigid3d c;
+      const auto s = detail::ResolveCamFromRig(&rigs[rig_im.first], *rig_im.second, c);
+      if (s == detail::CamFromRigStatus::kIdentity) continue;
+      const bool has = s == detail::CamFromRigStatus::kKnown;
+      if (!has || std::isnan(c.translation[0]) || std::isnan(c.translation[1]) || std::isnan(c.translation[2])) {
         const int node = n + (int)ucam.size();
         ucam[cam] = node;
         double aa[3] = {0, 0, 0};
-        if (has) {
-          const Rigid3d c = b200host_adapt::CamFromRig(rig, cam);
-          QuatToAngleAxis(c.rotation.coeffs().data(), aa);
-        }
+        if (has) detail::QuatToAngleAxis(c.rotation.coeffs().data(), aa);
         theta.insert(theta.end(), aa, aa + 3);
       }
     }
@@ -633,26 +746,29 @@ class RotationEstimator {
     int fixed_frame = 0;
     bool any_gravity = false;
     if (options_.use_gravity) {
-      for (auto& [id, f] : fsorted) {
-        if (!f->HasGravity()) continue;
-        const int i = fidx[id];
+      for (int i = 0; i < n; ++i) {
+        const Frame& f = *fsorted[i].second;
+        if (!f.HasGravity()) continue;
         double* Ra = &R_align[9 * (size_t)i];
-        b200host_adapt::RAlignRowMajor(*f, Ra);
+        b200host_adapt::RAlignRowMajor(f, Ra);
         double R0[9], M[9], q[4], aa[3];
-        QuatToR(f->RigFromWorld().rotation.coeffs().data(), R0);
-        for (int r = 0; r < 3; ++r)
-          for (int c = 0; c < 3; ++c) M[3 * r + c] = Ra[r] * R0[c] + Ra[3 + r] * R0[3 + c] + Ra[6 + r] * R0[6 + c];   // R_align^T R
-        RToQuat(M, q);
-        QuatToAngleAxis(q, aa);
+        detail::QuatToR(f.RigFromWorld().rotation.coeffs().data(), R0);
+        detail::MulAtB(Ra, R0, M);   // R_align^T R
+        detail::RToQuat(M, q);
+        detail::QuatToAngleAxis(q, aa);
         theta[3 * (size_t)i] = 0.0; theta[3 * (size_t)i + 1] = aa[1]; theta[3 * (size_t)i + 2] = 0.0;
         has_gravity[i] = 1;
         if (!any_gravity) fixed_frame = i;
         any_gravity = true;
       }
     }
-    std::map<image_pair_t, const ImagePair*> psorted;
-    for (const auto& [id, pr] : view_graph.image_pairs)
-      if (pr.is_valid) psorted[id] = &pr;
+    // cam_from_rig of an image of a known rig as a matrix (a missing one counts as the identity)
+    auto Rc = [&](const Image& im, double out[9]) {
+      Rigid3d c;
+      detail::ResolveCamFromRig(&rigs[frames[im.frame_id].RigId()], im, c);
+      detail::QuatToR(c.rotation.coeffs().data(), out);
+    };
+    const auto psorted = detail::SortedEntries(view_graph.image_pairs, [](const ImagePair& pr) { return pr.is_valid; });
     std::vector<int32_t> ei, ej, eci, ecj;
     std::vector<double> Rrel, w;
     for (const auto& [id, pr] : psorted) {
@@ -661,7 +777,7 @@ class RotationEstimator {
       const auto f1 = fidx.find(i1->second.frame_id), f2 = fidx.find(i2->second.frame_id);
       if (f1 == fidx.end() || f2 == fidx.end()) continue;                                     // .cc:365-368
       double R[9];
-      QuatToR(pr->cam2_from_cam1.rotation.coeffs().data(), R);
+      detail::QuatToR(pr->cam2_from_cam1.rotation.coeffs().data(), R);
       // known rigs: the unknowns are the frame rotations, R_rel = R_c2r2^T R_21 R_c1r1 (.cc:274-309); an image
       // pair inside one frame is a self loop and is skipped (.cc:300-303)
       // (has_sensor_from_rig of the reference: a non-reference sensor with a KNOWN cam_from_rig; an unknown one
@@ -670,36 +786,12 @@ class RotationEstimator {
       const bool rig1 = !i1->second.HasTrivialFrame() && u1 == ucam.end();
       const bool rig2 = !i2->second.HasTrivialFrame() && u2 == ucam.end();
       if (rig1 && rig2 && f1->second == f2->second) continue;
-      if (rig1) {
-        const Rigid3d c = b200host_adapt::CamFromRig(rigs[frames[i1->second.frame_id].RigId()], i1->second.camera_id);
-        double Rc[9], T[9];
-        QuatToR(c.rotation.coeffs().data(), Rc);
-        for (int r = 0; r < 3; ++r)
-          for (int k = 0; k < 3; ++k) T[3 * r + k] = R[3 * r] * Rc[k] + R[3 * r + 1] * Rc[3 + k] + R[3 * r + 2] * Rc[6 + k];
-        std::copy(T, T + 9, R);
-      }
-      if (rig2) {
-        const Rigid3d c = b200host_adapt::CamFromRig(rigs[frames[i2->second.frame_id].RigId()], i2->second.camera_id);
-        double Rc[9], T[9];
-        QuatToR(c.rotation.coeffs().data(), Rc);
-        for (int r = 0; r < 3; ++r)   // Rc^T R
-          for (int k = 0; k < 3; ++k) T[3 * r + k] = Rc[r] * R[k] + Rc[3 + r] * R[3 + k] + Rc[6 + r] * R[6 + k];
-        std::copy(T, T + 9, R);
-      }
+      double T[9];
+      if (rig1) { Rc(i1->second, T); detail::MulAB(R, T, R); }
+      if (rig2) { Rc(i2->second, T); detail::MulAtB(T, R, R); }                               // Rc^T R
       if (any_gravity) {   // align the relative rotation with the gravity frames (.cc:311-326)
-        double T[9];
-        if (has_gravity[f1->second]) {
-          const double* Ra = &R_align[9 * (size_t)f1->second];
-          for (int r = 0; r < 3; ++r)
-            for (int k = 0; k < 3; ++k) T[3 * r + k] = R[3 * r] * Ra[k] + R[3 * r + 1] * Ra[3 + k] + R[3 * r + 2] * Ra[6 + k];
-          std::copy(T, T + 9, R);
-        }
-        if (has_gravity[f2->second]) {
-          const double* Ra = &R_align[9 * (size_t)f2->second];
-          for (int r = 0; r < 3; ++r)   // R_align^T R
-            for (int k = 0; k < 3; ++k) T[3 * r + k] = Ra[r] * R[k] + Ra[3 + r] * R[3 + k] + Ra[6 + r] * R[6 + k];
-          std::copy(T, T + 9, R);
-        }
+        if (has_gravity[f1->second]) detail::MulAB(R, &R_align[9 * (size_t)f1->second], R);
+        if (has_gravity[f2->second]) detail::MulAtB(&R_align[9 * (size_t)f2->second], R, R);   // R_align^T R
       }
       ei.push_back(f1->second);
       ej.push_back(f2->second);
@@ -708,14 +800,7 @@ class RotationEstimator {
       Rrel.insert(Rrel.end(), R, R + 9);
       w.push_back(pr->weight);
     }
-    b200sfm_ra_opts o;
-    b200sfm_ra_default_opts(&o);
-    o.max_num_l1_iterations = options_.max_num_l1_iterations; o.max_num_irls_iterations = options_.max_num_irls_iterations;
-    o.l1_step_convergence_threshold = options_.l1_step_convergence_threshold;
-    o.irls_step_convergence_threshold = options_.irls_step_convergence_threshold;
-    o.irls_loss_parameter_sigma = options_.irls_loss_parameter_sigma;
-    o.weight_type = options_.weight_type == RotationEstimatorOptions::HALF_NORM ? 1 : 0;
-    o.use_weight = options_.use_weight; o.pcg_rel_tolerance = options_.pcg_rel_tolerance;
+    const b200sfm_ra_opts o = detail::RaOpts(options_);
     int rc;
     if (n_cams > 0) {   // frames that hold an image of each unknown camera (the quaternion average of .cc:675-693 runs over them)
       std::map<camera_t, std::set<int>> cam_frames_of;
@@ -739,68 +824,27 @@ class RotationEstimator {
     }
     if (rc != B200SFM_OK) { std::fprintf(stderr, "b200sfm_ra_solve: %s\n", b200sfm_last_error(ctx)); return false; }
     if (!summary.usable) return false;                                                        // NaN (.cc:508-512,590-593)
-    for (auto& [id, f] : fsorted) {                                                           // ConvertResults (.cc:787-798)
-      const int i = fidx[id];
-      double* qout = f->RigFromWorld().rotation.coeffs().data();
+    for (int i = 0; i < n; ++i) {                                                             // ConvertResults (.cc:787-798)
+      Rigid3d& pose = fsorted[i].second->RigFromWorld();
+      double* qout = pose.rotation.coeffs().data();
       if (has_gravity[i]) {   // R = R_align * AngleToRotUp(phi)
-        double qa[4], Ry[9], M[9];
-        AngleAxisToQuat(&theta[3 * (size_t)i], qa);
-        QuatToR(qa, Ry);
-        const double* Ra = &R_align[9 * (size_t)i];
-        for (int r = 0; r < 3; ++r)
-          for (int c = 0; c < 3; ++c) M[3 * r + c] = Ra[3 * r] * Ry[c] + Ra[3 * r + 1] * Ry[3 + c] + Ra[3 * r + 2] * Ry[6 + c];
-        RToQuat(M, qout);
+        double qa[4], M[9];
+        detail::AngleAxisToQuat(&theta[3 * (size_t)i], qa);
+        detail::QuatToR(qa, M);
+        detail::MulAB(&R_align[9 * (size_t)i], M, M);
+        detail::RToQuat(M, qout);
       } else {
-        AngleAxisToQuat(&theta[3 * (size_t)i], qout);
+        detail::AngleAxisToQuat(&theta[3 * (size_t)i], qout);
       }
-      for (int k = 0; k < 3; ++k) f->RigFromWorld().translation[k] = 0.0;                     // Vector3d::Zero() (.cc:795)
+      for (int k = 0; k < 3; ++k) pose.translation[k] = 0.0;                                  // Vector3d::Zero() (.cc:795)
     }
     for (auto& [cam, node] : ucam) {   // the estimated cam_from_rig rotations, translation not known yet (.cc:800-813)
       Rigid3d c;
-      AngleAxisToQuat(&theta[3 * (size_t)node], c.rotation.coeffs().data());
+      detail::AngleAxisToQuat(&theta[3 * (size_t)node], c.rotation.coeffs().data());
       for (int k = 0; k < 3; ++k) c.translation[k] = std::numeric_limits<double>::quiet_NaN();
-      b200host_adapt::SetCamFromRig(rigs[cam_rig[cam]], cam, c);
+      b200host_adapt::SetCamFromRig(rigs[cam_rig[cam].first], cam, c);
     }
     return true;
-  }
-
-  // rotation matrix (row-major) -> unit quaternion xyzw, w >= 0 (Shepperd's branches, as Eigen's conversion)
-  static void RToQuat(const double* R, double* q) {
-    const double tr = R[0] + R[4] + R[8];
-    if (tr > 0) {
-      const double s = std::sqrt(tr + 1.0) * 2;
-      q[3] = 0.25 * s; q[0] = (R[7] - R[5]) / s; q[1] = (R[2] - R[6]) / s; q[2] = (R[3] - R[1]) / s;
-    } else if (R[0] > R[4] && R[0] > R[8]) {
-      const double s = std::sqrt(1.0 + R[0] - R[4] - R[8]) * 2;
-      q[3] = (R[7] - R[5]) / s; q[0] = 0.25 * s; q[1] = (R[1] + R[3]) / s; q[2] = (R[2] + R[6]) / s;
-    } else if (R[4] > R[8]) {
-      const double s = std::sqrt(1.0 + R[4] - R[0] - R[8]) * 2;
-      q[3] = (R[2] - R[6]) / s; q[0] = (R[1] + R[3]) / s; q[1] = 0.25 * s; q[2] = (R[5] + R[7]) / s;
-    } else {
-      const double s = std::sqrt(1.0 + R[8] - R[0] - R[4]) * 2;
-      q[3] = (R[3] - R[1]) / s; q[0] = (R[2] + R[6]) / s; q[1] = (R[5] + R[7]) / s; q[2] = 0.25 * s;
-    }
-    if (q[3] < 0) for (int k = 0; k < 4; ++k) q[k] = -q[k];
-  }
-
-  static void QuatToAngleAxis(const double* q, double* v) {
-    double n = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
-    if (n > 0) {
-      const double ang = 2 * std::atan2(n, std::fabs(q[3]));
-      const double f = (q[3] < 0 ? -ang : ang) / n;
-      v[0] = q[0] * f; v[1] = q[1] * f; v[2] = q[2] * f;
-    } else {
-      v[0] = v[1] = v[2] = 0;
-    }
-  }
-  static void AngleAxisToQuat(const double* v, double* q) {
-    const double n = std::sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
-    if (n > 0) {
-      const double s = std::sin(n / 2) / n;
-      q[0] = v[0] * s; q[1] = v[1] * s; q[2] = v[2] * s; q[3] = std::cos(n / 2);
-    } else {
-      q[0] = q[1] = q[2] = 0; q[3] = 1;
-    }
   }
 
  private:
@@ -829,10 +873,8 @@ template <class ViewGraphT, class InlierOptions>
 void ImagePairsInlierCount(ViewGraphT& view_graph, const std::unordered_map<camera_t, Camera>& cameras,
                            const std::unordered_map<image_t, Image>& images, const InlierOptions& options, bool clean_inliers) {
   using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
-  std::map<image_pair_t, Pair*> psorted;
-  for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
   std::vector<Pair*> scored;
-  for (auto& [id, pr] : psorted) {
+  for (auto& [id, pr] : detail::SortedEntries(view_graph.image_pairs)) {
     if (!clean_inliers && pr->inliers.size() > 0) continue;
     pr->inliers.clear();
     if (pr->is_valid) scored.push_back(pr);
@@ -840,24 +882,17 @@ void ImagePairsInlierCount(ViewGraphT& view_graph, const std::unordered_map<came
   if (scored.empty()) return;
   b200sfm_ctx* ctx = DefaultContext();
   if (!ctx) return;
-  std::map<camera_t, int> cidx;
-  for (auto& [id, c] : cameras) cidx[id] = 0;
+  const auto csorted = detail::SortedEntries(cameras);
+  const auto cidx = detail::PositionOf(csorted);
   std::vector<int32_t> intr_model;
-  std::vector<double> intr(cidx.size() * B200SFM_INTR_STRIDE, 0.0);
-  for (auto& [id, k] : cidx) {
-    k = (int)intr_model.size();
-    const Camera& c = cameras.at(id);
-    intr_model.push_back(static_cast<int32_t>(c.model_id));
-    for (size_t j = 0; j < c.params.size() && j < B200SFM_INTR_STRIDE; ++j) intr[(size_t)k * B200SFM_INTR_STRIDE + j] = c.params[j];
-  }
-  std::map<image_t, const Image*> isorted;
-  for (auto& [id, im] : images) isorted[id] = &im;
-  std::map<image_t, int> iidx;
+  std::vector<double> intr;
+  detail::PackCameras(csorted, intr_model, intr);
+  const auto isorted = detail::SortedEntries(images);
+  const auto iidx = detail::PositionOf(isorted);
   std::vector<int64_t> feature_begin(1, 0);
   std::vector<double> features;
   std::vector<int32_t> image_intr;
   for (auto& [id, im] : isorted) {
-    iidx[id] = (int)image_intr.size();
     auto c = cidx.find(im->camera_id);
     image_intr.push_back(c == cidx.end() ? -1 : c->second);
     for (const auto& f : im->features) { features.push_back(f[0]); features.push_back(f[1]); }
@@ -912,36 +947,28 @@ struct RelPoseFilter {
   template <class ViewGraphT, class ImageMap>
   static int64_t FilterRotations(ViewGraphT& view_graph, const ImageMap& images, double max_angle) {
     using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
-    using Img = typename ImageMap::mapped_type;
-    std::map<image_t, const Img*> isorted;
-    for (auto& [id, im] : images) isorted[id] = &im;
-    std::map<image_t, int32_t> iidx;
+    const auto isorted = detail::SortedEntries(images);
+    const auto iidx = detail::PositionOf(isorted);
     std::vector<double> quat;
     std::vector<uint8_t> reg;
     const double nan = std::numeric_limits<double>::quiet_NaN();
     for (auto& [id, im] : isorted) {
-      iidx[id] = (int32_t)reg.size();
       reg.push_back(im->IsRegistered() ? 1 : 0);
       double q[4] = {nan, nan, nan, nan};
       if (reg.back() && im->frame_ptr->HasPose()) {
         const double* r = im->frame_ptr->RigFromWorld().rotation.coeffs().data();
-        const auto* rig = im->frame_ptr->RigPtr();
-        double c[4];
-        if (im->HasTrivialFrame() || !rig || b200host_adapt::IsRefSensor(*rig, im->camera_id)) {
-          std::copy(r, r + 4, q);
-        } else if (b200host_adapt::FrameCamFromRig(*im->frame_ptr, im->camera_id, c)) {
-          QuatMul(c, r, q);
-        }
+        auto* rig = im->frame_ptr->RigPtr();
+        Rigid3d c;   // an image of a frame without a rig: the identity
+        const auto s = rig ? detail::ResolveCamFromRig(rig, *im, c) : detail::CamFromRigStatus::kIdentity;
+        if (s == detail::CamFromRigStatus::kIdentity) std::copy(r, r + 4, q);
+        if (s == detail::CamFromRigStatus::kKnown) detail::QuatMul(c.rotation.coeffs().data(), r, q);
       }
       quat.insert(quat.end(), q, q + 4);
     }
-    std::map<image_pair_t, Pair*> psorted;
-    for (auto& [id, pr] : view_graph.image_pairs)
-      if (pr.is_valid) psorted[id] = &pr;
     std::vector<Pair*> pairs;
     std::vector<int32_t> img1, img2;
     std::vector<double> rel;
-    for (auto& [id, pr] : psorted) {
+    for (auto& [id, pr] : detail::SortedEntries(view_graph.image_pairs, [](const Pair& p) { return p.is_valid; })) {
       auto a = iidx.find(pr->image_id1), b = iidx.find(pr->image_id2);
       if (a == iidx.end() || b == iidx.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return -1; }
       pairs.push_back(pr);
@@ -976,34 +1003,22 @@ struct RelPoseFilter {
 template <class ViewGraphT, class FrameMap, class ImageMap>
 int KeepLargestConnectedComponentsDevice(ViewGraphT& view_graph, FrameMap& frames, ImageMap& images) {
   using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
-  using Frm = typename FrameMap::mapped_type;
-  std::map<frame_t, Frm*> fsorted;
-  for (auto& [id, f] : frames) fsorted[id] = &f;
-  std::map<frame_t, int32_t> fidx;
-  std::vector<Frm*> fr;
+  const auto fr = detail::SortedEntries(frames);
+  const auto fidx = detail::PositionOf(fr);
   std::vector<uint8_t> reg;
-  for (auto& [id, f] : fsorted) {
-    fidx[id] = (int32_t)fr.size();
-    fr.push_back(f);
-    reg.push_back(f->is_registered ? 1 : 0);
-  }
-  std::map<image_t, int32_t> iidx;
-  std::vector<image_t> ids;
-  for (auto& [id, im] : images) ids.push_back(id);
-  std::sort(ids.begin(), ids.end());
+  for (auto& [id, f] : fr) reg.push_back(f->is_registered ? 1 : 0);
+  const auto isorted = detail::SortedEntries(images);
+  const auto iidx = detail::PositionOf(isorted);
   std::vector<int32_t> image_frame;
-  for (image_t id : ids) {
-    auto f = fidx.find(images.at(id).frame_id);
+  for (auto& [id, im] : isorted) {
+    auto f = fidx.find(im->frame_id);
     if (f == fidx.end()) { std::fprintf(stderr, "b200sfm: image of an unknown frame\n"); return 0; }
-    iidx[id] = (int32_t)image_frame.size();
     image_frame.push_back(f->second);
   }
-  std::map<image_pair_t, Pair*> psorted;
-  for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
   std::vector<Pair*> pairs;
   std::vector<int32_t> img1, img2;
   std::vector<uint8_t> valid;
-  for (auto& [id, pr] : psorted) {
+  for (auto& [id, pr] : detail::SortedEntries(view_graph.image_pairs)) {
     auto a = iidx.find(pr->image_id1), b = iidx.find(pr->image_id2);
     if (a == iidx.end() || b == iidx.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return 0; }
     pairs.push_back(pr);
@@ -1022,7 +1037,7 @@ int KeepLargestConnectedComponentsDevice(ViewGraphT& view_graph, FrameMap& frame
     return 0;
   }
   if (n == 0) return 0;
-  for (size_t f = 0; f < fr.size(); ++f) fr[f]->is_registered = reg[f] != 0;
+  for (size_t f = 0; f < fr.size(); ++f) fr[f].second->is_registered = reg[f] != 0;
   for (size_t e = 0; e < pairs.size(); ++e) pairs[e]->is_valid = valid[e] != 0;
   return n;
 }
@@ -1088,18 +1103,11 @@ class ViewGraphCalibrator {
   template <class ViewGraphT, class CameraMap, class ImageMap>
   bool Solve(ViewGraphT& view_graph, CameraMap& cameras, ImageMap& images) {
     using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
-    using Cam = typename CameraMap::mapped_type;
-    std::map<image_pair_t, Pair*> psorted;
-    for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
-    std::map<camera_t, Cam*> csorted;
-    for (auto& [id, c] : cameras) csorted[id] = &c;
-    std::map<camera_t, int> cidx;
-    std::vector<Cam*> cams;
+    const auto cams = detail::SortedEntries(cameras);
+    const auto cidx = detail::PositionOf(cams);
     std::vector<double> pp, focal;
     std::vector<uint8_t> prior;
-    for (auto& [id, c] : csorted) {
-      cidx[id] = (int)cams.size();
-      cams.push_back(c);
+    for (auto& [id, c] : cams) {
       double p[2];
       VgcPrincipalPoint(*c, p);
       pp.push_back(p[0]); pp.push_back(p[1]);
@@ -1109,7 +1117,7 @@ class ViewGraphCalibrator {
     std::vector<Pair*> qual;
     std::vector<int32_t> cam1, cam2;
     std::vector<double> F;
-    for (auto& [id, pr] : psorted) {
+    for (auto& [id, pr] : detail::SortedEntries(view_graph.image_pairs)) {
       if (pr->config != B200SFM_TWO_VIEW_CALIBRATED && pr->config != B200SFM_TWO_VIEW_UNCALIBRATED) continue;
       if (!pr->is_valid) continue;
       auto a = images.find(pr->image_id1), b = images.find(pr->image_id2);
@@ -1149,8 +1157,8 @@ class ViewGraphCalibrator {
     }
     for (int32_t k = 0; k < K; ++k) {
       if (!accepted[k]) continue;
-      cams[k]->has_refined_focal_length = true;
-      for (const size_t idx : VgcFocalLengthIdxs(*cams[k])) cams[k]->params[idx] = focal[k];
+      cams[k].second->has_refined_focal_length = true;
+      for (const size_t idx : VgcFocalLengthIdxs(*cams[k].second)) cams[k].second->params[idx] = focal[k];
     }
     for (int64_t e = 0; e < E; ++e)
       if (!valid[e]) qual[e]->is_valid = false;
@@ -1173,27 +1181,18 @@ struct ViewGraphManipulater {
   template <class ViewGraphT, class CameraMap, class ImageMap>
   static int64_t UpdateImagePairsConfig(ViewGraphT& view_graph, const CameraMap& cameras, const ImageMap& images) {
     using Pair = typename std::remove_reference<decltype(view_graph.image_pairs.begin()->second)>::type;
-    std::map<camera_t, int32_t> cidx;
-    for (auto& [id, c] : cameras) cidx[id] = 0;
+    const auto csorted = detail::SortedEntries(cameras);
+    const auto cidx = detail::PositionOf(csorted);
     std::vector<int32_t> model;
     std::vector<double> params;
+    detail::PackCameras(csorted, model, params);
     std::vector<uint8_t> prior;
-    for (auto& [id, k] : cidx) {
-      const auto& c = cameras.at(id);
-      k = (int32_t)model.size();
-      model.push_back(static_cast<int32_t>(c.model_id));
-      double p[B200SFM_INTR_STRIDE] = {0};
-      for (size_t i = 0; i < c.params.size() && i < (size_t)B200SFM_INTR_STRIDE; ++i) p[i] = c.params[i];
-      params.insert(params.end(), p, p + B200SFM_INTR_STRIDE);
-      prior.push_back(c.has_prior_focal_length ? 1 : 0);
-    }
-    std::map<image_pair_t, Pair*> psorted;
-    for (auto& [id, pr] : view_graph.image_pairs) psorted[id] = &pr;
+    for (auto& [id, c] : csorted) prior.push_back(c->has_prior_focal_length ? 1 : 0);
     std::vector<Pair*> pairs;
     std::vector<int32_t> cam1, cam2, config;
     std::vector<uint8_t> valid;
     std::vector<double> quat, trans, F;
-    for (auto& [id, pr] : psorted) {
+    for (auto& [id, pr] : detail::SortedEntries(view_graph.image_pairs)) {
       auto a = images.find(pr->image_id1), b = images.find(pr->image_id2);
       if (a == images.end() || b == images.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return -1; }
       auto ca = cidx.find(a->second.camera_id), cb = cidx.find(b->second.camera_id);
@@ -1241,16 +1240,8 @@ template <class FrameMap, class ImageMap, class TrackMap>
 image_t PruneWeaklyConnectedImages(FrameMap& frames, ImageMap& images, TrackMap& tracks, int min_num_images = 2,
                                    int min_num_observations = 0) {
   (void)min_num_images;
-  using Frm = typename FrameMap::mapped_type;
-  using Trk = typename TrackMap::mapped_type;
-  std::map<frame_t, Frm*> fsorted;
-  for (auto& [id, f] : frames) fsorted[id] = &f;
-  std::map<frame_t, int32_t> fidx;
-  std::vector<Frm*> fr;
-  for (auto& [id, f] : fsorted) {
-    fidx[id] = (int32_t)fr.size();
-    fr.push_back(f);
-  }
+  const auto fr = detail::SortedEntries(frames);
+  const auto fidx = detail::PositionOf(fr);
   const int32_t F = (int32_t)fr.size();
   std::vector<int32_t> images_of(F, 0);
   for (auto& [id, im] : images) {
@@ -1260,10 +1251,9 @@ image_t PruneWeaklyConnectedImages(FrameMap& frames, ImageMap& images, TrackMap&
   std::vector<uint8_t> self_loop(F), reg(F);
   for (int32_t f = 0; f < F; ++f) {
     self_loop[f] = images_of[f] >= 2 ? 1 : 0;
-    reg[f] = fr[f]->is_registered ? 1 : 0;
+    reg[f] = fr[f].second->is_registered ? 1 : 0;
   }
-  std::map<track_t, const Trk*> tsorted;
-  for (auto& [id, t] : tracks) tsorted[id] = &t;
+  const auto tsorted = detail::SortedEntries(tracks);
   std::vector<int64_t> begin{0};
   std::vector<int32_t> obs_frame;
   for (auto& [id, t] : tsorted) {
@@ -1287,8 +1277,8 @@ image_t PruneWeaklyConnectedImages(FrameMap& frames, ImageMap& images, TrackMap&
     return 0;
   }
   for (int32_t f = 0; f < F; ++f) {
-    fr[f]->is_registered = reg[f] != 0;
-    fr[f]->cluster_id = cluster[f];
+    fr[f].second->is_registered = reg[f] != 0;
+    fr[f].second->cluster_id = cluster[f];
   }
   return (image_t)num_clusters;
 }
@@ -1328,12 +1318,9 @@ class TrackEngine {
   }
 
   size_t EstablishFullTracks(std::unordered_map<track_t, Track>& tracks) {
-    using Pair = typename std::remove_reference<decltype(view_graph_.image_pairs.begin()->second)>::type;
-    std::map<image_pair_t, const Pair*> psorted;
-    for (const auto& [id, pr] : view_graph_.image_pairs) psorted[id] = &pr;
     std::vector<uint64_t> g1, g2;
     std::vector<double> xy1, xy2;
-    for (const auto& [id, pr] : psorted) {
+    for (const auto& [id, pr] : detail::SortedEntries(view_graph_.image_pairs)) {
       if (!pr->is_valid) continue;
       auto a = images_.find(pr->image_id1), b = images_.find(pr->image_id2);
       if (a == images_.end() || b == images_.end()) { std::fprintf(stderr, "b200sfm: image pair with an unknown image\n"); return 0; }
@@ -1375,8 +1362,7 @@ class TrackEngine {
 
   size_t FindTracksForProblem(const std::unordered_map<track_t, Track>& tracks_full,
                               std::unordered_map<track_t, Track>& tracks_selected) {
-    std::map<track_t, const Track*> tsorted;
-    for (const auto& [id, t] : tracks_full) tsorted[id] = &t;
+    const auto tsorted = detail::SortedEntries(tracks_full);
     std::vector<uint64_t> ids;
     std::vector<int64_t> begin{0};
     std::vector<uint32_t> obs_image;
@@ -1448,46 +1434,36 @@ class GravityRefiner {
 
   template <class ViewGraphT, class FrameMap, class ImageMap>
   void RefineGravity(const ViewGraphT& view_graph, FrameMap& frames, ImageMap& images) {
-    using Frm = typename FrameMap::mapped_type;
-    std::map<frame_t, Frm*> fsorted;
-    for (auto& [id, f] : frames) fsorted[id] = &f;
-    std::map<frame_t, int32_t> fidx;
-    std::vector<Frm*> fr;
-    for (auto& [id, f] : fsorted) { fidx[id] = (int32_t)fr.size(); fr.push_back(f); }
+    using Pair = std::remove_reference_t<decltype(view_graph.image_pairs.begin()->second)>;
+    const auto fr = detail::SortedEntries(frames);
+    const auto fidx = detail::PositionOf(fr);
     const int32_t F = (int32_t)fr.size();
     std::vector<double> R_align(9 * (size_t)F, 0.0);
     std::vector<uint8_t> has(F, 0);
     for (int32_t f = 0; f < F; ++f) {
-      has[f] = fr[f]->HasGravity() ? 1 : 0;
-      if (has[f]) b200host_adapt::RAlignRowMajor(*fr[f], &R_align[9 * (size_t)f]);
+      has[f] = fr[f].second->HasGravity() ? 1 : 0;
+      if (has[f]) b200host_adapt::RAlignRowMajor(*fr[f].second, &R_align[9 * (size_t)f]);
     }
-    // an image's cam_from_rig rotation (identity for a trivial frame); false: the image has no gravity (image.h:78-84)
+    // an image's cam_from_rig rotation; false: the image has no gravity (image.h:78-84)
     auto cam_rot = [&](const auto& im, int32_t f, double R[9]) {
-      if (!has[f]) return false;
-      double q[4] = {0, 0, 0, 1};
-      if (!im.HasTrivialFrame() && !b200host_adapt::FrameCamFromRig(*fr[f], im.camera_id, q)) return false;
-      QuatToR(q, R);
+      Rigid3d c;
+      if (!has[f] || detail::ResolveCamFromRig(fr[f].second->RigPtr(), im, c) == detail::CamFromRigStatus::kMissing) return false;
+      detail::QuatToR(c.rotation.coeffs().data(), R);
       return true;
     };
-    using Pair = std::remove_reference_t<decltype(view_graph.image_pairs.begin()->second)>;
     std::vector<int32_t> f1, f2;
     std::vector<double> M;
-    std::map<image_pair_t, const Pair*> order;
-    for (const auto& [id, pr] : view_graph.image_pairs)
-      if (pr.is_valid) order[id] = &pr;
-    for (const auto& [id, pp] : order) {
+    for (const auto& [id, pp] : detail::SortedEntries(view_graph.image_pairs, [](const Pair& pr) { return pr.is_valid; })) {
       const Pair& pr = *pp;
       const auto i1 = images.find(pr.image_id1), i2 = images.find(pr.image_id2);
       if (i1 == images.end() || i2 == images.end()) continue;
       const auto a = fidx.find(i1->second.frame_id), b = fidx.find(i2->second.frame_id);
       if (a == fidx.end() || b == fidx.end()) continue;
-      double Rc1[9], Rc2[9], R[9], T[9], Me[9];
+      double Rc1[9], Rc2[9], Me[9];
       if (!cam_rot(i1->second, a->second, Rc1) || !cam_rot(i2->second, b->second, Rc2)) continue;   // .cc:62-64,149
-      QuatToR(pr.cam2_from_cam1.rotation.coeffs().data(), R);
-      for (int r = 0; r < 3; ++r)   // R Rc1
-        for (int c = 0; c < 3; ++c) T[3 * r + c] = R[3 * r] * Rc1[c] + R[3 * r + 1] * Rc1[3 + c] + R[3 * r + 2] * Rc1[6 + c];
-      for (int r = 0; r < 3; ++r)   // Rc2^T (R Rc1)
-        for (int c = 0; c < 3; ++c) Me[3 * r + c] = Rc2[r] * T[c] + Rc2[3 + r] * T[3 + c] + Rc2[6 + r] * T[6 + c];
+      detail::QuatToR(pr.cam2_from_cam1.rotation.coeffs().data(), Me);
+      detail::MulAB(Me, Rc1, Me);    // R Rc1
+      detail::MulAtB(Rc2, Me, Me);   // Rc2^T (R Rc1)
       f1.push_back(a->second);
       f2.push_back(b->second);
       M.insert(M.end(), Me, Me + 9);
@@ -1517,7 +1493,7 @@ class GravityRefiner {
       return;
     }
     for (int32_t f = 0; f < F; ++f)
-      if (status[f] == 2) b200host_adapt::SetFrameGravity(*fr[f], &g[3 * (size_t)f]);   // .cc:119-123
+      if (status[f] == 2) b200host_adapt::SetFrameGravity(*fr[f].second, &g[3 * (size_t)f]);   // .cc:119-123
     std::fprintf(stderr, "Number of rectified frames: %d / %d\n", summary.rectified_frames, summary.error_prone_frames);
   }
 
@@ -1622,65 +1598,57 @@ inline bool RigRotationPrePass(ViewGraph& view_graph, std::unordered_map<rig_t, 
   }
   b200sfm_ctx* ctx = DefaultContext();
   if (!ctx) return false;
-  using RE = RotationEstimator;
   // 1. registered frames, images and cameras in sorted-id order
-  std::map<frame_t, int> fidx;
-  for (auto& [id, f] : frames)
-    if (f.is_registered) fidx[id] = 0;
-  std::vector<frame_t> fids;
-  for (auto& [id, k] : fidx) { k = (int)fids.size(); fids.push_back(id); }
-  std::map<image_t, Image*> isorted;
-  for (auto& [id, im] : images)
-    if (fidx.count(im.frame_id)) isorted[id] = &im;
-  const int F = (int)fids.size(), I = (int)isorted.size();
+  const auto fsorted = detail::SortedEntries(frames, [](const Frame& f) { return f.is_registered; });
+  const auto fidx = detail::PositionOf(fsorted);
+  const auto isorted = detail::SortedEntries(images, [&](const Image& im) { return fidx.count(im.frame_id) != 0; });
+  const auto iidx = detail::PositionOf(isorted);
+  const int F = (int)fsorted.size(), I = (int)isorted.size();
   if (F == 0 || I == 0) return false;
-  auto rig_of = [&](frame_t f) -> Rig* {
-    const auto it = rigs.find(frames[f].RigId());
+  auto rig_of = [&](const Frame& f) -> Rig* {
+    const auto it = rigs.find(f.RigId());
     return it == rigs.end() ? nullptr : &it->second;
   };
   std::map<camera_t, int> cidx;
-  std::map<camera_t, rig_t> cam_rig;
+  std::map<camera_t, std::pair<rig_t, const Image*>> cam_rig;   // the rig and an image of the camera
   for (auto& [id, im] : isorted) {
     cidx[im->camera_id] = 0;
-    cam_rig[im->camera_id] = frames[im->frame_id].RigId();
+    cam_rig[im->camera_id] = {frames[im->frame_id].RigId(), im};
   }
-  for (frame_t f : fids)
-    if (Rig* r = rig_of(f)) cidx[b200host_adapt::RefCameraId(*r)] = 0;
+  for (auto& [id, f] : fsorted)
+    if (Rig* r = rig_of(*f)) cidx[b200host_adapt::RefCameraId(*r)] = 0;
   std::vector<camera_t> cids;
   for (auto& [c, k] : cidx) { k = (int)cids.size(); cids.push_back(c); }
   const int K = (int)cids.size();
   std::vector<uint8_t> known(K, 1);
   std::vector<double> cq(4 * (size_t)K, 0.0), cq_triv;
   for (int c = 0; c < K; ++c) cq[4 * (size_t)c + 3] = 1.0;
-  for (auto& [cam, rig_id] : cam_rig) {
-    const auto it = rigs.find(rig_id);
-    if (it == rigs.end() || b200host_adapt::IsRefSensor(it->second, cam)) continue;
-    if (!b200host_adapt::HasCamFromRig(it->second, cam)) { known[cidx[cam]] = 0; continue; }
-    const Rigid3d c = b200host_adapt::CamFromRig(it->second, cam);
-    std::copy(c.rotation.coeffs().data(), c.rotation.coeffs().data() + 4, &cq[4 * (size_t)cidx[cam]]);
+  for (auto& [cam, rig_im] : cam_rig) {
+    const auto it = rigs.find(rig_im.first);
+    if (it == rigs.end()) continue;
+    Rigid3d c;
+    const auto s = detail::ResolveCamFromRig(&it->second, *rig_im.second, c);
+    if (s == detail::CamFromRigStatus::kMissing) known[cidx[cam]] = 0;
+    if (s == detail::CamFromRigStatus::kKnown)
+      std::copy(c.rotation.coeffs().data(), c.rotation.coeffs().data() + 4, &cq[4 * (size_t)cidx[cam]]);
   }
   cq_triv = cq;   // the trivial rigs: an unknown camera is the reference sensor of its own rig (identity)
   std::vector<int32_t> ref_cam(F), img_frame(I), img_cam(I), tf(I);
   for (int f = 0; f < F; ++f) {
-    Rig* r = rig_of(fids[f]);
+    Rig* r = rig_of(*fsorted[f].second);
     ref_cam[f] = r ? cidx[b200host_adapt::RefCameraId(*r)] : -1;
   }
-  std::map<image_t, int> iidx;
   std::vector<int32_t> tref(ref_cam);
-  {
-    int i = 0;
-    for (auto& [id, im] : isorted) {
-      iidx[id] = i;
-      img_frame[i] = fidx[im->frame_id];
-      img_cam[i] = cidx[im->camera_id];
-      if (ref_cam[img_frame[i]] < 0) ref_cam[img_frame[i]] = tref[img_frame[i]] = img_cam[i];   // no rig: the first image
-      if (known[img_cam[i]]) {
-        tf[i] = img_frame[i];
-      } else {
-        tf[i] = (int)tref.size();
-        tref.push_back(img_cam[i]);
-      }
-      ++i;
+  for (int i = 0; i < I; ++i) {
+    const Image& im = *isorted[i].second;
+    img_frame[i] = fidx.at(im.frame_id);
+    img_cam[i] = cidx[im.camera_id];
+    if (ref_cam[img_frame[i]] < 0) ref_cam[img_frame[i]] = tref[img_frame[i]] = img_cam[i];   // no rig: the first image
+    if (known[img_cam[i]]) {
+      tf[i] = img_frame[i];
+    } else {
+      tf[i] = (int)tref.size();
+      tref.push_back(img_cam[i]);
     }
   }
   for (int c = 0; c < K; ++c)
@@ -1689,14 +1657,9 @@ inline bool RigRotationPrePass(ViewGraph& view_graph, std::unordered_map<rig_t, 
   // 2. valid pairs between registered images, folded onto the trivial frames
   struct P { ImagePair* pr; int a, b; };
   std::vector<P> pairs;
-  {
-    std::map<image_pair_t, ImagePair*> psorted;
-    for (auto& [id, pr] : view_graph.image_pairs)
-      if (pr.is_valid) psorted[id] = &pr;
-    for (auto& [id, pr] : psorted) {
-      const auto a = iidx.find(pr->image_id1), b = iidx.find(pr->image_id2);
-      if (a != iidx.end() && b != iidx.end()) pairs.push_back({pr, a->second, b->second});
-    }
+  for (auto& [id, pr] : detail::SortedEntries(view_graph.image_pairs, [](const ImagePair& p) { return p.is_valid; })) {
+    const auto a = iidx.find(pr->image_id1), b = iidx.find(pr->image_id2);
+    if (a != iidx.end() && b != iidx.end()) pairs.push_back({pr, a->second, b->second});
   }
   // 3. largest component of the trivial frames (equally large: the one with the smallest frame)
   std::vector<int> comp(T, -1), size;
@@ -1738,7 +1701,7 @@ inline bool RigRotationPrePass(ViewGraph& view_graph, std::unordered_map<rig_t, 
   std::vector<double> mR, mw;
   for (const P& p : kept) {
     double R[9];
-    QuatToR(p.pr->cam2_from_cam1.rotation.coeffs().data(), R);
+    detail::QuatToR(p.pr->cam2_from_cam1.rotation.coeffs().data(), R);
     mi.push_back(inode[p.a]); mj.push_back(inode[p.b]);
     mR.insert(mR.end(), R, R + 9);
     mw.push_back((double)p.pr->inliers.size());                                               // tree.cc:93-100 (INLIER_NUM)
@@ -1756,7 +1719,7 @@ inline bool RigRotationPrePass(ViewGraph& view_graph, std::unordered_map<rig_t, 
     t_frame[i] = in_t[i] ? tf[i] : -1;
     if (in_t[i] && parent[inode[i]] >= 0) {
       est[i] = 1;
-      RE::RToQuat(&Rimg[9 * (size_t)inode[i]], &qimg[4 * (size_t)i]);
+      detail::RToQuat(&Rimg[9 * (size_t)inode[i]], &qimg[4 * (size_t)i]);
     } else {
       qimg[4 * (size_t)i + 3] = 1.0;
     }
@@ -1775,28 +1738,19 @@ inline bool RigRotationPrePass(ViewGraph& view_graph, std::unordered_map<rig_t, 
   std::vector<double> tR, tw, theta(3 * (size_t)nT);
   for (const P& p : kept) {
     if (tf[p.a] == tf[p.b]) continue;
-    double R21[9], Rc1[9], Rc2[9], A[9], B[9];
-    QuatToR(p.pr->cam2_from_cam1.rotation.coeffs().data(), R21);
-    QuatToR(&cq_triv[4 * (size_t)img_cam[p.a]], Rc1);
-    QuatToR(&cq_triv[4 * (size_t)img_cam[p.b]], Rc2);
-    for (int r = 0; r < 3; ++r)   // A = R21 Rc1
-      for (int k = 0; k < 3; ++k) A[3 * r + k] = R21[3 * r] * Rc1[k] + R21[3 * r + 1] * Rc1[3 + k] + R21[3 * r + 2] * Rc1[6 + k];
-    for (int r = 0; r < 3; ++r)   // B = Rc2^T A
-      for (int k = 0; k < 3; ++k) B[3 * r + k] = Rc2[r] * A[k] + Rc2[3 + r] * A[3 + k] + Rc2[6 + r] * A[6 + k];
+    double Rc1[9], Rc2[9], B[9];
+    detail::QuatToR(p.pr->cam2_from_cam1.rotation.coeffs().data(), B);
+    detail::QuatToR(&cq_triv[4 * (size_t)img_cam[p.a]], Rc1);
+    detail::QuatToR(&cq_triv[4 * (size_t)img_cam[p.b]], Rc2);
+    detail::MulAB(B, Rc1, B);    // R21 Rc1
+    detail::MulAtB(Rc2, B, B);   // Rc2^T R21 Rc1
     ti.push_back(tnode[tf[p.a]]); tj.push_back(tnode[tf[p.b]]);
     tR.insert(tR.end(), B, B + 9);
     tw.push_back(p.pr->weight);
   }
   for (int t = 0; t < T; ++t)
-    if (tnode[t] >= 0) RE::QuatToAngleAxis(&tq[4 * (size_t)t], &theta[3 * (size_t)tnode[t]]);
-  b200sfm_ra_opts o;
-  b200sfm_ra_default_opts(&o);
-  o.max_num_l1_iterations = options.max_num_l1_iterations; o.max_num_irls_iterations = options.max_num_irls_iterations;
-  o.l1_step_convergence_threshold = options.l1_step_convergence_threshold;
-  o.irls_step_convergence_threshold = options.irls_step_convergence_threshold;
-  o.irls_loss_parameter_sigma = options.irls_loss_parameter_sigma;
-  o.weight_type = options.weight_type == RotationEstimatorOptions::HALF_NORM ? 1 : 0;
-  o.use_weight = options.use_weight; o.pcg_rel_tolerance = options.pcg_rel_tolerance;
+    if (tnode[t] >= 0) detail::QuatToAngleAxis(&tq[4 * (size_t)t], &theta[3 * (size_t)tnode[t]]);
+  const b200sfm_ra_opts o = detail::RaOpts(options);
   b200sfm_ra_stats st{};
   rc = b200sfm_ra_solve(ctx, &o, nT, (int64_t)ti.size(), ti.data(), tj.data(), tR.data(), tw.data(), 0, theta.data(), &st);
   if (rc != B200SFM_OK) { std::fprintf(stderr, "b200sfm_ra_solve: %s\n", b200sfm_last_error(ctx)); return false; }
@@ -1804,12 +1758,12 @@ inline bool RigRotationPrePass(ViewGraph& view_graph, std::unordered_map<rig_t, 
     est[i] = in_t[i];
     if (!in_t[i]) continue;
     double qf[4];
-    RE::AngleAxisToQuat(&theta[3 * (size_t)tnode[tf[i]]], qf);
-    QuatMul(&cq_triv[4 * (size_t)img_cam[i]], qf, &qimg[4 * (size_t)i]);
+    detail::AngleAxisToQuat(&theta[3 * (size_t)tnode[tf[i]]], qf);
+    detail::QuatMul(&cq_triv[4 * (size_t)img_cam[i]], qf, &qimg[4 * (size_t)i]);
   }
   // the real rigs
   for (int f = 0; f < F; ++f) {
-    const double* c = frames[fids[f]].RigFromWorld().rotation.coeffs().data();
+    const double* c = fsorted[f].second->RigFromWorld().rotation.coeffs().data();
     std::copy(c, c + 4, &fq[4 * (size_t)f]);
   }
   rc = b200sfm_rig_rotations_from_images(ctx, I, F, K, img_frame.data(), img_cam.data(), est.data(), qimg.data(), ref_cam.data(),
@@ -1822,11 +1776,11 @@ inline bool RigRotationPrePass(ViewGraph& view_graph, std::unordered_map<rig_t, 
     Rigid3d pose;
     std::copy(&cq[4 * (size_t)c], &cq[4 * (size_t)c] + 4, pose.rotation.coeffs().data());
     for (int k = 0; k < 3; ++k) pose.translation[k] = nan;
-    b200host_adapt::SetCamFromRig(rigs[cam_rig[cids[c]]], cids[c], pose);
+    b200host_adapt::SetCamFromRig(rigs[cam_rig[cids[c]].first], cids[c], pose);
   }
   for (int f = 0; f < F; ++f) {
     if (frame_n[f] == 0) continue;
-    Rigid3d& p = frames[fids[f]].RigFromWorld();
+    Rigid3d& p = fsorted[f].second->RigFromWorld();
     std::copy(&fq[4 * (size_t)f], &fq[4 * (size_t)f] + 4, p.rotation.coeffs().data());
     for (int k = 0; k < 3; ++k) p.translation[k] = nan;
   }
@@ -1839,9 +1793,9 @@ inline bool SolveRotationAveraging(ViewGraph& view_graph, std::unordered_map<rig
   KeepLargestConnectedComponents(view_graph, frames, images);                                 // .cc:13
   auto image_has_gravity = [&](const Image& im) {
     const auto f = frames.find(im.frame_id);
-    if (f == frames.end() || !f->second.HasGravity()) return false;
-    double q[4];
-    return im.HasTrivialFrame() || b200host_adapt::FrameCamFromRig(f->second, im.camera_id, q);
+    Rigid3d c;
+    return f != frames.end() && f->second.HasGravity() &&
+           detail::ResolveCamFromRig(f->second.RigPtr(), im, c) != detail::CamFromRigStatus::kMissing;
   };
   auto registered = [&](const Image& im) {
     const auto f = frames.find(im.frame_id);
@@ -1899,7 +1853,7 @@ inline bool SolveRotationAveraging(ViewGraph& view_graph, std::unordered_map<rig
 // reference writes.  A call that fails -- a failed device call, an observation of an unknown image, an image of an unknown
 // camera or without a posed frame, a feature outside its image, a rig sensor without cam_from_rig, a camera model outside
 // 0-3 where the intrinsics are read -- prints a message on stderr and changes nothing.
-namespace processors_detail {
+namespace detail {
 
 // The tracks' observations as a device problem: trivial frames -> one pose block per image (b200sfm_ba_problem_create),
 // otherwise frames plus (rig, camera) sensors (b200sfm_ba_problem_create_rig).  Only the pixel filter reads intrinsics
@@ -1948,25 +1902,17 @@ bool Flatten(const CameraMap* cameras, const ImageMap& images, const TrackPtrs& 
       obs_rec.push_back(r->second);
     }
   // cameras of the observed images, in sorted camera-id order
-  std::map<camera_t, int32_t> cidx;
+  std::set<camera_t> observed;
   if (cameras)
     for (const Rec& r : recs) {
       if (cameras->find(r.im->camera_id) == cameras->end()) return fail("image of an unknown camera");
-      cidx[r.im->camera_id] = 0;
+      observed.insert(r.im->camera_id);
     }
-  if (pixels) {
-    for (auto& [id, k] : cidx) {
-      const auto& c = cameras->at(id);
-      k = (int32_t)out.intr_model.size();
-      out.intr_model.push_back(static_cast<int32_t>(c.model_id));
-      out.intr.resize(out.intr.size() + B200SFM_INTR_STRIDE, 0.0);
-      for (size_t j = 0; j < c.params.size() && j < (size_t)B200SFM_INTR_STRIDE; ++j) out.intr[(size_t)k * B200SFM_INTR_STRIDE + j] = c.params[j];
-    }
-  } else {
-    out.intr_model.push_back(B200SFM_SIMPLE_PINHOLE);
-    out.intr.assign(B200SFM_INTR_STRIDE, 0.0);
-    out.intr[0] = 1.0;
-  }
+  std::vector<std::pair<camera_t, const typename CameraMap::mapped_type*>> csorted;
+  for (camera_t id : observed) csorted.emplace_back(id, &cameras->at(id));
+  auto cidx = PositionOf(csorted);
+  if (pixels) PackCameras(csorted, out.intr_model, out.intr);
+  else PlaceholderCamera(out.intr_model, out.intr);
   out.K = (int32_t)out.intr_model.size();
   auto block = [&](camera_t c) { return pixels ? cidx[c] : 0; };
   auto prior = [&](camera_t c) -> uint8_t { return cameras && cameras->at(c).has_prior_focal_length ? 1 : 0; };
@@ -1993,12 +1939,9 @@ bool Flatten(const CameraMap* cameras, const ImageMap& images, const TrackPtrs& 
       for (Rec* r : rs) r->sensor = out.S;
       ++out.S;
       const Img* im = rs.front()->im;
-      Rigid3d cfr;   // identity
-      auto* rig = im->frame_ptr->RigPtr();
-      if (!im->HasTrivialFrame() && !(rig && b200host_adapt::IsRefSensor(*rig, key.second))) {
-        if (!rig || !b200host_adapt::HasCamFromRig(*rig, key.second)) return fail("image of a rig sensor without cam_from_rig");
-        cfr = b200host_adapt::CamFromRig(*rig, key.second);
-      }
+      Rigid3d cfr;
+      if (ResolveCamFromRig(im->frame_ptr->RigPtr(), *im, cfr) == CamFromRigStatus::kMissing)
+        return fail("image of a rig sensor without cam_from_rig");
       for (int k = 0; k < 4; ++k) out.sensor_q.push_back(cfr.rotation.coeffs().data()[k]);
       for (int k = 0; k < 3; ++k) out.sensor_t.push_back(cfr.translation[k]);
       out.sensor_intr.push_back(block(key.second));
@@ -2055,11 +1998,7 @@ inline int CreateProblem(b200sfm_ctx* ctx, FlatTracks& f, b200sfm_ba_problem** p
 // mode 0: pixel reprojection, 1: angle, 2: triangulation angle, 3: reprojection in the normalised image plane
 template <class CameraMap, class ImageMap, class TrackMap>
 int RunTrackFilter(int mode, const CameraMap* cameras, const ImageMap& images, TrackMap& tracks, double threshold, const char* name) {
-  using Trk = typename TrackMap::mapped_type;
-  std::vector<std::pair<track_t, Trk*>> tsorted;   // sorted track-id order
-  tsorted.reserve(tracks.size());
-  for (auto& [id, t] : tracks) tsorted.emplace_back(id, &t);
-  std::sort(tsorted.begin(), tsorted.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  const auto tsorted = SortedEntries(tracks);
   if (tsorted.empty()) return 0;
   FlatTracks f;
   if (!Flatten(cameras, images, tsorted, mode == 0, mode == 1 || mode == 3, f)) return 0;
@@ -2103,7 +2042,7 @@ int RunTrackFilter(int mode, const CameraMap* cameras, const ImageMap& images, T
   return (int)n;
 }
 
-}  // namespace processors_detail
+}  // namespace detail
 
 // TrackFilter (processors/track_filter.{h,cc}) on the device: the tracks in sorted track-id order over
 // b200sfm_ba_problem_create / _create_rig, then b200sfm_ba_problem_filter_*.  Track::observations are rewritten as the
@@ -2119,21 +2058,21 @@ struct TrackFilter {
                                         TrackMap& tracks, double max_reprojection_error = 1e-2, bool in_normalized_image = true) {
     (void)view_graph;
     // the normalised-plane variant reads no camera (track_filter.cc:23-31)
-    return processors_detail::RunTrackFilter(in_normalized_image ? 3 : 0, in_normalized_image ? nullptr : &cameras, images, tracks,
+    return detail::RunTrackFilter(in_normalized_image ? 3 : 0, in_normalized_image ? nullptr : &cameras, images, tracks,
                                              max_reprojection_error, "FilterTracksByReprojection");
   }
   template <class ViewGraphT, class CameraMap, class ImageMap, class TrackMap>
   static int FilterTracksByAngle(const ViewGraphT& view_graph, const CameraMap& cameras, const ImageMap& images, TrackMap& tracks,
                                  double max_angle_error = 1.) {
     (void)view_graph;
-    return processors_detail::RunTrackFilter(1, &cameras, images, tracks, max_angle_error, "FilterTracksByAngle");
+    return detail::RunTrackFilter(1, &cameras, images, tracks, max_angle_error, "FilterTracksByAngle");
   }
   template <class ViewGraphT, class ImageMap, class TrackMap>
   static int FilterTrackTriangulationAngle(const ViewGraphT& view_graph, const ImageMap& images, TrackMap& tracks,
                                            double min_angle = 1.) {
     (void)view_graph;
     using Cam = std::unordered_map<camera_t, Camera>;
-    return processors_detail::RunTrackFilter(2, static_cast<const Cam*>(nullptr), images, tracks, min_angle,
+    return detail::RunTrackFilter(2, static_cast<const Cam*>(nullptr), images, tracks, min_angle,
                                              "FilterTrackTriangulationAngle");
   }
 };
@@ -2144,24 +2083,21 @@ struct TrackFilter {
 template <class CameraMap, class ImageMap>
 void UndistortImages(CameraMap& cameras, ImageMap& images, bool clean_points) {
   using Img = typename ImageMap::mapped_type;
-  std::map<image_t, Img*> todo;
-  for (auto& [id, im] : images)
-    if (clean_points || im.features_undist.size() != im.features.size()) todo[id] = &im;   // image_undistorter.cc:11-16
+  const auto todo = detail::SortedEntries(images, [&](const Img& im) {
+    return clean_points || im.features_undist.size() != im.features.size();               // image_undistorter.cc:11-16
+  });
   if (todo.empty()) return;
-  std::map<camera_t, int32_t> cidx;
+  std::set<camera_t> used;
   for (auto& [id, im] : todo) {
     if (cameras.find(im->camera_id) == cameras.end()) { std::fprintf(stderr, "b200sfm: image of an unknown camera\n"); return; }
-    cidx[im->camera_id] = 0;
+    used.insert(im->camera_id);
   }
+  std::vector<std::pair<camera_t, const typename CameraMap::mapped_type*>> csorted;
+  for (camera_t id : used) csorted.emplace_back(id, &cameras.at(id));
+  auto cidx = detail::PositionOf(csorted);
   std::vector<int32_t> model, feat_intr;
   std::vector<double> params, xy;
-  for (auto& [id, k] : cidx) {
-    const auto& c = cameras.at(id);
-    k = (int32_t)model.size();
-    model.push_back(static_cast<int32_t>(c.model_id));
-    params.resize(params.size() + B200SFM_INTR_STRIDE, 0.0);
-    for (size_t j = 0; j < c.params.size() && j < (size_t)B200SFM_INTR_STRIDE; ++j) params[(size_t)k * B200SFM_INTR_STRIDE + j] = c.params[j];
-  }
+  detail::PackCameras(csorted, model, params);
   for (auto& [id, im] : todo)
     for (const auto& f : im->features) {
       feat_intr.push_back(cidx[im->camera_id]);
@@ -2201,24 +2137,16 @@ b200host_adapt::Sim3d NormalizeReconstruction(RigMap& rigs, CameraMap& cameras, 
   (void)cameras;
   using Frm = typename FrameMap::mapped_type;
   using Img = typename ImageMap::mapped_type;
-  using Trk = typename TrackMap::mapped_type;
   const double zero[3] = {0, 0, 0};
   const b200host_adapt::Sim3d identity = b200host_adapt::MakeSim3d(1.0, zero);
-  std::map<frame_t, Frm*> fsorted;
-  for (auto& [id, f] : frames)
-    if (f.HasPose()) fsorted[id] = &f;
-  std::map<frame_t, int32_t> fidx;
-  std::vector<Frm*> fr;
+  const auto fr = detail::SortedEntries(frames, [](const Frm& f) { return f.HasPose(); });
+  const auto fidx = detail::PositionOf(fr);
   std::vector<double> quat, trans;
-  for (auto& [id, f] : fsorted) {
-    fidx[id] = (int32_t)fr.size();
-    fr.push_back(f);
+  for (auto& [id, f] : fr) {
     for (int k = 0; k < 4; ++k) quat.push_back(f->RigFromWorld().rotation.coeffs().data()[k]);
     for (int k = 0; k < 3; ++k) trans.push_back(f->RigFromWorld().translation[k]);
   }
-  std::map<image_t, const Img*> reg;
-  for (auto& [id, im] : images)
-    if (im.IsRegistered()) reg[id] = &im;
+  const auto reg = detail::SortedEntries(images, [](const Img& im) { return im.IsRegistered(); });
   if (reg.empty()) { std::fprintf(stderr, "b200sfm: NormalizeReconstruction without a registered image\n"); return identity; }
   std::map<std::pair<rig_t, camera_t>, int32_t> sidx;
   std::vector<int32_t> image_frame, image_sensor;
@@ -2226,18 +2154,15 @@ b200host_adapt::Sim3d NormalizeReconstruction(RigMap& rigs, CameraMap& cameras, 
   for (auto& [id, im] : reg) {
     const auto f = fidx.find(im->frame_id);
     if (f == fidx.end()) { std::fprintf(stderr, "b200sfm: registered image without a posed frame\n"); return identity; }
-    const auto key = std::make_pair(fr[f->second]->RigId(), im->camera_id);
+    Frm& frame = *fr[f->second].second;
+    const auto key = std::make_pair(frame.RigId(), im->camera_id);
     auto s = sidx.find(key);
     if (s == sidx.end()) {
       s = sidx.emplace(key, (int32_t)sidx.size()).first;
-      Rigid3d cfr;   // identity
-      auto* rig = fr[f->second]->RigPtr();
-      if (!im->HasTrivialFrame() && !(rig && b200host_adapt::IsRefSensor(*rig, im->camera_id))) {
-        if (!rig || !b200host_adapt::HasCamFromRig(*rig, im->camera_id)) {
-          std::fprintf(stderr, "b200sfm: image of a rig sensor without cam_from_rig\n");
-          return identity;
-        }
-        cfr = b200host_adapt::CamFromRig(*rig, im->camera_id);
+      Rigid3d cfr;
+      if (detail::ResolveCamFromRig(frame.RigPtr(), *im, cfr) == detail::CamFromRigStatus::kMissing) {
+        std::fprintf(stderr, "b200sfm: image of a rig sensor without cam_from_rig\n");
+        return identity;
       }
       for (int k = 0; k < 4; ++k) sensor_q.push_back(cfr.rotation.coeffs().data()[k]);
       for (int k = 0; k < 3; ++k) sensor_t.push_back(cfr.translation[k]);
@@ -2247,8 +2172,7 @@ b200host_adapt::Sim3d NormalizeReconstruction(RigMap& rigs, CameraMap& cameras, 
   }
   const int32_t S = (int32_t)sidx.size();
   if (S > 65535) { std::fprintf(stderr, "b200sfm: too many rig sensors\n"); return identity; }
-  std::map<track_t, Trk*> tsorted;
-  for (auto& [id, t] : tracks) tsorted[id] = &t;
+  const auto tsorted = detail::SortedEntries(tracks);
   const int32_t P = std::max<int32_t>((int32_t)tsorted.size(), 1);
   std::vector<double> points(3 * (size_t)P, 0.0);
   {
@@ -2257,18 +2181,18 @@ b200host_adapt::Sim3d NormalizeReconstruction(RigMap& rigs, CameraMap& cameras, 
   }
   std::vector<int64_t> ptb(P + 1, 1);
   ptb[0] = 0;   // the placeholder observation belongs to point 0
-  const int32_t obs_frame = 0, sensor_intr = 0, intr_model = B200SFM_SIMPLE_PINHOLE;
+  const int32_t obs_frame = 0;
   const uint16_t obs_sensor = 0;
   const double obs_xy[2] = {0, 0};
-  std::vector<double> intr(B200SFM_INTR_STRIDE, 0.0);
-  intr[0] = 1.0;
-  std::vector<int32_t> sensor_intrs(S, sensor_intr);
+  std::vector<int32_t> intr_model, sensor_intr(S, 0);
+  std::vector<double> intr;
+  detail::PlaceholderCamera(intr_model, intr);
   b200sfm_ctx* ctx = DefaultContext();
   if (!ctx) return identity;
   b200sfm_ba_problem* prob = nullptr;
   double scale = 1.0, t[3] = {0, 0, 0};
   int rc = b200sfm_ba_problem_create_rig(ctx, (int32_t)fr.size(), P, 1, 1, S, ptb.data(), &obs_frame, &obs_sensor, obs_xy, sensor_q.data(),
-                                         sensor_t.data(), sensor_intrs.data(), &intr_model, nullptr, 1, &prob);
+                                         sensor_t.data(), sensor_intr.data(), intr_model.data(), nullptr, 1, &prob);
   if (rc == B200SFM_OK) rc = b200sfm_ba_problem_set_state(prob, intr.data(), quat.data(), trans.data(), points.data());
   if (rc == B200SFM_OK) rc = b200sfm_ba_problem_set_images(prob, (int32_t)image_frame.size(), image_frame.data(), image_sensor.data());
   if (rc == B200SFM_OK) rc = b200sfm_ba_problem_normalize(prob, fixed_scale ? 1 : 0, extent, p0, p1, &scale, t);
@@ -2279,7 +2203,7 @@ b200host_adapt::Sim3d NormalizeReconstruction(RigMap& rigs, CameraMap& cameras, 
     return identity;
   }
   for (size_t f = 0; f < fr.size(); ++f)                                                       // .cc:64-68
-    for (int k = 0; k < 3; ++k) fr[f]->RigFromWorld().translation[k] = trans[3 * f + k];
+    for (int k = 0; k < 3; ++k) fr[f].second->RigFromWorld().translation[k] = trans[3 * f + k];
   for (auto& [id, rig] : rigs) b200host_adapt::ScaleCamFromRigTranslations(rig, scale);        // .cc:70-78
   size_t p = 0;
   for (auto& [id, tr] : tsorted) { for (int k = 0; k < 3; ++k) tr->xyz[k] = points[3 * p + k]; ++p; }   // .cc:80-82

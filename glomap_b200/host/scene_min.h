@@ -34,14 +34,6 @@ inline void RAlignRowMajor(const glomap::Frame& f, double out[9]) {
   for (int r = 0; r < 3; ++r)
     for (int c = 0; c < 3; ++c) out[3 * r + c] = R(r, c);
 }
-// cam_from_rig rotation (quaternion xyzw) of a non-reference camera through the frame's rig pointer; false when unknown
-inline bool FrameCamFromRig(const glomap::Frame& f, glomap::camera_t camera_id, double q[4]) {
-  if (!f.RigPtr()) return false;
-  const auto& c = f.RigPtr()->MaybeSensorFromRig(glomap::sensor_t(glomap::SensorType::CAMERA, camera_id));
-  if (!c.has_value()) return false;
-  for (int k = 0; k < 4; ++k) q[k] = c->rotation.coeffs().data()[k];
-  return true;
-}
 // GravityInfo::SetGravity (scene/frame.h:46-50): gravity and R_align = GetAlignRot(g).  A template, so that it is
 // compiled only where a refiner writes gravity back.
 template <class FrameT>
@@ -226,12 +218,6 @@ inline b200host::camera_t RefCameraId(const b200host::Rig& rig) { return rig.ref
 inline bool HasCamFromRig(const b200host::Rig& rig, b200host::camera_t camera_id) { return rig.cam_from_rig.count(camera_id) != 0; }
 inline void RAlignRowMajor(const b200host::Frame& f, double out[9]) {
   for (int k = 0; k < 9; ++k) out[k] = f.gravity_info.R_align[k];
-}
-inline bool FrameCamFromRig(const b200host::Frame& f, b200host::camera_t camera_id, double q[4]) {
-  if (!f.RigPtr() || !HasCamFromRig(*f.RigPtr(), camera_id)) return false;
-  const b200host::Rigid3d c = f.RigPtr()->SensorFromRig(camera_id);
-  for (int k = 0; k < 4; ++k) q[k] = c.rotation.c[k];
-  return true;
 }
 inline void SetFrameGravity(b200host::Frame& f, const double g[3]) { f.gravity_info.SetGravity({{g[0], g[1], g[2]}}); }
 inline void ScaleCamFromRigTranslations(b200host::Rig& rig, double scale) {

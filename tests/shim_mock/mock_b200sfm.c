@@ -7,6 +7,7 @@
 #include <string.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
 struct b200sfm_ctx { int dummy; };
 struct b200sfm_ba_problem { b200sfm_ctx* ctx; };
@@ -21,7 +22,7 @@ static void remember_ba(int32_t P, int64_t N, const int64_t* ptb) {
 }
 /* filter stub: keeps everything, or drops every m-th observation when $MOCK_DROP_EVERY = m > 0 */
 static long long stub_filter(const char* name, double thr, uint8_t* keep) {
-  FILE* f = fopen(getenv("MOCK_DUMP") ? getenv("MOCK_DUMP") : "/dev/null", "a");
+  FILE* f = mock_dump_open();
   fprintf(f, "call %s\nthreshold 1 %.17g\nnobs 1 %lld\n", name, thr, g_ba_n);
   fclose(f);
   const char* e = getenv("MOCK_DROP_EVERY");
@@ -42,31 +43,6 @@ static struct b200sfm_ctx g_ctx;
 static long long g_gp_n = 0;
 static int g_ba_S = 0;   /* sensors of the last rig problem */
 
-static FILE* out(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_d(const char* name, const double* v, long long n) {
-  FILE* f = out();
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-  fclose(f);
-}
-#define DUMP_INT(NAME, PTR, N)                                              \
-  do {                                                                      \
-    FILE* f_ = out();                                                       \
-    fprintf(f_, "%s %lld", NAME, (PTR) ? (long long)(N) : 0ll);             \
-    for (long long i_ = 0; (PTR) && i_ < (long long)(N); ++i_) fprintf(f_, " %lld", (long long)(PTR)[i_]); \
-    fprintf(f_, "\n");                                                      \
-    fclose(f_);                                                             \
-  } while (0)
-static void dump_call(const char* name) {
-  FILE* f = out();
-  fprintf(f, "call %s\n", name);
-  fclose(f);
-}
-
 int b200sfm_version(void) { return B200SFM_VERSION; }
 int b200sfm_create(int device, b200sfm_ctx** o) { (void)device; *o = &g_ctx; return B200SFM_OK; }
 void b200sfm_destroy(b200sfm_ctx* c) { (void)c; }
@@ -81,14 +57,16 @@ int b200sfm_ba_solve(b200sfm_ctx* ctx, const b200sfm_ba_opts* o, int32_t C, int3
                      const int32_t* intr_model, double* intr, double* quat, double* trans, const uint8_t* mask, double* points,
                      b200sfm_lm_stats* st) {
   (void)ctx;
-  dump_call("ba_solve");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ba_solve\n");
   int32_t dims[4] = {C, P, (int32_t)N, K};
-  DUMP_INT("dims", dims, 4);
+  dump_i32(f, "dims", dims, 4);
   int32_t flags[3] = {o->optimize_rotations, o->optimize_intrinsics, o->optimize_rig_poses};
-  DUMP_INT("flags", flags, 3);
-  DUMP_INT("pt_obs_begin", ptb, P + 1); DUMP_INT("obs_cam", obs_cam, N); dump_d("obs_xy", obs_xy, 2 * N);
-  DUMP_INT("cam_intr", cam_intr, C); DUMP_INT("intr_model", intr_model, K); dump_d("intr", intr, (long long)K * B200SFM_INTR_STRIDE);
-  dump_d("quat", quat, 4ll * C); dump_d("trans", trans, 3ll * C); DUMP_INT("mask", mask, C); dump_d("points", points, 3ll * P);
+  dump_i32(f, "flags", flags, 3);
+  dump_i64(f, "pt_obs_begin", ptb, P + 1); dump_i32(f, "obs_cam", obs_cam, N); dump_f64(f, "obs_xy", obs_xy, 2 * N);
+  dump_i32(f, "cam_intr", cam_intr, C); dump_i32(f, "intr_model", intr_model, K); dump_f64(f, "intr", intr, (long long)K * B200SFM_INTR_STRIDE);
+  dump_f64(f, "quat", quat, 4ll * C); dump_f64(f, "trans", trans, 3ll * C); dump_u8(f, "mask", mask, C); dump_f64(f, "points", points, 3ll * P);
+  fclose(f);
   memset(st, 0, sizeof(*st)); st->usable = 1;
   return B200SFM_OK;
 }
@@ -96,12 +74,14 @@ int b200sfm_ba_problem_create_rig(b200sfm_ctx* ctx, int32_t F, int32_t P, int64_
                                   const int32_t* obs_frame, const uint16_t* obs_sensor, const double* obs_xy,
                                   const double* sq, const double* stv, const int32_t* sintr, const int32_t* intr_model,
                                   const uint8_t* mask, int32_t minv, b200sfm_ba_problem** o) {
-  dump_call("ba_problem_create_rig");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ba_problem_create_rig\n");
   int32_t dims[6] = {F, P, (int32_t)N, K, S, minv};
-  DUMP_INT("dims", dims, 6);
-  DUMP_INT("pt_obs_begin", ptb, P + 1); DUMP_INT("obs_frame", obs_frame, N); DUMP_INT("obs_sensor", obs_sensor, N);
-  dump_d("obs_xy", obs_xy, 2 * N); dump_d("sensor_quat", sq, 4ll * S); dump_d("sensor_trans", stv, 3ll * S);
-  DUMP_INT("sensor_intr", sintr, S); DUMP_INT("intr_model", intr_model, K); DUMP_INT("mask", mask, F);
+  dump_i32(f, "dims", dims, 6);
+  dump_i64(f, "pt_obs_begin", ptb, P + 1); dump_i32(f, "obs_frame", obs_frame, N); dump_u16(f, "obs_sensor", obs_sensor, N);
+  dump_f64(f, "obs_xy", obs_xy, 2 * N); dump_f64(f, "sensor_quat", sq, 4ll * S); dump_f64(f, "sensor_trans", stv, 3ll * S);
+  dump_i32(f, "sensor_intr", sintr, S); dump_i32(f, "intr_model", intr_model, K); dump_u8(f, "mask", mask, F);
+  fclose(f);
   remember_ba(P, N, ptb);
   g_ba_S = S;
   static struct b200sfm_ba_problem p; p.ctx = ctx; *o = &p;
@@ -114,8 +94,10 @@ int b200sfm_ba_problem_set_state(b200sfm_ba_problem* p, const double* intr, cons
 }
 int b200sfm_ba_problem_set_sensor_variable(b200sfm_ba_problem* p, const uint8_t* v) {
   (void)p;
-  dump_call("ba_problem_set_sensor_variable");
-  DUMP_INT("sensor_variable", v, g_ba_S);
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ba_problem_set_sensor_variable\n");
+  dump_u8(f, "sensor_variable", v, g_ba_S);
+  fclose(f);
   return B200SFM_OK;
 }
 /* a recognisable "optimised" cam_from_rig for every sensor: rotation 90 deg about z, translation (7 + s, 8, 9) */
@@ -129,8 +111,10 @@ int b200sfm_ba_problem_get_sensor_poses(b200sfm_ba_problem* p, double* q, double
 }
 int b200sfm_ba_problem_set_images(b200sfm_ba_problem* p, int32_t I, const int32_t* image_frame, const int32_t* image_sensor) {
   (void)p;
-  dump_call("ba_problem_set_images");
-  DUMP_INT("image_frame", image_frame, I); DUMP_INT("image_sensor", image_sensor, I);
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ba_problem_set_images\n");
+  dump_i32(f, "image_frame", image_frame, I); dump_i32(f, "image_sensor", image_sensor, I);
+  fclose(f);
   return B200SFM_OK;
 }
 int b200sfm_ba_problem_normalize(b200sfm_ba_problem* p, int32_t fixed_scale, double extent, double p0, double p1, double* sc,
@@ -159,36 +143,44 @@ int b200sfm_gp_solve(b200sfm_ctx* ctx, const b200sfm_gp_opts* o, int32_t C, int3
                      const int32_t* obs_cam, const double* obs_dir, const uint8_t* cal, const uint8_t* mask, double* cen,
                      double* pts, double* sc, b200sfm_lm_stats* st) {
   (void)ctx; (void)o; (void)mask; (void)cen; (void)pts; (void)sc;
-  dump_call("gp_solve");
-  DUMP_INT("pt_obs_begin", ptb, P + 1); DUMP_INT("obs_cam", obs_cam, N); dump_d("obs_dir", obs_dir, 3 * N); DUMP_INT("calibrated", cal, C);
+  FILE* f = mock_dump_open();
+  fprintf(f, "call gp_solve\n");
+  dump_i64(f, "pt_obs_begin", ptb, P + 1); dump_i32(f, "obs_cam", obs_cam, N); dump_f64(f, "obs_dir", obs_dir, 3 * N); dump_u8(f, "calibrated", cal, C);
+  fclose(f);
   memset(st, 0, sizeof(*st)); st->usable = 1;
   return B200SFM_OK;
 }
 int b200sfm_gp_problem_create(b200sfm_ctx* ctx, int32_t C, int32_t P, int64_t N, const int64_t* ptb, const int32_t* obs_cam,
                               const double* obs_dir, const uint8_t* cal, const uint8_t* mask, int32_t minv, b200sfm_gp_problem** o) {
   (void)mask; (void)minv;
-  dump_call("gp_problem_create");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call gp_problem_create\n");
   int32_t dims[3] = {C, P, (int32_t)N};
-  DUMP_INT("dims", dims, 3);
-  DUMP_INT("pt_obs_begin", ptb, P + 1); DUMP_INT("obs_cam", obs_cam, N); dump_d("obs_dir", obs_dir, 3 * N); DUMP_INT("calibrated", cal, C);
+  dump_i32(f, "dims", dims, 3);
+  dump_i64(f, "pt_obs_begin", ptb, P + 1); dump_i32(f, "obs_cam", obs_cam, N); dump_f64(f, "obs_dir", obs_dir, 3 * N); dump_u8(f, "calibrated", cal, C);
+  fclose(f);
   static struct b200sfm_gp_problem p; p.ctx = ctx; *o = &p;
   g_gp_n = N;
   return B200SFM_OK;
 }
 int b200sfm_gp_problem_set_rig_terms(b200sfm_gp_problem* p, const double* off, const uint8_t* cal) {
   (void)p;
-  dump_call("gp_problem_set_rig_terms");
-  dump_d("obs_offset", off, 3 * g_gp_n); DUMP_INT("obs_calibrated", cal, g_gp_n);
+  FILE* f = mock_dump_open();
+  fprintf(f, "call gp_problem_set_rig_terms\n");
+  dump_f64(f, "obs_offset", off, 3 * g_gp_n); dump_u8(f, "obs_calibrated", cal, g_gp_n);
+  fclose(f);
   return B200SFM_OK;
 }
 static int g_gp_su = 0;
 int b200sfm_gp_problem_set_rig_unknown(b200sfm_gp_problem* p, int32_t su, const int32_t* os, const double* fr, const double* c) {
   (void)p; (void)fr;
-  dump_call("gp_problem_set_rig_unknown");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call gp_problem_set_rig_unknown\n");
   int32_t dims[1] = {su};
-  DUMP_INT("dims", dims, 1);
-  DUMP_INT("obs_unknown_sensor", os, g_gp_n);
-  dump_d("centers", c, 3ll * su);
+  dump_i32(f, "dims", dims, 1);
+  dump_i32(f, "obs_unknown_sensor", os, g_gp_n);
+  dump_f64(f, "centers", c, 3ll * su);
+  fclose(f);
   g_gp_su = su;
   return B200SFM_OK;
 }
@@ -208,10 +200,12 @@ void b200sfm_gp_problem_free(b200sfm_gp_problem* p) { (void)p; }
 int b200sfm_ra_solve(b200sfm_ctx* ctx, const b200sfm_ra_opts* o, int32_t n, int64_t E, const int32_t* ei, const int32_t* ej,
                      const double* R, const double* w, int32_t fixed, double* theta, b200sfm_ra_stats* st) {
   (void)ctx; (void)o; (void)fixed;
-  dump_call("ra_solve");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ra_solve\n");
   int32_t dims[2] = {n, (int32_t)E};
-  DUMP_INT("dims", dims, 2);
-  DUMP_INT("ei", ei, E); DUMP_INT("ej", ej, E); dump_d("R_rel", R, 9 * E); dump_d("weight", w, E); dump_d("theta", theta, 3ll * n);
+  dump_i32(f, "dims", dims, 2);
+  dump_i32(f, "ei", ei, E); dump_i32(f, "ej", ej, E); dump_f64(f, "R_rel", R, 9 * E); dump_f64(f, "weight", w, E); dump_f64(f, "theta", theta, 3ll * n);
+  fclose(f);
   memset(st, 0, sizeof(*st)); st->usable = 1;
   return B200SFM_OK;
 }
@@ -227,9 +221,11 @@ int b200sfm_ba_problem_create(b200sfm_ctx* ctx, int32_t C, int32_t P, int64_t N,
                               const int32_t* obs_cam, const double* obs_xy, const int32_t* cam_intr, const int32_t* intr_model,
                               const uint8_t* mask, int32_t minv, b200sfm_ba_problem** o) {
   (void)obs_cam; (void)obs_xy; (void)cam_intr; (void)intr_model; (void)mask;
-  dump_call("ba_problem_create");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ba_problem_create\n");
   int32_t dims[5] = {C, P, (int32_t)N, K, minv};
-  DUMP_INT("dims", dims, 5);
+  dump_i32(f, "dims", dims, 5);
+  fclose(f);
   remember_ba(P, N, ptb);
   static struct b200sfm_ba_problem p; p.ctx = ctx; *o = &p;
   return B200SFM_OK;
@@ -248,7 +244,9 @@ int b200sfm_ba_problem_filter_angle(b200sfm_ba_problem* p, const double* b, cons
 }
 int b200sfm_ba_problem_filter_triangulation_angle(b200sfm_ba_problem* p, double thr, uint8_t* keep_track, int64_t* n) {
   (void)p;
-  FILE* f = out(); fprintf(f, "call filter_triangulation_angle\nthreshold 1 %.17g\n", thr); fclose(f);
+  FILE* f = mock_dump_open();
+  fprintf(f, "call filter_triangulation_angle\nthreshold 1 %.17g\n", thr);
+  fclose(f);
   for (long long i = 0; i < g_ba_p; ++i) keep_track[i] = 1;
   if (n) *n = 0;
   return B200SFM_OK;
@@ -259,13 +257,15 @@ int b200sfm_ra_solve_rig(b200sfm_ctx* ctx, const b200sfm_ra_opts* o, int32_t nf,
                          const int32_t* ej, const int32_t* eci, const int32_t* ecj, const double* R, const double* w,
                          const int32_t* cfb, const int32_t* cf, int32_t fixed, double* theta, b200sfm_ra_stats* st) {
   (void)ctx; (void)o;
-  dump_call("ra_solve_rig");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ra_solve_rig\n");
   int32_t dims[4] = {nf, nc, (int32_t)ne, fixed};
-  DUMP_INT("dims", dims, 4);
-  DUMP_INT("ei", ei, ne); DUMP_INT("ej", ej, ne); DUMP_INT("eci", eci, ne); DUMP_INT("ecj", ecj, ne);
-  dump_d("R_rel", R, 9 * ne); dump_d("w", w, ne);
-  DUMP_INT("cam_frames_begin", cfb, nc + 1); DUMP_INT("cam_frames", cf, cfb ? cfb[nc] : 0);
-  dump_d("theta", theta, 3ll * (nf + nc));
+  dump_i32(f, "dims", dims, 4);
+  dump_i32(f, "ei", ei, ne); dump_i32(f, "ej", ej, ne); dump_i32(f, "eci", eci, ne); dump_i32(f, "ecj", ecj, ne);
+  dump_f64(f, "R_rel", R, 9 * ne); dump_f64(f, "w", w, ne);
+  dump_i32(f, "cam_frames_begin", cfb, nc + 1); dump_i32(f, "cam_frames", cf, cfb ? cfb[nc] : 0);
+  dump_f64(f, "theta", theta, 3ll * (nf + nc));
+  fclose(f);
   /* a recognisable result for the camera nodes: rotation 0.3 rad about z */
   for (int c = 0; c < nc; ++c) { theta[3 * (nf + c)] = 0; theta[3 * (nf + c) + 1] = 0; theta[3 * (nf + c) + 2] = 0.3; }
   if (st) { memset(st, 0, sizeof(*st)); st->usable = 1; }
@@ -274,10 +274,12 @@ int b200sfm_ra_solve_rig(b200sfm_ctx* ctx, const b200sfm_ra_opts* o, int32_t nf,
 int b200sfm_ra_solve_gravity(b200sfm_ctx* ctx, const b200sfm_ra_opts* o, int32_t n, int64_t E, const int32_t* ei, const int32_t* ej,
                              const double* R, const double* w, const uint8_t* hg, int32_t fixed, double* theta, b200sfm_ra_stats* st) {
   (void)ctx; (void)o; (void)w;
-  dump_call("ra_solve_gravity");
+  FILE* f = mock_dump_open();
+  fprintf(f, "call ra_solve_gravity\n");
   int32_t dims[3] = {n, (int32_t)E, fixed};
-  DUMP_INT("dims", dims, 3);
-  DUMP_INT("ei", ei, E); DUMP_INT("ej", ej, E); dump_d("R_rel", R, 9 * E); DUMP_INT("has_gravity", hg, n); dump_d("theta", theta, 3ll * n);
+  dump_i32(f, "dims", dims, 3);
+  dump_i32(f, "ei", ei, E); dump_i32(f, "ej", ej, E); dump_f64(f, "R_rel", R, 9 * E); dump_u8(f, "has_gravity", hg, n); dump_f64(f, "theta", theta, 3ll * n);
+  fclose(f);
   memset(st, 0, sizeof(*st)); st->usable = 1;
   return B200SFM_OK;
 }

@@ -7,17 +7,8 @@
 #include <string.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
-static void dump_d(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_i32(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
 
 void b200sfm_gravity_default_opts(b200sfm_gravity_opts* o) {
   memset(o, 0, sizeof(*o));
@@ -31,19 +22,18 @@ int b200sfm_gravity_refine(b200sfm_ctx* ctx, const b200sfm_gravity_opts* opts, i
                            const uint8_t* has_gravity, int64_t E, const int32_t* frame1, const int32_t* frame2,
                            const double* M, double* gravity, uint8_t* status, b200sfm_gravity_stats* stats) {
   (void)ctx;
-  const char* p = getenv("MOCK_DUMP");
-  FILE* f = fopen(p ? p : "/dev/null", "a");
+  FILE* f = mock_dump_open();
   fprintf(f, "call gravity_refine\n");
   const double scalars[6] = {opts->max_outlier_ratio, opts->max_gravity_error, opts->min_num_neighbors,
                              opts->max_num_iterations, (double)F, (double)E};
-  dump_d(f, "scalars", scalars, 6);
-  dump_d(f, "R_align", R_align, 9LL * F);
+  dump_f64(f, "scalars", scalars, 6);
+  dump_f64(f, "R_align", R_align, 9LL * F);
   fprintf(f, "has_gravity %d", F);
   for (int32_t k = 0; k < F; ++k) fprintf(f, " %d", (int)has_gravity[k]);
   fprintf(f, "\n");
   dump_i32(f, "frame1", frame1, E);
   dump_i32(f, "frame2", frame2, E);
-  dump_d(f, "M", M, 9 * E);
+  dump_f64(f, "M", M, 9 * E);
   fclose(f);
   if (stats) memset(stats, 0, sizeof(*stats));
   for (int32_t k = 0; k < F; ++k) {

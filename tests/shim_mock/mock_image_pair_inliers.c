@@ -5,26 +5,8 @@
 #include <stdlib.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
-static FILE* dump_file(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_i32(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_i64(FILE* f, const char* name, const int64_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %lld", (long long)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_f64(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
 
 int b200sfm_image_pairs_inlier_count(b200sfm_ctx* ctx, int32_t I, const int64_t* fb, const double* feat, const int32_t* image_intr,
                                      int32_t K, const int32_t* intr_model, const double* intr, int64_t E, const int32_t* i1,
@@ -33,7 +15,7 @@ int b200sfm_image_pairs_inlier_count(b200sfm_ctx* ctx, int32_t I, const int64_t*
                                      uint8_t* inl, int32_t* n_inl, double* score) {
   (void)ctx;
   const long long M = E > 0 ? mb[E] : 0;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call image_pairs_inlier_count\n");
   const int64_t dims[4] = {I, K, E, M};
   const double thr[3] = {eE, eF, eH};

@@ -5,33 +5,15 @@
 #include <stdlib.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
-static FILE* dump_file(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_i32(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u8(FILE* f, const char* name, const uint8_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", (int)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_f64(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
 
 int b200sfm_view_graph_update_pairs_config(b200sfm_ctx* ctx, int32_t K, const int32_t* intr_model, const double* intr_params,
                                            const uint8_t* has_prior_focal, int64_t num_pairs, const int32_t* pair_cam1,
                                            const int32_t* pair_cam2, const uint8_t* pair_valid, const double* pair_quat_xyzw,
                                            const double* pair_trans, int32_t* pair_config, double* pair_F, int64_t* num_promoted) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call view_graph_update_pairs_config\n");
   dump_i32(f, "intr_model", intr_model, K);
   dump_f64(f, "intr_params", intr_params, (long long)K * B200SFM_INTR_STRIDE);

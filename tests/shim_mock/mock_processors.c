@@ -10,39 +10,11 @@
 #include <stdlib.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
 static int g_ctx_storage;
 static struct { int rig; int32_t C, P, K, S; int64_t N; } g_prob;
 
-static FILE* dump_file(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_i(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u16(FILE* f, const char* name, const uint16_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %u", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u8(FILE* f, const char* name, const uint8_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %u", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_i64(FILE* f, const char* name, const int64_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %lld", (long long)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_d(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
 static int bad_model(const int32_t* m, int32_t K) {
   for (int32_t k = 0; k < K; ++k)
     if (m[k] < 0 || m[k] > 3) return 1;
@@ -63,15 +35,15 @@ int b200sfm_ba_problem_create(b200sfm_ctx* ctx, int32_t C, int32_t P, int64_t N,
                               const int32_t* obs_cam, const double* obs_xy, const int32_t* cam_intr, const int32_t* intr_model,
                               const uint8_t* mask, int32_t min_views, b200sfm_ba_problem** out) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call create\n");
   const int32_t dims[5] = {C, P, (int32_t)N, K, min_views};
-  dump_i(f, "dims", dims, 5);
+  dump_i32(f, "dims", dims, 5);
   dump_i64(f, "ptb", ptb, P + 1);
-  dump_i(f, "obs_cam", obs_cam, N);
-  dump_d(f, "obs_xy", obs_xy, 2 * N);
-  dump_i(f, "cam_intr", cam_intr, C);
-  dump_i(f, "intr_model", intr_model, K);
+  dump_i32(f, "obs_cam", obs_cam, N);
+  dump_f64(f, "obs_xy", obs_xy, 2 * N);
+  dump_i32(f, "cam_intr", cam_intr, C);
+  dump_i32(f, "intr_model", intr_model, K);
   dump_u8(f, "mask", mask, C);
   fclose(f);
   if (bad_model(intr_model, K)) return B200SFM_ERR_UNSUPPORTED;
@@ -85,18 +57,18 @@ int b200sfm_ba_problem_create_rig(b200sfm_ctx* ctx, int32_t F, int32_t P, int64_
                                   const double* st, const int32_t* sensor_intr, const int32_t* intr_model, const uint8_t* mask,
                                   int32_t min_views, b200sfm_ba_problem** out) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call create_rig\n");
   const int32_t dims[6] = {F, P, (int32_t)N, K, S, min_views};
-  dump_i(f, "dims", dims, 6);
+  dump_i32(f, "dims", dims, 6);
   dump_i64(f, "ptb", ptb, P + 1);
-  dump_i(f, "obs_frame", obs_frame, N);
+  dump_i32(f, "obs_frame", obs_frame, N);
   dump_u16(f, "obs_sensor", obs_sensor, N);
-  dump_d(f, "obs_xy", obs_xy, 2 * N);
-  dump_d(f, "sensor_q", sq, 4 * S);
-  dump_d(f, "sensor_t", st, 3 * S);
-  dump_i(f, "sensor_intr", sensor_intr, S);
-  dump_i(f, "intr_model", intr_model, K);
+  dump_f64(f, "obs_xy", obs_xy, 2 * N);
+  dump_f64(f, "sensor_q", sq, 4 * S);
+  dump_f64(f, "sensor_t", st, 3 * S);
+  dump_i32(f, "sensor_intr", sensor_intr, S);
+  dump_i32(f, "intr_model", intr_model, K);
   dump_u8(f, "mask", mask, F);
   fclose(f);
   if (bad_model(intr_model, K)) return B200SFM_ERR_UNSUPPORTED;
@@ -107,10 +79,10 @@ int b200sfm_ba_problem_create_rig(b200sfm_ctx* ctx, int32_t F, int32_t P, int64_
 
 int b200sfm_ba_problem_set_images(b200sfm_ba_problem* p, int32_t I, const int32_t* image_frame, const int32_t* image_sensor) {
   (void)p;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call set_images\n");
-  dump_i(f, "image_frame", image_frame, I);
-  dump_i(f, "image_sensor", image_sensor, I);
+  dump_i32(f, "image_frame", image_frame, I);
+  dump_i32(f, "image_sensor", image_sensor, I);
   fclose(f);
   return B200SFM_OK;
 }
@@ -118,12 +90,12 @@ int b200sfm_ba_problem_set_images(b200sfm_ba_problem* p, int32_t I, const int32_
 int b200sfm_ba_problem_set_state(b200sfm_ba_problem* p, const double* intr, const double* quat, const double* trans,
                                  const double* points) {
   (void)p;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call set_state\n");
-  dump_d(f, "intr", intr, (long long)g_prob.K * B200SFM_INTR_STRIDE);
-  dump_d(f, "quat", quat, 4LL * g_prob.C);
-  dump_d(f, "trans", trans, 3LL * g_prob.C);
-  dump_d(f, "points", points, 3LL * g_prob.P);
+  dump_f64(f, "intr", intr, (long long)g_prob.K * B200SFM_INTR_STRIDE);
+  dump_f64(f, "quat", quat, 4LL * g_prob.C);
+  dump_f64(f, "trans", trans, 3LL * g_prob.C);
+  dump_f64(f, "points", points, 3LL * g_prob.P);
   fclose(f);
   return B200SFM_OK;
 }
@@ -139,10 +111,10 @@ void b200sfm_ba_problem_free(b200sfm_ba_problem* p) { (void)p; }
 
 static int observation_filter(const char* name, double thr, const double* bearings, const uint8_t* calibrated, uint8_t* keep,
                               int64_t* n) {
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call %s\n", name);
-  dump_d(f, "threshold", &thr, 1);
-  dump_d(f, "bearings", bearings, 3 * g_prob.N);
+  dump_f64(f, "threshold", &thr, 1);
+  dump_f64(f, "bearings", bearings, 3 * g_prob.N);
   dump_u8(f, "calibrated", calibrated, g_prob.rig ? g_prob.S : g_prob.C);
   fclose(f);
   for (int64_t o = 0; o < g_prob.N; ++o) keep[o] = o % 3 != 1;
@@ -165,9 +137,9 @@ int b200sfm_ba_problem_filter_angle(b200sfm_ba_problem* p, const double* bearing
 }
 int b200sfm_ba_problem_filter_triangulation_angle(b200sfm_ba_problem* p, double thr, uint8_t* keep, int64_t* n) {
   (void)p;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call filter_triangulation_angle\n");
-  dump_d(f, "threshold", &thr, 1);
+  dump_f64(f, "threshold", &thr, 1);
   fclose(f);
   for (int32_t t = 0; t < g_prob.P; ++t) keep[t] = t % 2 == 0;
   *n = 5;
@@ -177,10 +149,10 @@ int b200sfm_ba_problem_filter_triangulation_angle(b200sfm_ba_problem* p, double 
 int b200sfm_ba_problem_normalize(b200sfm_ba_problem* p, int32_t fixed_scale, double extent, double p0, double p1, double* scale,
                                  double* t) {
   (void)p;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call normalize\n");
   const double args[4] = {(double)fixed_scale, extent, p0, p1};
-  dump_d(f, "args", args, 4);
+  dump_f64(f, "args", args, 4);
   fclose(f);
   *scale = 2.0;
   t[0] = 1.0; t[1] = 2.0; t[2] = 3.0;
@@ -190,12 +162,12 @@ int b200sfm_ba_problem_normalize(b200sfm_ba_problem* p, int32_t fixed_scale, dou
 int b200sfm_undistort_features(b200sfm_ctx* ctx, int32_t K, const int32_t* intr_model, const double* intr_params, int64_t n,
                                const int32_t* feat_intr, const double* xy, double* out) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call undistort_features\n");
-  dump_i(f, "intr_model", intr_model, K);
-  dump_d(f, "intr", intr_params, (long long)K * B200SFM_INTR_STRIDE);
-  dump_i(f, "feat_intr", feat_intr, n);
-  dump_d(f, "xy", xy, 2 * n);
+  dump_i32(f, "intr_model", intr_model, K);
+  dump_f64(f, "intr", intr_params, (long long)K * B200SFM_INTR_STRIDE);
+  dump_i32(f, "feat_intr", feat_intr, n);
+  dump_f64(f, "xy", xy, 2 * n);
   fclose(f);
   for (int64_t i = 0; i < n; ++i)
     if (intr_model[feat_intr[i]] < 0 || intr_model[feat_intr[i]] > 3) return B200SFM_ERR_UNSUPPORTED;

@@ -6,22 +6,8 @@
 #include <stdlib.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
-static void dump_i64(FILE* f, const char* name, const int64_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %lld", (long long)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_i32(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u8(FILE* f, const char* name, const uint8_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", (int)v[i]);
-  fprintf(f, "\n");
-}
 
 int b200sfm_prune_weakly_connected(b200sfm_ctx* ctx, int32_t num_frames, int64_t num_tracks, const int64_t* track_begin,
                                    const int32_t* obs_frame, const uint8_t* frame_self_loop, int32_t min_num_observations,
@@ -29,8 +15,7 @@ int b200sfm_prune_weakly_connected(b200sfm_ctx* ctx, int32_t num_frames, int64_t
                                    int32_t* num_clusters, b200sfm_prune_stats* stats) {
   (void)ctx;
   (void)stats;
-  const char* p = getenv("MOCK_DUMP");
-  FILE* f = fopen(p ? p : "/dev/null", "a");
+  FILE* f = mock_dump_open();
   fprintf(f, "call prune_weakly_connected\n");
   const int64_t scalars[3] = {min_num_observations, max_pair_keys_per_pass, num_frames};
   dump_i64(f, "scalars", scalars, 3);

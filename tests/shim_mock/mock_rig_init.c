@@ -7,35 +7,17 @@
 #include <string.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
-static FILE* out(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_d(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_i32(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u8(FILE* f, const char* name, const uint8_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", (int)v[i]);
-  fprintf(f, "\n");
-}
 
 int b200sfm_ra_mst_init(b200sfm_ctx* ctx, int32_t n, int64_t E, const int32_t* ei, const int32_t* ej, const double* R,
                         const double* w, int32_t root, double* Rout, int32_t* parent, b200sfm_mst_stats* st) {
   (void)ctx; (void)Rout;
-  FILE* f = out();
+  FILE* f = mock_dump_open();
   fprintf(f, "call ra_mst_init\n");
   const int32_t dims[3] = {n, (int32_t)E, root};
   dump_i32(f, "dims", dims, 3);
-  dump_i32(f, "ei", ei, E); dump_i32(f, "ej", ej, E); dump_d(f, "R_rel", R, 9 * E); dump_d(f, "weight", w, E);
+  dump_i32(f, "ei", ei, E); dump_i32(f, "ej", ej, E); dump_f64(f, "R_rel", R, 9 * E); dump_f64(f, "weight", w, E);
   fclose(f);
   for (int32_t v = 0; parent && v < n; ++v) parent[v] = root;
   if (st) memset(st, 0, sizeof(*st));
@@ -46,12 +28,12 @@ int b200sfm_rig_rotations_from_images(b200sfm_ctx* ctx, int64_t I, int32_t F, in
                                       const uint8_t* est, const double* q, const int32_t* ref, const uint8_t* known, double* cq,
                                       int32_t* cn, double* fq, int32_t* fn, b200sfm_rig_init_stats* st) {
   (void)ctx; (void)fq;
-  FILE* f = out();
+  FILE* f = mock_dump_open();
   fprintf(f, "call rig_rotations_from_images\n");
   const int32_t dims[3] = {(int32_t)I, F, K};
   dump_i32(f, "dims", dims, 3);
   dump_i32(f, "image_frame", fr, I); dump_i32(f, "image_camera", cam, I); dump_u8(f, "image_estimated", est, I);
-  dump_d(f, "cam_from_world", q, 4 * I); dump_i32(f, "frame_ref_camera", ref, F); dump_u8(f, "camera_known", known, K);
+  dump_f64(f, "cam_from_world", q, 4 * I); dump_i32(f, "frame_ref_camera", ref, F); dump_u8(f, "camera_known", known, K);
   fclose(f);
   for (int32_t c = 0; cn && c < K; ++c) cn[c] = 0;
   for (int64_t i = 0; i < I; ++i) {

@@ -7,33 +7,10 @@
 #include <stdlib.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
 static int g_ctx_storage;
 
-static FILE* dump_file(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_u64(FILE* f, const char* name, const uint64_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %llu", (unsigned long long)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_i64(FILE* f, const char* name, const int64_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %lld", (long long)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u32(FILE* f, const char* name, const uint32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %u", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_d(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
 
 int b200sfm_create(int device, b200sfm_ctx** o) {
   (void)device;
@@ -48,13 +25,13 @@ const char* b200sfm_last_error(const b200sfm_ctx* c) {
 int b200sfm_tracks_establish(b200sfm_ctx* ctx, int64_t m, const uint64_t* g1, const uint64_t* g2, const double* xy1, const double* xy2,
                              double thr, b200sfm_tracks** out, int64_t* nt, int64_t* no, int64_t* nd) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call tracks_establish\n");
-  dump_d(f, "thres", &thr, 1);
+  dump_f64(f, "thres", &thr, 1);
   dump_u64(f, "gid1", g1, m);
   dump_u64(f, "gid2", g2, m);
-  dump_d(f, "xy1", xy1, 2 * m);
-  dump_d(f, "xy2", xy2, 2 * m);
+  dump_f64(f, "xy1", xy1, 2 * m);
+  dump_f64(f, "xy2", xy2, 2 * m);
   fclose(f);
   *out = (b200sfm_tracks*)&g_ctx_storage;
   *nt = 2;
@@ -77,7 +54,7 @@ int b200sfm_tracks_select(b200sfm_ctx* ctx, int64_t num_tracks, const uint64_t* 
                           int32_t min_num_tracks_per_view, int32_t min_num_view_per_track, int32_t max_num_view_per_track,
                           int32_t max_num_tracks, uint8_t* keep, int64_t* num_selected) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call tracks_select\n");
   const int64_t opts[4] = {min_num_tracks_per_view, min_num_view_per_track, max_num_view_per_track, max_num_tracks};
   dump_i64(f, "options", opts, 4);

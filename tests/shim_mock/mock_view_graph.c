@@ -8,33 +8,15 @@
 #include <stdlib.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
-static FILE* dump_file(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_i32(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u8(FILE* f, const char* name, const uint8_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", (int)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_f64(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
 
 int b200sfm_view_graph_filter_rotations(b200sfm_ctx* ctx, int32_t num_images, const double* cam_from_world_quat_xyzw,
                                         const uint8_t* image_registered, int64_t num_pairs, const int32_t* pair_image1,
                                         const int32_t* pair_image2, const double* pair_quat_xyzw, double max_angle_deg,
                                         uint8_t* pair_valid, int64_t* num_invalidated) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call view_graph_filter_rotations\n");
   dump_f64(f, "max_angle", &max_angle_deg, 1);
   dump_f64(f, "cam_from_world", cam_from_world_quat_xyzw, 4LL * num_images);
@@ -57,7 +39,7 @@ int b200sfm_view_graph_keep_largest_component(b200sfm_ctx* ctx, int32_t num_fram
                                               int64_t num_pairs, const int32_t* pair_image1, const int32_t* pair_image2,
                                               uint8_t* pair_valid, uint8_t* frame_registered, int32_t* num_registered_images) {
   (void)ctx;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call view_graph_keep_largest_component\n");
   dump_i32(f, "image_frame", image_frame, num_images);
   dump_i32(f, "pair_image1", pair_image1, num_pairs);

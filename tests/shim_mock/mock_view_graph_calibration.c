@@ -6,26 +6,8 @@
 #include <stdlib.h>
 
 #include "b200sfm.h"
+#include "mock_dump.h"
 
-static FILE* dump_file(void) {
-  const char* p = getenv("MOCK_DUMP");
-  return fopen(p ? p : "/dev/null", "a");
-}
-static void dump_i32(FILE* f, const char* name, const int32_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", v[i]);
-  fprintf(f, "\n");
-}
-static void dump_u8(FILE* f, const char* name, const uint8_t* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %d", (int)v[i]);
-  fprintf(f, "\n");
-}
-static void dump_f64(FILE* f, const char* name, const double* v, long long n) {
-  fprintf(f, "%s %lld", name, v ? n : 0);
-  for (long long i = 0; v && i < n; ++i) fprintf(f, " %.17g", v[i]);
-  fprintf(f, "\n");
-}
 
 void b200sfm_vgc_default_opts(b200sfm_vgc_opts* o) {
   b200sfm_vgc_opts d = {100, 20, 1e-2, 1e-5, 1e-10, 1e-8, 0.1, 10.0, 2.0, 1000, 0, 1e-12, 0, 0};
@@ -38,7 +20,7 @@ int b200sfm_view_graph_calibrate(b200sfm_ctx* ctx, const b200sfm_vgc_opts* o, in
                                  b200sfm_lm_stats* stats) {
   (void)ctx;
   (void)pair_residual;
-  FILE* f = dump_file();
+  FILE* f = mock_dump_open();
   fprintf(f, "call view_graph_calibrate\n");
   const double opts[9] = {o->max_num_iterations, o->max_num_line_search_step_size_iterations, o->thres_loss_function,
                           o->function_tolerance, o->thres_lower_ratio, o->thres_higher_ratio, o->thres_two_view_error,

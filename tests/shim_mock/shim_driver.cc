@@ -3,6 +3,9 @@
 // recomputed in Python (tests/test_shim_cpu.py) from the same closed-form construction.
 #include <cmath>
 #include <cstdio>
+#include <limits>
+#include <random>
+#include <string>
 
 #include "estimators_shim.h"
 
@@ -13,7 +16,77 @@ static void SetQuat(Quaternion& q, double ax, double ay, double az, double ang) 
   q.c[0] = ax * s; q.c[1] = ay * s; q.c[2] = az * s; q.c[3] = std::cos(ang / 2);
 }
 
-int main() {
+// `shim_driver pinned`: a second world for the rules the first one never reaches.  Frame 5 holds an image that no track
+// observes (a pose block for BA and GP all the same, and not BA's gauge); track 2 observes image 999, which is not in
+// `images`; track 4 is shorter than min_num_view_per_track; cameras 2 and 3 of rig 1 have a cam_from_rig with a NaN
+// translation and are first met as 3 then 2, the reverse of their sorted order.  GP draws its random positions and
+// points, so that the centres of the unknown sensors show where they fall in the sequence of draws.
+static int PinnedWorld() {
+  std::unordered_map<rig_t, Rig> rigs;
+  std::unordered_map<camera_t, Camera> cameras;
+  std::unordered_map<frame_t, Frame> frames;
+  std::unordered_map<image_t, Image> images;
+  std::unordered_map<track_t, Track> tracks;
+  for (camera_t c = 1; c <= 3; ++c) {
+    Camera cam; cam.camera_id = c; cam.model_id = 0; cam.params = {600.0 + c, 320.0, 240.0};
+    cameras[c] = cam;
+  }
+  Rig rig1; rig1.rig_id = 1; rig1.ref_camera_id = 1;
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  for (camera_t c = 2; c <= 3; ++c) {
+    Rigid3d p; SetQuat(p.rotation, 0.3 * c, 1.0, -0.2, 0.1 * c); p.translation = {{nan, nan, nan}};
+    rig1.cam_from_rig[c] = p;
+  }
+  rigs[1] = rig1;
+  for (frame_t id : {5u, 10u, 20u}) {
+    Frame f; f.frame_id = id; f.rig_id = 1;
+    SetQuat(f.rig_from_world.rotation, 1.0, 0.01 * id, 0.3, 0.05 * id);
+    f.rig_from_world.translation = {{0.1 * id, 1.0, -2.0}};
+    frames[id] = f;
+  }
+  const image_t ids[7] = {51, 101, 102, 103, 201, 202, 203};
+  for (int k = 0; k < 7; ++k) {
+    Image im; im.image_id = ids[k]; im.frame_id = ids[k] < 100 ? 5 : (ids[k] / 100) * 10; im.camera_id = ids[k] % 10;
+    im.trivial_frame = false;
+    for (int f = 0; f < 4; ++f) {
+      im.features.push_back({{5.0 * k + f, 7.0 * k - f}});
+      const double b[3] = {0.02 * k - 0.01 * f, 0.01 * f + 0.005 * k, 1.0};
+      const double n = std::sqrt(b[0] * b[0] + b[1] * b[1] + 1.0);
+      im.features_undist.push_back({{b[0] / n, b[1] / n, 1.0 / n}});
+    }
+    images[ids[k]] = im;
+  }
+  for (auto& [id, im] : images) im.frame_ptr = &frames[im.frame_id];
+  const std::vector<std::pair<image_t, feature_t>> obs[3] = {
+      {{203, 0}, {102, 1}, {201, 2}, {999, 0}}, {{101, 0}, {202, 1}}, {{101, 2}, {102, 3}, {103, 0}, {201, 1}}};
+  const track_t tids[3] = {2, 4, 6};
+  for (int t = 0; t < 3; ++t) {
+    Track tr; tr.track_id = tids[t]; tr.xyz = {{1.0 + t, -1.0, 3.0 + 0.5 * t}};
+    tr.observations = obs[t];
+    tracks[tids[t]] = tr;
+  }
+  ViewGraph vg;
+  BundleAdjusterOptions bo;
+  BundleAdjuster ba(bo);
+  if (!ba.Solve(rigs, cameras, frames, images, tracks)) return 1;
+  GlobalPositionerOptions go;   // random positions and points, seed 1
+  GlobalPositioner gp(go);
+  if (!gp.Solve(vg, rigs, cameras, frames, images, tracks)) return 2;
+  for (camera_t c = 2; c <= 3; ++c) {
+    const Rigid3d& p = rigs[1].cam_from_rig[c];
+    std::printf("cfr%u %.17g %.17g %.17g %.17g %.17g %.17g %.17g\n", (unsigned)c, p.rotation.c[0], p.rotation.c[1], p.rotation.c[2],
+                p.rotation.c[3], p.translation[0], p.translation[1], p.translation[2]);
+  }
+  std::mt19937 g(go.seed);   // the sequence GlobalPositioner draws from
+  std::uniform_real_distribution<double> U(-1, 1);
+  std::printf("draws");
+  for (int k = 0; k < 24; ++k) std::printf(" %.17g", U(g));
+  std::printf("\nshim driver ok\n");
+  return 0;
+}
+
+int main(int argc, char** argv) {
+  if (argc > 1 && std::string(argv[1]) == "pinned") return PinnedWorld();
   std::unordered_map<rig_t, Rig> rigs;
   std::unordered_map<camera_t, Camera> cameras;
   std::unordered_map<frame_t, Frame> frames;

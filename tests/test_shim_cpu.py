@@ -19,14 +19,14 @@ def _quat(ax, ay, az, ang):
     return np.concatenate([a / np.linalg.norm(a) * np.sin(ang / 2), [np.cos(ang / 2)]])
 
 
-def _run(tmp_path):
+def _run(tmp_path, *args):
     lib, exe, dump = tmp_path / "libb200sfm_mock.so", tmp_path / "shim_driver", tmp_path / "dump.txt"
     subprocess.run(["/usr/bin/gcc", "-std=c99", "-O1", "-fPIC", "-shared", "-I" + os.path.join(ROOT, "include"), "-o", str(lib),
                     os.path.join(ROOT, "tests", "shim_mock", "mock_b200sfm.c")], check=True, capture_output=True)
     subprocess.run(["g++", "-std=c++17", "-O1", "-I" + os.path.join(ROOT, "glomap_b200", "host"), "-o", str(exe),
                     os.path.join(ROOT, "tests", "shim_mock", "shim_driver.cc"), str(lib), "-Wl,-rpath," + str(tmp_path)],
                    check=True, capture_output=True)
-    r = subprocess.run([str(exe)], env=dict(os.environ, MOCK_DUMP=str(dump)), capture_output=True, text=True)
+    r = subprocess.run([str(exe)] + list(args), env=dict(os.environ, MOCK_DUMP=str(dump)), capture_output=True, text=True)
     assert r.returncode == 0 and "shim driver ok" in r.stdout, (r.returncode, r.stdout, r.stderr)
     calls, cur = [{"_name": "_stdout", "lines": r.stdout.splitlines()}], None
     for line in dump.read_text().splitlines():
@@ -186,6 +186,42 @@ def test_shim_flattening_of_a_rig_world(tmp_path):
     assert np.allclose([float(x) for x in stdout_line(calls, "gpt2")], want_t, atol=1e-15)
     est2 = stdout_line(calls, "est2")
     assert np.allclose([float(x) for x in est2[:4]], [0, 0, np.sin(0.15), np.cos(0.15)], atol=1e-15) and est2[4] == "1"
+
+
+def test_shim_pose_blocks_sensors_and_draws_of_a_partly_observed_world(tmp_path):
+    """The second world of shim_driver.cc: frame 5 is seen by no track, track 2 observes image 999 that is not in `images`,
+    track 4 has two observations (< min_num_view_per_track = 3), and the NaN-translation sensors (rig 1, camera 3) and
+    (rig 1, camera 2) are first met in that order."""
+    calls = _run(tmp_path, "pinned")
+    out = {l.split()[0]: np.array([float(x) for x in l.split()[1:]]) for l in calls[0]["lines"] if l != "shim driver ok"}
+    calls = calls[1:]
+    assert [c["_name"] for c in calls] == ["ba_problem_create_rig", "ba_problem_set_state", "ba_problem_solve",
+                                           "gp_problem_create", "gp_problem_set_rig_terms", "gp_problem_set_rig_unknown",
+                                           "gp_problem_solve"]
+    frame_of = {101: 1, 102: 1, 103: 1, 201: 2, 202: 2, 203: 2}                 # frames 5, 10, 20
+    # the observation of image 999 is dropped, the short track keeps its point but no observation (bundle_adjustment.cc:122-125)
+    obs = [203, 102, 201] + [101, 102, 103, 201]
+    ba = calls[0]
+    assert ba["dims"].tolist() == [3, 3, 7, 3, 3, 1]                            # a pose block for frame 5 too
+    assert ba["pt_obs_begin"].tolist() == [0, 3, 3, 7]
+    assert ba["obs_frame"].tolist() == [frame_of[i] for i in obs]
+    assert ba["obs_sensor"].tolist() == [i % 10 - 1 for i in obs]             # sorted (rig, camera): (1,1) (1,2) (1,3)
+    assert ba["mask"].tolist() == [0, 3, 0]                                    # gauge: the first frame with an observation
+    assert np.isnan(ba["sensor_trans"].reshape(3, 3)[1:]).all()
+    gp, unk = calls[3], calls[5]
+    assert gp["dims"].tolist() == [3, 3, 7] and gp["obs_cam"].tolist() == ba["obs_frame"].tolist()
+    assert gp["pt_obs_begin"].tolist() == [0, 3, 3, 7]
+    # unknown sensors numbered in order of first appearance: camera 3 -> 0, camera 2 -> 1
+    assert unk["dims"].tolist() == [2]
+    assert unk["obs_unknown_sensor"].tolist() == [{1: -1, 2: 1, 3: 0}[i % 10] for i in obs]
+    # one mt19937: 3 frame positions, then the points of tracks 2 and 6 (not the short track 4), then the sensor centres
+    assert np.array_equal(unk["centers"], out["draws"][15:21])
+    # ConvertResults in sorted order with the mock's centre (1 + s, 2, 3) of unknown sensor s: translation = -(R_cr u)
+    for cam, s in ((2, 1), (3, 0)):
+        q = _quat(0.3 * cam, 1.0, -0.2, 0.1 * cam)
+        assert np.abs(out["cfr%d" % cam][:4] - q).max() < 1e-15
+        want = -(G.quat_xyzw_to_rotmat(q[None])[0] @ np.array([1.0 + s, 2.0, 3.0]))
+        assert np.abs(out["cfr%d" % cam][4:] - want).max() < 1e-14
 
 
 def test_shim_typechecks_against_the_glomap_api():
