@@ -221,16 +221,14 @@ __global__ void __launch_bounds__(128) bax_linearize_blocks(BAView v, ExtView ex
       g[i2] += Jb[0][i2] * o.r[0] + Jb[1][i2] * o.r[1];
     }
   }
+  double vals[27];
 #pragma unroll
-  for (int k = 0; k < 21; ++k) {
-    const double s = warp_sum(U[k]);
-    if (lane == k && s != 0.0) atomicAdd(&v.U[(size_t)target * 21 + k], s);
-  }
+  for (int k = 0; k < 21; ++k) vals[k] = U[k];
 #pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    const double s = warp_sum(g[k]);
-    if (lane == 21 + k && s != 0.0) atomicAdd(&v.gc[(size_t)target * 6 + k], s);
-  }
+  for (int k = 0; k < 6; ++k) vals[21 + k] = g[k];
+  const double s = warp_reduce_scatter(vals);   // total k in lane k
+  if (lane < 27 && s != 0.0)
+    atomicAdd(lane < 21 ? &v.U[(size_t)target * 21 + lane] : &v.gc[(size_t)target * 6 + (lane - 21)], s);
 }
 
 // ---- pass A (ELL, one thread per point): s_p = [g_p] + sum_o J_pt^T (J_o x_o), z_p = Vinv s_p ----------------------
@@ -393,25 +391,27 @@ __global__ void __launch_bounds__(128) bax_pass_b(BAView v, ExtView ex, BAViewV2
       }
     }
   }
+  // the frame, intrinsics and sensor sums in one reduce-scatter, one atomic per lane that holds a total
+  constexpr int NKV = WK ? kMaxBlockDof : 0, KV = 6 + NKV + (WS ? 6 : 0), S = warp_rs_stride<KV>();
+  double vals[KV];
 #pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    const double s = warp_sum(ac[k]);
-    if (lane == k && s != 0.0) atomicAdd(&y[(size_t)cam * 6 + k], s);
-  }
-  if (WK) {
+  for (int k = 0; k < 6; ++k) vals[k] = ac[k];
 #pragma unroll
-    for (int j = 0; j < kMaxBlockDof; ++j) {
-      const double s = warp_sum(ak[j]);
-      if (lane == 8 + j && j < iv.mb && s != 0.0) atomicAdd(&y[(size_t)(ex.C + blk) * 6 + j], s);
-    }
-  }
-  if (WS) {
+  for (int j = 0; j < NKV; ++j) vals[6 + j] = ak[j];
 #pragma unroll
-    for (int k = 0; k < 6; ++k) {
-      const double s = warp_sum(as[k]);
-      if (lane == 16 + k && svar && s != 0.0) atomicAdd(&y[(size_t)(ex.C + ex.K + sidx) * 6 + k], s);
-    }
+  for (int k = 0; k < (WS ? 6 : 0); ++k) vals[6 + NKV + k] = as[k];
+  const double s = warp_reduce_scatter(vals);
+  const int k = lane / S;
+  bool live = lane % S == 0 && k < KV && s != 0.0;
+  double* dst = &y[(size_t)cam * 6 + k];
+  if (k >= 6 && k < 6 + NKV) {
+    live = live && k - 6 < iv.mb;
+    dst = &y[(size_t)(ex.C + blk) * 6 + (k - 6)];
+  } else if (k >= 6 + NKV) {
+    live = live && svar;
+    dst = &y[(size_t)(ex.C + ex.K + sidx) * 6 + (k - 6 - NKV)];
   }
+  if (live) atomicAdd(dst, s);
 }
 
 // ---- trial step of the extra blocks -----------------------------------------------------------------------------------

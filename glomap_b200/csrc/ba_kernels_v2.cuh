@@ -116,12 +116,6 @@ __device__ __forceinline__ void cam_frame_jac(const ObsCore& o, const double r[3
   w[1] = s1;
   w[2] = -(p.u * s0 + p.v * s1);
 }
-// x <- R_cr^T x  (the B^T of a known-rig segment)
-__device__ __forceinline__ void rig_to_frame(const double* __restrict__ sr, double x[3]) {
-  const double x0 = x[0], x1 = x[1], x2 = x[2];
-#pragma unroll
-  for (int k = 0; k < 3; ++k) x[k] = sr[k] * x0 + sr[3 + k] * x1 + sr[6 + k] * x2;
-}
 
 // xp[c] = { R^T x_r , R^T x_t, pad, pad }: 64-B rows, so pass A gathers a camera with three 128-bit
 // loads out of a single line  (masked dofs of x are zero already: PCG keeps them at 0)
@@ -288,35 +282,38 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
     }
     Xc = Xn; xy = xyn; pt_nxt = pt_nn;
   }
-  if (NK > 0) {
+  // epilogue: reduce-scatter rounds of <= 32 sums, one atomic per lane that holds a total
+  if (NK > 0) {   // U_kk (upper triangle), g_k, then U_fk row-major: 17 sums for NK = 2
+    constexpr int nU = NKK * (NKK + 1) / 2, KV = nU + NKK + 6 * NKK, S = warp_rs_stride<KV>();
+    double vals[KV];
+#pragma unroll
+    for (int k = 0; k < nU; ++k) vals[k] = Ukk[k];
+#pragma unroll
+    for (int a = 0; a < NKK; ++a) {
+      vals[nU + a] = gk[a];
+#pragma unroll
+      for (int i2 = 0; i2 < 6; ++i2) vals[nU + NKK + i2 * NKK + a] = Ufk[i2][a];
+    }
+    const double s = warp_reduce_scatter(vals);
+    const int k = lane / S;
     const size_t kb = (size_t)(v2.C + blk);
+    double* dst = &v2.Ufk[(size_t)cam * 6 * NKK + (k - nU - NKK)];
+    if (k < nU + NKK) dst = &v.gc[kb * 6 + (k - nU)];
     int ik = 0;
 #pragma unroll
-    for (int a = 0; a < NK; ++a) {
+    for (int a = 0; a < NKK; ++a)
 #pragma unroll
-      for (int c = a; c < NK; ++c) {
-        const double sacc = warp_sum(Ukk[ik++]);
-        if (lane == 0 && sacc != 0.0) atomicAdd(&v.U[kb * 21 + sym_idx(6, a, c)], sacc);
-      }
-      const double sg = warp_sum(gk[a]);
-      if (lane == 0 && sg != 0.0) atomicAdd(&v.gc[kb * 6 + a], sg);
-#pragma unroll
-      for (int i2 = 0; i2 < 6; ++i2) {
-        const double sf = warp_sum(Ufk[i2][a]);
-        if (lane == 0 && sf != 0.0) atomicAdd(&v2.Ufk[((size_t)cam * 6 + i2) * NK + a], sf);
-      }
-    }
+      for (int c = a; c < NKK; ++c, ++ik)
+        if (k == ik) dst = &v.U[kb * 21 + sym_idx(6, a, c)];
+    if (lane % S == 0 && k < KV && s != 0.0) atomicAdd(dst, s);
   }
+  double vals[27];
 #pragma unroll
-  for (int k = 0; k < 21; ++k) {
-    const double s = warp_sum(U[k]);
-    if (lane == k && s != 0.0) atomicAdd(&v.U[(size_t)cam * 21 + k], s);
-  }
+  for (int k = 0; k < 21; ++k) vals[k] = U[k];
 #pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    const double s = warp_sum(g[k]);
-    if (lane == 21 + k && s != 0.0) atomicAdd(&v.gc[(size_t)cam * 6 + k], s);
-  }
+  for (int k = 0; k < 6; ++k) vals[21 + k] = g[k];
+  const double s = warp_reduce_scatter(vals);   // total k in lane k
+  if (lane < 27 && s != 0.0) atomicAdd(lane < 21 ? &v.U[(size_t)cam * 21 + lane] : &v.gc[(size_t)cam * 6 + (lane - 21)], s);
 }
 
 // ---------------------------------------------------------------------------
@@ -326,6 +323,26 @@ __global__ void __launch_bounds__(128, NK > 0 ? 3 : B200_LC_MIN_CTAS) ba2_linear
 // with Q = (rho' iz^2)^2 K Q' K, Q' = L' Vinv L'^T, L' = [I | -(u, v)^T] Rs, K = M^T M.  Per observation the kernel
 // gathers the point (pts4, 32 B) and Vinv_p (48 B).
 // ---------------------------------------------------------------------------
+// The 21 per-segment sums of ba2_schur_diag, in order RR (packed upper 3 x 3), RT (row-major 3 x 3), TT (packed upper
+// 3 x 3), are the upper triangle of the symmetric 6 x 6 M = [RR RT; RT^T TT].  sd_entry: sum k -> its entry (r, c),
+// r <= c (k < 21);  sd_value: entry (p, q) of M -> the sum that holds it.
+__device__ __forceinline__ void sd_entry(int k, int& r, int& c) {
+  if (k >= 6 && k < 15) {
+    r = (k - 6) / 3;
+    c = 3 + (k - 6) % 3;
+  } else {
+    const int o = k < 6 ? 0 : 3, t = k < 6 ? k : k - 15;   // packed 3 x 3: 00 01 02 11 12 22
+    const int i = (t >= 3) + (t >= 5);
+    r = o + i;
+    c = o + t - (i == 0 ? 0 : i == 1 ? 2 : 3);
+  }
+}
+__device__ __forceinline__ int sd_value(int p, int q) {
+  const int i = min(p, q), j = max(p, q);
+  if (j < 3) return sym_idx(3, i, j);
+  if (i >= 3) return 15 + sym_idx(3, i - 3, j - 3);
+  return 6 + 3 * i + (j - 3);
+}
 __global__ void __launch_bounds__(128, B200_SD_MIN_CTAS) ba2_schur_diag(BAView v, BAViewV2 v2, const double* __restrict__ cam_rec,
                                                                         const double* __restrict__ intr_rec, double huber_a) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -426,46 +443,39 @@ __global__ void __launch_bounds__(128, B200_SD_MIN_CTAS) ba2_schur_diag(BAView v
     TT[0] += N[0][0]; TT[1] += N[0][1]; TT[2] += N[0][2]; TT[3] += N[1][1]; TT[4] += N[1][2]; TT[5] += N[2][2];
     Xc = Xn; xy = xyn; va = van; vb = vbn; vc = vcn; pt_nxt = pt_nn;
   }
+  // epilogue: the 21 sums of M (the 6 x 6 block in the sensor-camera frame) reduce-scattered, total k in lane k, and
+  // lane k stores entry (r, c) of S = B^T M B with one atomic
+  double vals[21];
 #pragma unroll
-  for (int k = 0; k < 6; ++k) RR[k] = warp_sum(RR[k]);
+  for (int k = 0; k < 6; ++k) vals[k] = RR[k];
 #pragma unroll
-  for (int k = 0; k < 9; ++k) RT[k] = warp_sum(RT[k]);
+  for (int k = 0; k < 9; ++k) vals[6 + k] = RT[k];
 #pragma unroll
-  for (int k = 0; k < 6; ++k) TT[k] = warp_sum(TT[k]);
-  if (lane == 0) {
-    const int mask = (int)(__double_as_longlong(sg.t4.w) & 0xff);
-    // R = R_cr^T of a known rig (identity for a trivial frame): S = Rb M Rb^T = B^T M B
-    double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-    if (sg.sr) {
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 3; ++c) R[3 * r + c] = sg.sr[3 * c + r];
+  for (int k = 0; k < 6; ++k) vals[15 + k] = TT[k];
+  double s = warp_reduce_scatter(vals);
+  int r, c;
+  sd_entry(lane, r, c);
+  if (sg.sr) {
+    // known rig: S = Rb M Rb^T, Rb = blockdiag(R, R), R = R_cr^T.  Lane k forms S[r][c] from the 3 x 3 block of M
+    // it needs, read from a per-warp stage.  (A trivial frame has B = I and stores M as it is.)
+    __shared__ double stage[4][21];
+    double* st = stage[threadIdx.x >> 5];
+    if (lane < 21) st[lane] = s;
+    __syncwarp();
+    if (lane < 21) {
+      const int rb = r - r % 3, cb = c - c % 3;
+      const double* sr = sg.sr;
+      double t[3];   // t_j = sum_a R[r % 3][a] M[rb + a][cb + j],  R[i][a] = sr[3a + i]
+#pragma unroll
+      for (int j = 0; j < 3; ++j)
+        t[j] = sr[r % 3] * st[sd_value(rb, cb + j)] + sr[3 + r % 3] * st[sd_value(rb + 1, cb + j)] +
+               sr[6 + r % 3] * st[sd_value(rb + 2, cb + j)];
+      s = t[0] * sr[c % 3] + t[1] * sr[3 + c % 3] + t[2] * sr[6 + c % 3];
     }
-    // full 6x6 in the sensor-camera frame, then S = Rb M Rb^T
-    double M[6][6];
-    const double rr[3][3] = {{RR[0], RR[1], RR[2]}, {RR[1], RR[3], RR[4]}, {RR[2], RR[4], RR[5]}};
-    const double tt[3][3] = {{TT[0], TT[1], TT[2]}, {TT[1], TT[3], TT[4]}, {TT[2], TT[4], TT[5]}};
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) {
-        M[r][c] = rr[r][c];
-        M[3 + r][3 + c] = tt[r][c];
-        M[r][3 + c] = RT[3 * r + c];
-        M[3 + c][r] = RT[3 * r + c];
-      }
-    double T[6][6];
-    for (int blk = 0; blk < 2; ++blk)       // T = Rb M
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 6; ++c)
-          T[3 * blk + r][c] = R[3 * r] * M[3 * blk][c] + R[3 * r + 1] * M[3 * blk + 1][c] + R[3 * r + 2] * M[3 * blk + 2][c];
-    int idx = 0;
-    for (int r = 0; r < 6; ++r)
-      for (int c = r; c < 6; ++c, ++idx) {
-        const int cb = c / 3, cc = c % 3;     // S[r][c] = sum_k T[r][3cb+k] R[cc][k]
-        double s = T[r][3 * cb] * R[3 * cc] + T[r][3 * cb + 1] * R[3 * cc + 1] + T[r][3 * cb + 2] * R[3 * cc + 2];
-        const bool rfix = (r < 3) ? (mask & 1) : (mask & 2), cfix = (c < 3) ? (mask & 1) : (mask & 2);
-        if (rfix || cfix) s = 0.0;
-        if (s != 0.0) atomicAdd(&v.Sd[(size_t)cam * 21 + idx], s);
-      }
   }
+  const int mask = (int)(__double_as_longlong(sg.t4.w) & 0xff);
+  const bool rfix = (r < 3) ? (mask & 1) : (mask & 2), cfix = (c < 3) ? (mask & 1) : (mask & 2);
+  if (lane < 21 && !rfix && !cfix && s != 0.0) atomicAdd(&v.Sd[(size_t)cam * 21 + sym_idx(6, r, c)], s);
 }
 
 // ---------------------------------------------------------------------------
@@ -744,26 +754,30 @@ __global__ void __launch_bounds__(128, B200_PB_MIN_CTAS) ba2_pass_b(BAView v, BA
     }
     X = Xn; z = zn; xy = xyn; pt_nxt = pt_nn;
   }
+  // epilogue: one reduce-scatter of the 6 + NK sums, then one atomic per lane that holds a total
+  constexpr int KV = 6 + NK, S = warp_rs_stride<KV>();
+  double vals[KV];
 #pragma unroll
-  for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
-  if (sg.sr) {
-    rig_to_frame(sg.sr, acc);
-    rig_to_frame(sg.sr, acc + 3);
+  for (int k = 0; k < 6; ++k) vals[k] = acc[k];
+#pragma unroll
+  for (int k = 0; k < NK; ++k) vals[6 + k] = accK[k];
+  double s = warp_reduce_scatter(vals);
+  const int k = lane / S;
+  if (sg.sr) {   // B^T of a known rig: dof k mixes the three totals of its half, read from a per-warp stage
+    __shared__ double stage[4][6];
+    double* st = stage[threadIdx.x >> 5];
+    if (lane % S == 0 && k < 6) st[k] = s;
+    __syncwarp();
+    if (k < 6) {
+      const int c = k % 3, h = k - c;
+      s = sg.sr[c] * st[h] + sg.sr[3 + c] * st[h + 1] + sg.sr[6 + c] * st[h + 2];
+    }
   }
   const int mask = (int)(__double_as_longlong(sg.t4.w) & 0xff);
-#pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    const double s = k < 3 ? 2.0 * acc[k] : acc[k];
-    const bool fixed = k < 3 ? (mask & 1) : (mask & 2);
-    if (lane == k && !fixed && s != 0.0) atomicAdd(&y[(size_t)cam * 6 + k], -s);
-  }
-  if (NK > 0) {
-    const size_t kb = (size_t)(v2.C + blk);
-#pragma unroll
-    for (int k = 0; k < NK; ++k) {
-      const double sk = warp_sum(accK[k]);
-      if (lane == 0 && sk != 0.0) atomicAdd(&y[kb * 6 + k], -sk);
-    }
+  const bool fixed = k < 3 ? (mask & 1) : k < 6 ? (mask & 2) : false;
+  if (lane % S == 0 && k < KV && !fixed && s != 0.0) {
+    double* dst = k < 6 ? &y[(size_t)cam * 6 + k] : &y[(size_t)(v2.C + blk) * 6 + (k - 6)];
+    atomicAdd(dst, k < 3 ? -(2.0 * s) : -s);
   }
 }
 

@@ -213,6 +213,43 @@ __device__ __forceinline__ double warp_sum(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// Reduce-scatter of K <= 32 per-lane values: the warp total of value k ends in lanes [k * S, (k + 1) * S), S =
+// warp_rs_stride<K>(), so lane l returns the total of value l / S.  Recursive halving with partners at xor distances
+// 16, 8, 4, 2, 1 (K padded with zeros to a power of two Kp; once one value is left the remaining distances are plain
+// butterfly steps): Kp - 1 + (5 - log2 Kp) exchanges in place of warp_sum's 5 K.  Every partial is the sum of the same
+// two operands warp_sum adds at that distance, so each total is bit-identical to warp_sum's.
+template <int K>
+__host__ __device__ constexpr int warp_rs_stride() {
+  static_assert(K >= 1 && K <= 32, "warp_reduce_scatter takes 1..32 values");
+  return K <= 1 ? 32 : K <= 2 ? 16 : K <= 4 ? 8 : K <= 8 ? 4 : K <= 16 ? 2 : 1;
+}
+// one level of warp_reduce_scatter: M values per lane, partner at xor distance D (a template per level, so that every
+// index into a[] is a constant and the array stays in registers)
+template <int M, int D>
+__device__ __forceinline__ double warp_rs_level(double* a, int lane) {
+  if constexpr (D == 0) {
+    return a[0];
+  } else if constexpr (M > 1) {   // keep the half of the values selected by lane bit D, send the other half
+    const bool hi = lane & D;
+#pragma unroll
+    for (int j = 0; j < M / 2; ++j) {
+      const double keep = hi ? a[M / 2 + j] : a[j], send = hi ? a[j] : a[M / 2 + j];
+      a[j] = keep + __shfl_xor_sync(0xffffffffu, send, D);
+    }
+    return warp_rs_level<M / 2, D / 2>(a, lane);
+  } else {
+    a[0] += __shfl_xor_sync(0xffffffffu, a[0], D);
+    return warp_rs_level<1, D / 2>(a, lane);
+  }
+}
+template <int K>
+__device__ __forceinline__ double warp_reduce_scatter(const double (&v)[K]) {
+  constexpr int Kp = 32 / warp_rs_stride<K>();
+  double a[Kp];
+#pragma unroll
+  for (int k = 0; k < Kp; ++k) a[k] = k < K ? v[k] : 0.0;
+  return warp_rs_level<Kp, 16>(a, threadIdx.x & 31);
+}
 __device__ __forceinline__ double warp_max(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
