@@ -447,11 +447,22 @@ class GlobalPositioner:
             return False
         ctx = self.ctx or default_context()
         lib = ctx.lib
-        # InitializeRandomPositions (.cc:123-165) / random points (.cc:261-264): 100 * U(-1,1)^3
+        # InitializeRandomPositions (.cc:123-165) / random points (.cc:258-264): 100 * U(-1,1)^3.  Given initial
+        # centres and points, only the frames observed by a track of >= min_num_view_per_track views and those tracks
+        # are randomised, as in the reference; the others keep their input (the problem does not contain them)
+        lens = np.diff(np.asarray(prob.pt_obs_begin, np.int64))
+        long_track = lens >= o.min_num_view_per_track
         if o.generate_random_positions and o.optimize_positions or prob.centers is None:
-            prob.centers = 100.0 * self.rng.uniform(-1, 1, size=(prob.C, 3))
+            rand = 100.0 * self.rng.uniform(-1, 1, size=(prob.C, 3))
+            if prob.centers is None:
+                prob.centers = rand
+            else:
+                constrained = np.zeros(prob.C, bool)
+                constrained[np.asarray(prob.obs_cam, np.int64)[np.repeat(long_track, lens)]] = True
+                prob.centers = np.where(constrained[:, None], rand, prob.centers)
         if o.generate_random_points and o.optimize_points or prob.points is None:
-            prob.points = 100.0 * self.rng.uniform(-1, 1, size=(prob.P, 3))
+            rand = 100.0 * self.rng.uniform(-1, 1, size=(prob.P, 3))
+            prob.points = rand if prob.points is None else np.where(long_track[:, None], rand, prob.points)
         if o.generate_scales or prob.scales is None:
             prob.scales = np.ones(prob.N)                               # .cc:298
         ptb, cam = _c(prob.pt_obs_begin, np.int64), _c(prob.obs_cam, np.int32)

@@ -252,6 +252,7 @@ class GlobalMapper:
         self.focal_refined: np.ndarray | None = None      # stage 1: intrinsics blocks whose focal the calibrator set
         self._prior_focal: np.ndarray | None = None       # [K] has_prior_focal_length per intrinsics block, or None
         self._gravity: np.ndarray | None = None           # [C,3] (trivial frames) / [F,3] (rigs) gravity priors, or None
+        self._keep_input_state = False                     # global positioning starts from the input reconstruction
 
     # -- helpers ------------------------------------------------------------------------------------
     def _filters(self, scene: S.Scene, what) -> S.Scene:
@@ -360,7 +361,7 @@ class GlobalMapper:
 
     # -- controllers/global_mapper.cc:19-355 (stages 0, 1, 3, 5, 6) ----------------------------------
     def Solve(self, view_graph: S.ViewGraph, scene: S.Scene, image_pairs=None, features: dict | None = None,
-              camera_prior_focal=None, gravity=None):
+              camera_prior_focal=None, gravity=None, registered=None, keep_input_state: bool = False):
         """Returns (ok, scene): poses / points / intrinsics of ``scene`` estimated from the relative rotations of
         ``view_graph`` and the tracks of ``scene`` (its poses and points are only used when a stage is skipped).
         Given ``image_pairs`` (``track_establishment.ImagePairMatches``) and ``features`` ({image_id: [n,2] pixels}; camera k
@@ -381,12 +382,29 @@ class GlobalMapper:
         ``gravity``: the gravity priors (Frame::gravity_info), one row per camera of a ``Scene`` or per frame of a
         ``RigScene``, NaN rows for none.  With ``opt_ra.use_gravity`` stage 3 runs the gravity-aligned, stratified
         SolveRotationAveraging (see ``_rotation_averaging`` / ``_rotation_averaging_rig``); without it the priors are not
-        read.  As in the reference, use_gravity with a sensor whose cam_from_rig is not known fails the solve."""
+        read.  As in the reference, use_gravity with a sensor whose cam_from_rig is not known fails the solve.
+
+        ``registered``: the input registration, [C] images of a ``Scene`` or [F] frames of a ``RigScene`` (all by
+        default).  Only the registered images or frames reach stages 4-8, through the same compaction as stage 3's
+        component cut (which can only unregister more of them); the others keep their input poses and lose their
+        observations.
+
+        ``keep_input_state``: the poses and points of ``scene`` are a reconstruction (a resumed model), so global
+        positioning starts from them and randomises only what the reference randomises (global_positioning.cc:145-151,
+        258-263): the frames observed by a track of >= min_num_view_per_track views and those tracks, and only with
+        generate_random_* and optimize_* on; the other centres and points keep their input.  Without it every centre
+        and point starts random, as before."""
+        self._keep_input_state = bool(keep_input_state)
         self._prior_focal = None if camera_prior_focal is None else np.asarray(camera_prior_focal, bool).reshape(-1)
         self._gravity = None if gravity is None else np.asarray(gravity, np.float64)
         self.pair_valid_after_calibration = self.focal_refined = None
+        n = scene.F if isinstance(scene, S.RigScene) else scene.C
+        registered = np.ones(n, bool) if registered is None else np.asarray(registered, bool).reshape(-1)
+        if registered.shape != (n,):
+            raise ValueError(f"registered has {registered.shape[0]} flags, the scene has {n} "
+                             f"{'frames' if isinstance(scene, S.RigScene) else 'images'}")
         if isinstance(scene, S.RigScene):
-            return self._solve_rig(view_graph, scene, image_pairs, features)
+            return self._solve_rig(view_graph, scene, image_pairs, features, registered)
         o, thr = self.options_, self.options_.inlier_thresholds
         scene = scene.copy()
         edge_valid = np.ones(view_graph.E, bool)
@@ -397,11 +415,11 @@ class GlobalMapper:
         track_stage = image_pairs is not None and features is not None and not o.skip_track_establishment
         # 3. rotation averaging: first run for filtering, second for the estimate, each followed by FilterRotations and
         # KeepLargestConnectedComponents (:84-116)
-        self.image_registered = reg = np.ones(scene.C, bool)
+        self.image_registered = reg = registered
         if not o.skip_rotation_averaging:
             if not self._rotation_averaging(view_graph, scene, edge_valid):
                 return False, scene
-            reg = self.image_registered
+            self.image_registered = reg = self.image_registered & registered
         # cameras of the registered images: the problem of stages 4-6 (all of them unless stage 3 cut some off)
         cams = np.flatnonzero(reg)
         full = scene
@@ -568,7 +586,8 @@ class GlobalMapper:
         scene.sensor_trans[estimated] = np.nan
         return True
 
-    def _solve_rig(self, view_graph: S.ViewGraph, scene: S.RigScene, image_pairs=None, features: dict | None = None):
+    def _solve_rig(self, view_graph: S.ViewGraph, scene: S.RigScene, image_pairs=None, features: dict | None = None,
+                   registered=None):
         """``Solve`` on rigs (global_mapper.cc:82-353).  Stage 3 (``_rotation_averaging_rig``) registers the images of
         the frames in the view graph's largest component.  Stages 4-6 run on the problem compacted to those frames and
         the sensors their images use: tracks over the registered images, global positioning with the known
@@ -585,10 +604,11 @@ class GlobalMapper:
             if not ok:
                 return False, scene
         track_stage = image_pairs is not None and features is not None and not o.skip_track_establishment
-        self.frame_in_component = np.ones(full.F, bool)
-        self.image_registered = np.ones(full.I, bool)
+        registered = np.ones(full.F, bool) if registered is None else registered
         if not o.skip_rotation_averaging and not self._rotation_averaging_rig(view_graph, full, edge_valid):
             return False, scene
+        self.frame_in_component = registered if o.skip_rotation_averaging else self.frame_in_component & registered
+        self.image_registered = self.frame_in_component[full.image_frame]
         frames = np.flatnonzero(self.frame_in_component)
         part, sensors = compact_frames(full, frames)
         # 4. track establishment (:119-137) over the registered images
@@ -621,16 +641,21 @@ class GlobalMapper:
         if not o.skip_global_positioning:
             bear = PR.undistort_images(scene)
             gp = E.GlobalPositioner(o.opt_gp, self.ctx)
+            # with keep_input_state the input centres and points, kept where the positioner does not randomise
+            centers = points = None
+            if self._keep_input_state:
+                centers = geo.centers_from_pose(geo.quat_xyzw_to_rotmat(scene.quat), scene.trans)
+                points = np.array(scene.points, np.float64, copy=True)
             if isinstance(scene, S.RigScene):
                 # RigBATA with the known cam_from_rig; a NaN translation (rotation averaging's estimate) is unknown
                 unk = np.isnan(scene.sensor_trans).any(axis=1)
                 prob = E.PositioningProblem(scene.quat, scene.pt_obs_begin, scene.obs_frame, bear, obs_sensor=scene.obs_sensor,
                                             sensor_quat=scene.sensor_quat, sensor_trans=scene.sensor_trans,
                                             sensor_calibrated=self._calibrated_flags(scene),
-                                            sensor_unknown=unk if unk.any() else None)
+                                            sensor_unknown=unk if unk.any() else None, centers=centers, points=points)
             else:
                 prob = E.PositioningProblem(scene.quat, scene.pt_obs_begin, scene.obs_cam, bear,
-                                            cam_calibrated=self._calibrated_flags(scene), centers=None, points=None)
+                                            cam_calibrated=self._calibrated_flags(scene), centers=centers, points=points)
             if not gp.Solve(prob):
                 return False, scene
             scene.trans, scene.points = prob.trans, prob.points
