@@ -109,14 +109,18 @@ def make_cameras(C: int, seed: int = 1, jitter_deg: float = 10.0):
     return R, t
 
 
-def make_intrinsics(C: int, model: int, focal: float, image_size: int, num_intrinsics: int):
+def make_intrinsics(C: int, model, focal: float, image_size: int, num_intrinsics: int):
+    """``model``: one camera model for every block, or a sequence of models that block k takes cyclically
+    (model[k % len(model)]), as a database with several kinds of camera has."""
     K = num_intrinsics
-    intr_model = np.full(K, model, dtype=np.int32)
+    models = np.atleast_1d(np.asarray(model, dtype=np.int32))
+    intr_model = models[np.arange(K) % len(models)]
     intr_params = np.zeros((K, INTR_STRIDE))
     half = image_size / 2
     for k in range(K):
         # a few shared blocks: 2 % steps around `focal`; many (per-image) blocks: bounded +-10 % variation
         f = focal * (1 + 0.02 * (k - (K - 1) / 2)) if K <= 8 else focal * (1 + 0.1 * np.sin(1.7 * k))
+        model = int(intr_model[k])
         if model == SIMPLE_PINHOLE:
             intr_params[k, :3] = [f, half, half]
         elif model == PINHOLE:
@@ -349,7 +353,8 @@ def make_rig_scene(F: int, S: int, P: int, mean_track_len: float = 8.0, seed: in
                    shared_intrinsics: bool = False, sensor_rot_deg: float = 20.0, sensor_offset: float = 0.4) -> RigScene:
     """F rigs of S cameras looking at a ball of points.  Sensor 0 is the reference sensor (identity
     cam_from_rig); the others are rotated by up to ``sensor_rot_deg`` and shifted by ``sensor_offset``.
-    Every sensor has its own intrinsics block unless ``shared_intrinsics``.  Small sizes only (tests)."""
+    Every sensor has its own intrinsics block unless ``shared_intrinsics``; ``model`` may list one model per sensor
+    (make_intrinsics).  Small sizes only (tests)."""
     rng = np.random.default_rng([seed, 77])
     Rf, tf = make_cameras(F, seed=seed, jitter_deg=5.0)
     w = rng.normal(size=(S, 3))
