@@ -244,6 +244,13 @@ class GPStepProbeOut(ct.Structure):
               [(f, c_int32) for f in ("pcg_iterations", "schur_jacobi", "CB", "n_us", "pcg_depth")]
 
 
+class GravityProbeOut(ct.Structure):
+    """b200sfm_test_gravity_out (include/b200sfm_testing.h)."""
+    _fields_ = [(f, c_void_p) for f in ("mistake", "angle", "offs", "inc", "total", "mistakes", "error_prone", "ep", "gobs",
+                                        "x", "status", "iterations", "trace")] + \
+              [("trace_cap", c_int32), ("n_error_prone", c_int32)]
+
+
 # name -> (restype, argtypes); the test-only probe of include/b200sfm_testing.h (not part of the drop-in ABI)
 TEST_PROTOTYPES = {
     "b200sfm_test_ba_step": (c_int32, [c_void_p, P(BAOpts), c_double, c_double, P(BAStepProbeOut)]),
@@ -260,6 +267,9 @@ TEST_PROTOTYPES = {
     "b200sfm_test_ra_update": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "b200sfm_test_gp_step": (c_int32, [c_void_p, P(GPOpts), c_double, c_double, c_double, P(GPStepProbeOut)]),
     "b200sfm_test_gp_apply": (c_int32, [c_void_p, c_void_p, c_void_p]),
+    "b200sfm_test_gravity": (c_int32, [c_void_p, P(GravityOpts), c_int32, c_void_p, c_void_p, c_int64] + [c_void_p] * 3
+                             + [P(GravityProbeOut)]),
+    "b200sfm_test_device_helpers": (c_int32, [c_void_p, c_int32, c_int64, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -917,6 +917,51 @@ int b200sfm_gravity_refine(b200sfm_ctx* ctx, const b200sfm_gravity_opts* opts, i
   return rc;
 }
 
+// ---- gravity test probe (include/b200sfm_testing.h) --------------------------------------------------------------
+int b200sfm_test_gravity(b200sfm_ctx* ctx, const b200sfm_gravity_opts* opts, int32_t F, const double* R_align,
+                         const uint8_t* has_gravity, int64_t E, const int32_t* frame1, const int32_t* frame2,
+                         const double* M, b200sfm_test_gravity_out* out) {
+  if (!ctx || !opts || !out || F < 1 || E < 1 || out->trace_cap < 0) return B200SFM_ERR_INVALID_ARG;
+  auto invalid = [&](const char* msg) { ctx->err = msg; return (int)B200SFM_ERR_INVALID_ARG; };
+  if (!R_align || !has_gravity || !frame1 || !frame2 || !M) return invalid("null argument");
+  if (E >= (1LL << 30)) return invalid("2^30 or more pairs");
+  if (ctx->world > 1) return invalid("the test probe is single-rank only");
+  out->n_error_prone = 0;
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    b200::GravityParams prm{opts->max_outlier_ratio,  opts->max_gravity_error,  opts->min_num_neighbors,
+                            opts->max_num_iterations, opts->function_tolerance, opts->gradient_tolerance,
+                            opts->parameter_tolerance};
+    prm.trace_cap = out->trace_cap;
+    std::vector<double> g(3 * (size_t)F);
+    std::vector<unsigned char> status(F);
+    b200::GravityStats st;
+    b200::GravityRunner r(ctx);
+    const int bad = r.run(prm, F, R_align, has_gravity, E, frame1, frame2, M, g.data(), status.data(), st, out);
+    B200_CUDA_OK(cudaGetLastError());
+    if (bad & 1) throw b200::InvalidInput{"frame index outside [0, F)"};
+    if (bad & 2) throw b200::InvalidInput{"a frame with gravity has a non-finite or zero gravity"};
+    if (bad & 4) throw b200::InvalidInput{"a pair has a non-finite M"};
+    return (int)B200SFM_OK;
+  });
+}
+
+int b200sfm_test_device_helpers(b200sfm_ctx* ctx, int32_t op, int64_t n, const double* in, double* out) {
+  if (!ctx || op < 0 || op > 5 || n < 1 || !in || !out) return B200SFM_ERR_INVALID_ARG;
+  return guarded(ctx, [&]() {
+    B200_CUDA_OK(cudaSetDevice(ctx->device));
+    const size_t wi = b200::GRV_HELPER_IN[op], wo = b200::GRV_HELPER_OUT[op];
+    b200::DevBuf<double> din, dout;
+    din.alloc(wi * n);
+    dout.alloc(wo * n);
+    din.upload(in, wi * n, ctx->stream);
+    B200_LAUNCH(ctx, b200::grv_test_helpers, b200::cdiv(n, 128), 128, 0, op, (long long)n, din.p, dout.p);
+    dout.download(out, wo * n, ctx->stream);
+    B200_CUDA_OK(cudaStreamSynchronize(ctx->stream));
+    return (int)B200SFM_OK;
+  });
+}
+
 // ---- track establishment ----------------------------------------------------------
 int b200sfm_tracks_establish(b200sfm_ctx* ctx, int64_t num_matches, const uint64_t* gid1, const uint64_t* gid2, const double* xy1,
                              const double* xy2, double thres_inconsistency, b200sfm_tracks** out, int64_t* num_tracks,

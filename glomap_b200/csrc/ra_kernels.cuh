@@ -775,20 +775,49 @@ __device__ __forceinline__ void quat_outer_acc(double M[10], const double q[4]) 
 #pragma unroll
     for (int b = a; b < 4; ++b) M[idx++] += q[a] * q[b];
 }
-// dominant eigenvector by power iteration from the first quaternion q0 (the averaged rotations are estimates of one
-// rotation: the gap to the second eigenvalue is large); the sign follows q0
-__device__ __forceinline__ void quat_avg_power(const double M[10], const double q0[4], double v[4]) {
-  const double S[4][4] = {{M[0], M[1], M[2], M[3]}, {M[1], M[4], M[5], M[6]}, {M[2], M[5], M[7], M[8]}, {M[3], M[6], M[8], M[9]}};
-  v[0] = q0[0]; v[1] = q0[1]; v[2] = q0[2]; v[3] = q0[3];
-  for (int it = 0; it < 200; ++it) {
-    double u[4];
+// dominant eigenvector by cyclic Jacobi, a fixed 8 sweeps over the 6 planes (quadratic convergence: the off-diagonal
+// mass is at rounding level after 4-5 on a 4x4, so the result is exact to about eps / relative gap however close the
+// second eigenvalue is; a power iteration would need ~ log(eps) / log(lambda2 / lambda1) steps); the sign follows q0
+__device__ __forceinline__ void quat_avg_eig(const double M[10], const double q0[4], double v[4]) {
+  double A[4][4] = {{M[0], M[1], M[2], M[3]}, {M[1], M[4], M[5], M[6]}, {M[2], M[5], M[7], M[8]}, {M[3], M[6], M[8], M[9]}};
+  double V[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
+  for (int sweep = 0; sweep < 8; ++sweep) {
 #pragma unroll
-    for (int a = 0; a < 4; ++a) u[a] = S[a][0] * v[0] + S[a][1] * v[1] + S[a][2] * v[2] + S[a][3] * v[3];
-    const double nn = sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2] + u[3] * u[3]);
-    if (!(nn > 0.0)) break;
+    for (int pq = 0; pq < 6; ++pq) {
+      const int p = pq < 3 ? 0 : (pq < 5 ? 1 : 2), q = pq < 3 ? pq + 1 : (pq < 5 ? pq - 1 : 3);
+      const double apq = A[p][q];
+      if (apq == 0.0) continue;
+      const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
+      const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
+      const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
 #pragma unroll
-    for (int a = 0; a < 4; ++a) v[a] = u[a] / nn;
+      for (int k = 0; k < 4; ++k) {   // A <- J^T A J, J = rotation in (p, q)
+        const double akp = A[k][p], akq = A[k][q];
+        A[k][p] = c * akp - s * akq;
+        A[k][q] = s * akp + c * akq;
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const double apk = A[p][k], aqk = A[q][k];
+        A[p][k] = c * apk - s * aqk;
+        A[q][k] = s * apk + c * aqk;
+      }
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const double vkp = V[k][p], vkq = V[k][q];
+        V[k][p] = c * vkp - s * vkq;
+        V[k][q] = s * vkp + c * vkq;
+      }
+    }
   }
+  int m = 0;
+#pragma unroll
+  for (int k = 1; k < 4; ++k)
+    if (A[k][k] > A[m][m]) m = k;
+  const double dot = V[0][m] * q0[0] + V[1][m] * q0[1] + V[2][m] * q0[2] + V[3][m] * q0[3];
+  const double sg = dot < 0.0 ? -1.0 : 1.0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) v[k] = sg * V[k][m];
 }
 
 // Unknown cam_from_rig rotations (.cc:646-693): for every frame f that holds an image of camera c the updated rotation
@@ -844,7 +873,7 @@ __global__ void __launch_bounds__(128) ra_update_cams(int n_frames, int n_cams, 
   for (int k = 0; k < 10; ++k) M[k] = warp_sum(M[k]);
   if (lane != 0 || cf_begin[c + 1] == cf_begin[c]) return;
   double v[4];
-  quat_avg_power(M, q0, v);
+  quat_avg_eig(M, q0, v);
   double R[9], out[3];
   quat_to_R(v, R);
   R_to_aa(R, out);

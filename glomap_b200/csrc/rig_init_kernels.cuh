@@ -9,14 +9,14 @@
 //      gives the camera segments, samples in ascending image index inside each
 //   4. one warp per camera segment, then one warp per frame segment: the 10 packed entries of sum q q^T accumulated
 //      lane-strided and reduced by warp_sum (a fixed order: repeated calls are bit-identical, no floating-point atomics);
-//      lane 0 takes the dominant eigenvector (quat_avg_power, shared with ra_update_cams)
+//      lane 0 takes the dominant eigenvector (quat_avg_eig, shared with ra_update_cams)
 #pragma once
 #include <cub/cub.cuh>
 
 #include <vector>
 
 #include "context.cuh"
-#include "ra_kernels.cuh"      // quat_outer_acc, quat_avg_power
+#include "ra_kernels.cuh"      // quat_outer_acc, quat_avg_eig
 #include "track_kernels.cuh"   // trk_iota
 
 namespace b200 {
@@ -105,7 +105,7 @@ __device__ __forceinline__ int rig_warp_average(int lo, int hi, int lane, Sample
 #pragma unroll
     for (int a = 0; a < 4; ++a) out[a] = q0[a];
   } else if (n > 1) {
-    quat_avg_power(M, q0, out);
+    quat_avg_eig(M, q0, out);
   }
   if (n > 0 && out[3] < 0.0)   // canonical sign
 #pragma unroll

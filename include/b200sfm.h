@@ -598,10 +598,9 @@ typedef struct {
  *      another image whose camera is known or was averaged in rule 3 contributes conj(q_cam_from_rig) q_i, any other
  *      is skipped.  The reference re-averages inside the image loop; its final value is the average over all samples
  *   5. the average is colmap::AverageQuaternions with unit weights (UPSTREAM-UNVERIFIED restatement): the dominant
- *      eigenvector of sum q q^T over the normalised samples, by the power iteration ra_update_cams uses (200 steps from
- *      the first sample: exact to rounding when the samples estimate one rotation, as they do here; samples spread
- *      over very different rotations converge more slowly); a single sample is returned as it is (normalised).  The
- *      sign is canonical: w >= 0
+ *      eigenvector of sum q q^T over the normalised samples, by the 8-sweep 4x4 Jacobi eigensolver ra_update_cams
+ *      uses (exact to about eps / relative eigengap however wide the samples spread); a single sample is returned as it
+ *      is (normalised).  The sign is canonical: w >= 0 (w < 0 flips, w == 0 does not)
  *   6. sums run in a fixed order without floating-point atomics: repeated calls give bit-identical outputs
  * A null context or array (but image_estimated, cam_samples, frame_samples, stats), n_images < 1 or > INT32_MAX,
  * n_frames < 1, n_cameras < 1, and a frame or camera index out of range give B200SFM_ERR_INVALID_ARG before the device is

@@ -1,5 +1,5 @@
 /* b200sfm_testing.h -- test-only probes into resident bundle-adjustment, rotation-averaging and global-positioning
- * problems.
+ * problems, the gravity refiner's stages and the solvers' small device helpers.
  *
  * NOT part of the drop-in ABI of b200sfm.h: these entry points exist so that the
  * test suite can compare every quantity one Levenberg-Marquardt step forms on the
@@ -194,6 +194,50 @@ int b200sfm_test_gp_step(b200sfm_gp_problem* problem, const b200sfm_gp_opts* opt
 /* y = (S + D) x over the CB*3 block dofs with the linearisation of the last b200sfm_test_gp_step, through the kernels
  * of one PCG iteration.  x, y: host arrays [CB*3]. */
 int b200sfm_test_gp_apply(b200sfm_gp_problem* problem, const double* x, double* y);
+
+/* ---- gravity refinement ----------------------------------------------------------------------------------------
+ * b200sfm_test_gravity runs b200sfm_gravity_refine's stages (gravity_kernels.cuh) on its arguments and downloads what
+ * each stage leaves.  Every array pointer is caller-owned and may be NULL (not downloaded).  E is the number of pairs
+ * given, k indexes the error-prone frames in the order of ep.  Sizes: mistake, angle [E]; offs [F+1]; inc [2E];
+ * total, mistakes, error_prone, ep [F]; gobs [2E*3]; x [F*3], status, iterations [F] (the first n_error_prone rows);
+ * trace [F * (5 + 5 trace_cap)]. */
+typedef struct {
+  uint8_t* mistake;      /* per pair: CalcAngle > max_gravity_error (0 for a pair with a frame without gravity) */
+  double* angle;         /* per pair: the angle in degrees (unwritten for a pair with a frame without gravity) */
+  int32_t* offs;         /* frame f's incidences are inc[offs[f] .. offs[f+1]) */
+  int32_t* inc;          /* the incidences 2 pair + side sorted by frame, ascending inside a frame */
+  int32_t* total;        /* per frame: counted incidences */
+  int32_t* mistakes;     /* per frame: incidences of pairs with a mistake */
+  uint8_t* error_prone;  /* per frame: the error-prone flag */
+  int32_t* ep;           /* the error-prone frames, ascending (n_error_prone entries) */
+  double* gobs;          /* per incidence of an error-prone frame: its observed gravity (NaN: not a term); NaN elsewhere */
+  double* x;             /* per k: the LM result before the consistency check */
+  uint8_t* status;       /* per k: 1 too few terms, 2 accepted, 3 rejected */
+  int32_t* iterations;   /* per k: LM iterations */
+  double* trace;         /* per k, stride 5 + 5 trace_cap: the AverageGravity start x0 [3] (after the sign rule), the
+                            termination (-1 too few terms, 0 gradient tolerance at x0, 1 max iterations, 2 min radius,
+                            3 too many invalid steps, 4 parameter tolerance, 5 function tolerance, 6 gradient tolerance),
+                            the number of recorded iterations, then per iteration up to trace_cap: cost, radius, model
+                            cost change, candidate cost (NaN for an invalid step) and a code (-1 invalid step, 0 rejected,
+                            1 accepted, 2 stopped by the parameter tolerance, 3 stopped by the function tolerance) */
+  int32_t trace_cap;     /* in: iterations recorded per frame */
+  int32_t n_error_prone; /* out */
+} b200sfm_test_gravity_out;
+
+/* Arguments and return codes as b200sfm_gravity_refine (gravity and status are not written).  Single-rank only. */
+int b200sfm_test_gravity(b200sfm_ctx* ctx, const b200sfm_gravity_opts* opts, int32_t F, const double* R_align,
+                         const uint8_t* has_gravity, int64_t E, const int32_t* frame1, const int32_t* frame2,
+                         const double* M, b200sfm_test_gravity_out* out);
+
+/* The solvers' per-warp device helpers on n inputs, one thread each, through the production __device__ functions.
+ * Row widths in -> out per op:
+ *   0 grv_householder      x [3]                      -> v [3], beta
+ *   1 grv_plus             x [3], d [2]               -> x [+] d [3]
+ *   2 grv_plus_jacobian    x [3]                      -> P [3x2 row-major]
+ *   3 grv_principal        A [3x3 row-major, symmetric] -> its principal eigenvector [3]
+ *   4 quat_avg_eig         M [10 packed 4x4 upper triangle], q0 [4] -> the dominant eigenvector [4] (q0 picks its sign)
+ *   5 grv_pair_angle       R [3x3 row-major]          -> RotUpToAngle(R), CalcAngle(R, AngleToRotUp(.)) in degrees */
+int b200sfm_test_device_helpers(b200sfm_ctx* ctx, int32_t op, int64_t n, const double* in, double* out);
 
 #ifdef __cplusplus
 }

@@ -20,8 +20,8 @@ def qangle(a, b):
 
 def conversion_case(F=2000, seed=0):
     """Two rigs (4 and 6 cameras: 10 cameras, 0 and 4 the references), ~30 % of the images unregistered, the images in a
-    random order, image rotations R_cam R_frame with 0.02 rad of noise (the averages are estimates of one rotation, as
-    the power iteration of rule 5 assumes); some cameras known."""
+    random order, image rotations R_cam R_frame with 0.02 rad of noise (the averages are estimates of one rotation;
+    wider spreads are in tests/test_rig_average_gpu.py); some cameras known."""
     rng = np.random.default_rng(seed)
     rig_cams = [np.arange(0, 4), np.arange(4, 10)]
     rig_of = rng.integers(0, 2, F)
